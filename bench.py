@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Benchmark of the per-MD-step energy+force hot path (BASELINE.json metric:
-atom-updates/sec per MD step, SevenNet-0, 1/2/4/8 B200).
+atom-updates/sec per MD step, SevenNet-0, 1/2/4/8 H100).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA engine
     python bench.py --impl reference --gpus N --steps K ...   # the CPU oracle (reference arm)
@@ -12,6 +12,9 @@ One "step" = one energy+force evaluation of one periodic Si cell with a fixed ne
 `value` is timed with inputs resident in HBM (CUDA events, L2 flushed between steps); `e2e` is
 the same metric through the host-buffer C-ABI call with pinned host inputs copied in and
 forces/energy copied out inside the timed region.
+`--dump-outputs DIR` writes what the timed path computed in its last timed step as DIR/<name>.npy
+(float32 / float64); the inputs are fixed by the arguments (seeded positions), so two builds can be
+compared output for output.
 """
 import argparse
 import json
@@ -193,7 +196,7 @@ def oracle_parity(model, species, ei, ev, energy, forces, device):
 
 def gpu_standin(model, cells):
     """torch-CUDA unfused stand-in of the reference GPU path (tools/gpu_standin.py), in a subprocess so
-    that its ~84 GiB of autograd state never coexists with the engine's buffers."""
+    that its autograd state (about 7 MiB per atom) never coexists with the engine's buffers."""
     try:
         r = subprocess.run([sys.executable, os.path.join(ROOT, 'tools', 'gpu_standin.py'), model] + [str(c) for c in cells] + ['--json'],
                            capture_output=True, text=True, timeout=600)
@@ -275,7 +278,7 @@ def run_engine(args):
     meta, arrays = load_weights(os.path.join(ROOT, 'weights', f'{args.model}.npz'))
     tm = {int(k): int(v) for k, v in meta['type_map'].items()}
     cells = CELLS[args.gpus] if args.cells is None else tuple(args.cells)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
 
     sampler = ClockSampler(local_rank)
     if world == 1:
@@ -347,6 +350,13 @@ def run_engine(args):
         runner.set_cuda_graph(True)
     total_ms, launches, clocks = timed_run()
     value = n_atoms * args.steps / (total_ms * 1e-3)
+    if args.dump_outputs:
+        if world == 1:
+            res = eng.results()
+        else:
+            res = gather_distributed(runner, n_atoms, dev)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, res)
 
     # ---- per-kernel breakdown + roofline of the dominant kernel (rank 0) ---------------------------
     # (every rank runs the same steps -- the exchanges are collective; only rank 0 records events)
@@ -427,7 +437,8 @@ def run_engine(args):
             extra = {'l3i5': extra_model(args, 'sevennet_l3i5', cells, flush, dev, local_rank, 'cuda' if args.parity != 'off' else 'off')}
             del flush
             torch.cuda.empty_cache()
-            standin = gpu_standin(args.model, cells)
+            # half the cell: the stand-in's autograd state for the full 12 000-atom cell exceeds 80 GB
+            standin = gpu_standin(args.model, (cells[0], cells[1], max(1, cells[2] // 2)))
     else:
         parity = distributed_parity(runner, eng, meta, arrays, pos, cell, species_all, local_rank)
 
@@ -644,6 +655,12 @@ def run_nacl_d3(args):
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
     total, t_net, t_d3 = (float(v) for v in tt.cpu())
     e_net = float((eng.buffer('energy', dtype='f8')).cpu()[0])
+    if args.dump_outputs:
+        net = eng.results() if world == 1 else gather_distributed(runner, n_atoms, dev)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, {'energy': net['energy'], 'forces': net['forces'], 'atomic_energy': net['atomic_energy'],
+                                             'd3_energy': np.float64(e_d3), 'd3_forces': np.asarray(f_d3),
+                                             'd3_stress': np.asarray(s_d3)})
     parity = None
     if world > 1:      # rank 0: the same system on one GPU, network and D3
         f_all = torch.zeros(n_atoms, 3, dtype=torch.float32, device=dev)
@@ -684,6 +701,40 @@ def run_nacl_d3(args):
         shutdown(runner)
 
 
+def gather_distributed(runner, n_atoms, dev):
+    """the multi-rank result of the last step in global atom order (forces and per-atom energies summed over
+    the ranks that own the atoms); energy as the runner reports it"""
+    import torch
+    import torch.distributed as dist
+    r = runner.results()
+    gids = torch.as_tensor(np.asarray(r['global_ids']), dtype=torch.long, device=dev)
+    f_all = torch.zeros(n_atoms, 3, dtype=torch.float32, device=dev)
+    e_all = torch.zeros(n_atoms, dtype=torch.float32, device=dev)
+    f_all[gids] = r['forces']
+    e_all[gids] = r['atomic_energy']
+    dist.all_reduce(f_all)
+    dist.all_reduce(e_all)
+    return {'energy': r['energy'], 'forces': f_all, 'atomic_energy': e_all}
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy per output (float64 stays float64, everything else float32).  An array that would take
+    the total above 64 MiB is replaced by a fixed sample of its rows (every k-th row), named <name>_every<k>."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, v in arrays.items():
+        a = v.detach().cpu().numpy() if hasattr(v, 'detach') else np.asarray(v)
+        a = np.ascontiguousarray(a, dtype=np.float64 if a.dtype == np.float64 else np.float32)
+        if total + a.nbytes > DUMP_LIMIT and a.ndim > 0 and len(a) > 1:
+            k = -(-a.nbytes // max(DUMP_LIMIT - total, 1))
+            a, name = np.ascontiguousarray(a[::k]), f'{name}_every{k}'
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
+        total += a.nbytes
+
+
 def roofline_from_profile(eng, prof, n_edges, n_dst, steps):
     """Roofline of the dominant kernel from the engine's CUDA-event profile (DESIGN.md section 4).
     The convolution kernels keep x (23 MB) and the radial tables (23 MB/layer) L2-resident, so their
@@ -691,7 +742,7 @@ def roofline_from_profile(eng, prof, n_edges, n_dst, steps):
     mid-feature slice; `achieved`/`frac` (bound = hbm, as the contract asks) are therefore small by
     construction.  What actually bounds them is reported next to it: `l2_gbs` (all algorithmic bytes
     incl. the L2-served table and gather traffic) and `fp32` (flops of the generated code vs the FP32
-    pipe peak 148 SM x 128 lanes x 2 x SM clock)."""
+    pipe peak n_SM x 128 lanes x 2 x SM clock)."""
     if not prof:
         return None, None
     # per profiled STEP, not per call: the split schedule of the multi-GPU runner launches a convolution label twice
@@ -704,13 +755,15 @@ def roofline_from_profile(eng, prof, n_edges, n_dst, steps):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    peak = float(peaks.get('hbm_gbs', 6650.0))
-    src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'fallback 6.65 TB/s (B200_PROFILING.md)'
-    sm_mhz = float(peaks.get('sm_max_mhz', 1965.0))
-    fp32_peak = 148 * 128 * 2 * sm_mhz * 1e6 / 1e12
+    peak = float(peaks.get('hbm_gbs', 3350.0))
+    src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet, 3.35 TB/s'
+    sm_mhz = float(peaks.get('sm_max_mhz', 1980.0))
+    import torch
+    n_sm = torch.cuda.get_device_properties(eng.device).multi_processor_count
+    fp32_peak = n_sm * 128 * 2 * sm_mhz * 1e6 / 1e12
     out = {'kernel': name, 'ms': ms, 'bound': 'fp32', 'achieved': None, 'peak': fp32_peak, 'unit': 'TFLOP/s', 'frac': None,
-           'traffic': None, 'peak_source': f'FP32 FMA pipe: 148 SM x 128 lanes x 2 flop x {sm_mhz:.0f} MHz (theoretical; '
-                                           f'MEASURED_PEAKS.json holds no fp32 entry)'}
+           'peak_source': f'FP32 FMA pipe: {n_sm} SM x 128 lanes x 2 flop x {sm_mhz:.0f} MHz (theoretical; '
+                          f'MEASURED_PEAKS.json holds no fp32 entry)'}
     if name.startswith('conv_'):
         import importlib.util
         spec_ = importlib.util.spec_from_file_location('gen_kernels', os.path.join(ROOT, 'sevenn_b200', 'csrc', 'gen_kernels.py'))
@@ -736,15 +789,8 @@ def roofline_from_profile(eng, prof, n_edges, n_dst, steps):
         out['hbm'] = {'achieved_gbs': hbm / (ms * 1e-3) / 1e9, 'peak_gbs': peak, 'frac': hbm / (ms * 1e-3) / 1e9 / peak,
                       'algorithmic_bytes': int(hbm), 'peak_source': src}
         out['l2_gbs'] = (hbm + l2) / (ms * 1e-3) / 1e9
-        try:   # dram bytes per launch of this kernel kind from the committed ncu --set full capture (mid layers, 12k atoms)
-            tr = json.load(open(os.path.join(ROOT, 'profiles', 'ncu_traffic.json')))
-            if 1 <= t <= 3 and n_dst == 12000:
-                out['traffic'] = tr.get('sevennet_0' if eng.spec.lmax_filter == 2 else 'sevennet_l3i5', {}).get(f'{parts[0]}.l{l1}')
-        except Exception:
-            pass
         out['note'] = ('bound = the FP32 FMA pipe: the channel-wise Clebsch-Gordan product is not GEMM-shaped (DESIGN.md 4); x and the '
-                       'radial tables are L2-resident, so the HBM fraction (`hbm`) is small by construction; traffic = ncu dram '
-                       'bytes per launch from profiles/ncu_traffic.json')
+                       'radial tables are L2-resident, so the HBM fraction (`hbm`) is small by construction')
     return out, breakdown
 
 
@@ -784,6 +830,8 @@ def main():
     ap.add_argument('--no-extras', action='store_true', help='skip the l3i5 / gpu_standin legs of the N = 1 line')
     ap.add_argument('--workload', default='si', choices=['si', 'nacl_d3'],
                     help="'si': the headline benchmark (BASELINE configs[1]/[3]); 'nacl_d3': configs[4], SevenNet-0 + D3 on NaCl")
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/<name>.npy')
     ap.add_argument('--nacl-a', type=float, default=5.64,
                     help='lattice constant of the nacl_d3 workload; 4.0 is the dense variant of SURVEY 8(d).5 (about 65 neighbours per atom)')
     args = ap.parse_args()

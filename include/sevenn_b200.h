@@ -1,4 +1,4 @@
-/* sevenn_b200 -- C ABI of the B200-native SevenNet energy/force engine.
+/* sevenn_b200 -- C ABI of the H100-native SevenNet energy/force engine.
  *
  * Plain pointers and sizes only (no torch / C++ types): this is the boundary a maintainer of
  * the reference binds with ctypes / cgo-style FFI (see INTEGRATION.md).  All device pointers
@@ -92,8 +92,8 @@ enum {
 S7B_API const char* s7b_last_error(void);
 S7B_API int s7b_version(void);
 
-/* Runtime options: "tc_gemm" = 1 (default) runs the node linears on tcgen05 tensor cores (TMA-fed,
- * TMEM accumulators, error-free bf16x3 fixed-point slices: sevenn_b200/csrc/tc_gemm.cuh); 0 selects the
+/* Runtime options: "tc_gemm" = 1 (default) runs the node linears on the tensor cores (TMA-fed
+ * wgmma, register accumulators, error-free bf16x3 fixed-point slices: sevenn_b200/csrc/tc_gemm.cuh); 0 selects the
  * FP32 SIMT GEMM kernel (IEEE fp32 FMA chain).  "tc_swizzle" (default 1): 128B-swizzled TMA tiles.
  * "atomic_virial" = 1: engines created afterwards also fill the buffer "atomic_virial" [n_nodes, 6]
  * (force_output.py:198-214).  "concurrent_conv" (default 1): co-schedule the per-l1 convolution kernels.
@@ -106,7 +106,7 @@ S7B_API int s7b_version(void);
 S7B_API int s7b_set_option(const char* name, int value);
 
 /* C[rows, N] = A[rows, K] * W[K, N] (row-major, device pointers) through the same GEMM kernels the
- * engine uses for its linears; use_tc selects the tcgen05 path (needs K % 32 == 0, N % 16 == 0). */
+ * engine uses for its linears; use_tc selects the tensor-core path (needs K % 32 == 0, N % 16 == 0). */
 S7B_API int s7b_dense_linear(const float* A, const float* W, float* C, int64_t rows, int32_t K, int32_t N,
                              int32_t use_tc, void* stream);
 
@@ -122,7 +122,7 @@ S7B_API int s7b_scatter_add_rows(float* dst, int32_t ld_dst, const int32_t* idx,
 
 /* One block-diagonal irreps linear C_l (+)= A_l W_l, l = 0..n_l-1 (block l: 2l+1 rows per node, component-
  * major rows of K_l / N_l floats at a_off[l] / c_off[l] inside node rows of lda / ldc floats) through the
- * engine's own kernels: use_tc = 1 the tcgen05 path, 0 the FP32 SIMT kernel.  A, C device; W host. */
+ * engine's own kernels: use_tc = 1 the tensor-core path, 0 the FP32 SIMT kernel.  A, C device; W host. */
 S7B_API int s7b_block_linear(const float* A, int32_t lda, int32_t n_nodes, int32_t n_l, const int32_t* a_off,
                              const int32_t* a_K, const float* W_host, float* C, int32_t ldc, const int32_t* c_off,
                              const int32_t* c_N, int32_t accumulate, int32_t use_tc, void* stream);

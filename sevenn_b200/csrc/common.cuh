@@ -1,4 +1,4 @@
-// Shared declarations for the sevenn_b200 CUDA library (sm_100a).
+// Shared declarations for the sevenn_b200 CUDA library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

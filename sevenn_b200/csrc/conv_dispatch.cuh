@@ -12,7 +12,7 @@
 #define S7B_FWD_L0_NV 2   // channel pairs per lane in the l1 = 0 forward kernels (1 was measured 4 % slower)
 #endif
 #ifndef S7B_FWD_ODD_PAIRS
-#define S7B_FWD_ODD_PAIRS 1   // mul = 32 forward kernels: 1 = channel pairs on half warps (two nodes per warp, FFMA2),
+#define S7B_FWD_ODD_PAIRS 1   // mul = 32 forward kernels: 1 = channel pairs on half warps (two nodes per warp, float2 math),
                               // 0 = one channel per lane.  Pairs are 29 % faster since the edge records are fetched
                               // cooperatively (0.099 vs 0.139 ms, 7net-0 l1 = 2); before that the scalar form won.
 #endif

@@ -9,8 +9,8 @@
 //
 // Mapping: a group of LPN lanes (32 = a warp, or 16 = half a warp for 32-channel irreps) owns one
 // destination atom n and one l1 block.  Every lane carries NV channel PAIRS (channels 2*lane,
-// 2*lane+1, then +2*LPN): all per-channel arithmetic is issued as Blackwell packed-FP32
-// instructions (FFMA2/FMUL2, csrc/vec_ops.cuh), every global access of a group is one contiguous
+// 2*lane+1, then +2*LPN): all per-channel arithmetic is written on channel pairs
+// (csrc/vec_ops.cuh), every global access of a group is one contiguous
 // 8-byte-per-lane segment of the component-major ("cm") layout, and the node accumulators of all
 // paths stay in registers over the whole CSR row -- no atomics in the forward.
 // The radial weights w_p,u(r) come either from a cubic-Hermite table indexed by the edge length
@@ -27,7 +27,8 @@ namespace s7b {
 
 constexpr int kConvWarpsPerBlock = 4;
 // Register budget, as the min-resident-CTAs argument of __launch_bounds__ (128-thread CTAs: 4 -> 128
-// registers, 3 -> 168, 1 -> 255).  Measured on B200 (7net-0, 12k atoms, A/B inside one box):
+// registers, 3 -> 168, 1 -> 255).  Chosen by A/B timing on the previous GPU generation (7net-0, 12k atoms;
+// not re-tuned on H100):
 //  * forward: an explicit 1 lets ptxas keep more gathers in flight for the l1 = 0 kernels (96 -> 128
 //    registers, -22 % time); the l1 >= 1 kernels do not change;
 //  * backward: l1 = 0 is fastest at 3 (-6 %), l1 = 1 at 4 (128 registers; 168 or 220 are 3-4 % slower),
@@ -112,7 +113,7 @@ __device__ __forceinline__ void load_Y(const float* __restrict__ Yrow, float (&Y
 
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
-// Per-lane value type: V2 = two adjacent channels (packed FFMA2 math), float = one channel.
+// Per-lane value type: V2 = two adjacent channels (float2 math), float = one channel.
 template <class V> struct VT;
 template <> struct VT<V2> {
   static constexpr int CH = 2;

@@ -325,7 +325,7 @@ static int g_opt_concurrent = 1;   // co-schedule the per-l1 convolution kernels
 static int g_opt_gate_bwd_rows = 0; // gate backward also leaves the row maxima of dg (saves one row-exponent pass per layer; opt-in)
 static int g_opt_stage_graphs = 0;  // s7b_engine_run_stage replays one captured graph per (stage, layer)
 static int g_opt_cuda_graph = 1;   // s7b_engine_compute replays a captured CUDA graph of the step (table mode)
-static int g_opt_tc_gemm = 1;   // 1 (default): node linears on tcgen05 (error-free bf16x3 slices, tc_gemm.cuh); 0: FP32 SIMT
+static int g_opt_tc_gemm = 1;   // 1 (default): node linears on wgmma tensor cores (error-free bf16x3 slices, tc_gemm.cuh); 0: FP32 SIMT
 static long long* g_tc_trace = nullptr;   // device buffer [1 + 4 * cap] when s7b_tc_trace_enable was called (debug)
 static int g_tc_trace_cap = 0;
 static int g_opt_tc_swizzle = 1;   // 128B-swizzled TMA tile for the raw A chunk (0: plain rows; A/B switch)
@@ -361,7 +361,7 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
 
 // ---- tensor-core linear: host side --------------------------------------------------------------
 // Pre-sliced weights of one block-diagonal linear (see tc_gemm.cuh): per block l the three bf16 slices of
-// W^T in the canonical K-major UMMA layout, cut into (n tile, 32-wide K chunk) blobs that one
+// W^T in the canonical K-major core-matrix layout, cut into (n tile, 32-wide K chunk) blobs that one
 // cp.async.bulk moves into a pipeline stage, plus the per-column scales 2^(Eb-7).
 struct TcWeights {
   DevBuf q, fb;
@@ -684,7 +684,7 @@ int s7b_gather_rows(const float* src, int32_t ld_src, const int32_t* idx, int64_
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bool vec = width % 4 == 0 && ld_src % 4 == 0 && (reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(out)) % 16 == 0;
   const size_t total = (size_t)n * (vec ? width / 4 : width);
-  const int grd = (int)std::min<size_t>((total + 255) / 256, 148 * 16);
+  const int grd = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
   if (vec) gather_rows_idx_kernel<true><<<grd, 256, 0, st>>>(src, ld_src, idx, n, width, out);
   else gather_rows_idx_kernel<false><<<grd, 256, 0, st>>>(src, ld_src, idx, n, width, out);
   S7B_LAUNCH_CHECK();
@@ -696,7 +696,7 @@ int s7b_scatter_add_rows(float* dst, int32_t ld_dst, const int32_t* idx, int64_t
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bool vec = width % 4 == 0 && ld_dst % 4 == 0 && (reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(in)) % 16 == 0;
   const size_t total = (size_t)n * (vec ? width / 4 : width);
-  const int grd = (int)std::min<size_t>((total + 255) / 256, 148 * 16);
+  const int grd = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
   if (vec) scatter_add_rows_idx_kernel<true><<<grd, 256, 0, st>>>(dst, ld_dst, idx, n, width, in);
   else scatter_add_rows_idx_kernel<false><<<grd, 256, 0, st>>>(dst, ld_dst, idx, n, width, in);
   S7B_LAUNCH_CHECK();
@@ -1031,7 +1031,7 @@ static ConvArgs make_conv_args(const S7bEngine* e, int t, const float* x) {
 
 static int grid1d(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  if (g > 148 * 64) g = 148 * 64;
+  if (g > 132 * 64) g = 132 * 64;
   if (g < 1) g = 1;
   return (int)g;
 }

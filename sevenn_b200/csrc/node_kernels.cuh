@@ -40,7 +40,7 @@ struct LinArgs {
 constexpr int kGemmBM = 128, kGemmBN = 64, kGemmBK = 16, kGemmThreads = 256;
 constexpr int kGemmPadM = kGemmBM + 4;
 
-// FP32 SIMT GEMM tile: 128 x 64 per CTA, 8 x 4 per thread, inner product issued as packed FFMA2
+// FP32 SIMT GEMM tile: 128 x 64 per CTA, 8 x 4 per thread, inner product on float2 pairs
 // (scalar-broadcast A element x a pair of B columns).  grid = (ceil(max rows / BM), ceil(max N / BN), nblocks)
 __global__ void __launch_bounds__(kGemmThreads, 3) blocklin_gemm_kernel(const LinArgs a) {
   const LinBlock b = a.blk[blockIdx.z];

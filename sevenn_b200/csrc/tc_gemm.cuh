@@ -1,10 +1,10 @@
-// Block-diagonal irreps linear on the 5th-generation tensor cores (tcgen05 + TMEM + TMA, sm_100a):
+// Block-diagonal irreps linear on the Hopper tensor cores (wgmma + TMA + mbarrier, sm_90a):
 //   C[(n,i), :N] (+)= A[(n,i), :K] * W[K, N]        fp32 in / fp32 out
 // Same operand addressing as blocklin_gemm_kernel (node_kernels.cuh); replaces e3nn o3.Linear
 // (sevenn/nn/linear.py:94-100) for self_interaction_1/2 and the self connection, forward and backward.
 //
 // Arithmetic: error-free tensor-core accumulation.  The tensor core adds into its fp32 accumulator with
-// truncation, which biases long fp32/TF32 accumulations (round 1 measured -8.7e-6 eV/atom with 3xTF32).
+// truncation, which biases long fp32/TF32 accumulations.
 // Here every operand is first brought to 24-bit fixed point relative to a power-of-two bound of its row
 // (A: per (node, component) row over all K, from row_exponent_kernel; W: per output column, on the host)
 // and cut into three signed 8-bit slices  q = q0*2^16 + q1*2^8 + q2,  |q_i| <= 128, each exactly
@@ -13,49 +13,51 @@
 //   ACC0 = sum_k A0*B0                 integers < 2^23: EXACT in the fp32 accumulator, nothing to truncate
 //   ACC1 = sum_k A0*B1+A1*B0+A0*B2+A1*B1+A2*B0     2^-8 of ACC0: its truncation is 2^-32 relative
 //   C    = 2^(Ea-7) * 2^(Eb-7) * (ACC0 + ACC1)     one round-to-nearest fp32 add in the epilogue
-// (the dropped A1*B2, A2*B1, A2*B2 are < 2^-24 relative).  Six kind::f16 (bf16) MMAs per K = 16 step cost
-// the same tensor time as 3xTF32.  Emulated bit for bit on the CPU by tests/test_tc_pack_cpu.py.
+// (the dropped A1*B2, A2*B1, A2*B2 are < 2^-24 relative).  Six bf16 MMAs per K = 16 step cost the same
+// tensor time as 3xTF32.  Emulated bit for bit on the CPU by tests/test_tc_pack_cpu.py.
 //
-// Structure (persistent, one CTA per SM, 480 threads = 15 warps, tiles of 128 rows x NT <= 128 columns):
-//   warp 12  TMA producer A: per 32-wide K chunk one cp.async.bulk.tensor (3-D map over (k, component,
-//            node); 128B swizzle) for the raw fp32 A tile into a 5-deep ring (the HBM/L2 round trip of
-//            these loads is what has to be hidden: 80 KB in flight per SM)
-//   warp 14  producer W: one cp.async.bulk per chunk for the pre-sliced, pre-arranged W chunk (3-deep ring)
-//   warps 0-7 transform: two threads per row of a raw chunk (16 of its 32 k each) pull it into registers
-//            (freeing the raw slot), cut it into the three bf16 slices with packed fp32x2 arithmetic and write
-//            them in the canonical K-major UMMA layout (8-row x 16-byte core matrices) into a 2-deep operand ring
-//   warp 13  TMEM allocation + MMA issuer: one thread issues 12 tcgen05.mma per chunk (M = 128, N = NT, K = 16)
-//            into the two TMEM accumulators of the tile; tcgen05.commit frees the operand slots / publishes the tile
-//   warps 8-11 epilogue: tcgen05.ld the accumulators (double-buffered in TMEM, so the next tile's MMAs
-//            overlap), scale, transpose a 32x32 slab through shared memory (STS.128 / LDS.128) and write C with
-//            128-bit row segments, or RED.ADD.F32x4 when accumulating.
+// Structure (persistent, one CTA per SM, 320 threads = 10 warps, tiles of 64 rows x NT <= 128 columns):
+//   warp 8   TMA producer A: per 32-wide K chunk one cp.async.bulk.tensor (3-D map over (k, component,
+//            node); 128B swizzle) for the raw fp32 A tile into an 8-deep ring (the HBM/L2 round trip of
+//            these loads is what has to be hidden: 64 KB in flight per SM)
+//   warp 9   producer W: one cp.async.bulk per chunk for the pre-sliced, pre-arranged W chunk (3-deep ring)
+//   warps 0-3 transform: two threads per row of a raw chunk (16 of its 32 k each) pull it into registers
+//            (freeing the raw slot), cut it into the three bf16 slices and write them in the canonical
+//            K-major no-swizzle core-matrix layout (8-row x 16-byte core matrices) into a 3-deep operand ring
+//   warps 4-7 one warpgroup: issues 12 wgmma.mma_async m64nNTk16 per chunk into its two register
+//            accumulators (64 x NT each, NT/2 + NT/2 registers per thread), releases a chunk's operand slots
+//            once the next chunk's MMAs are in flight (wgmma.wait_group 1), and after the tile's last chunk
+//            scales the accumulators and writes C straight from the fragments (8-byte stores per thread, a
+//            quad of lanes covers one 32-byte row segment), or RED.ADD.F32x2 when accumulating.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "node_kernels.cuh"
 
 namespace s7b {
 
-constexpr int kTcBM = 128;          // rows (nodes) per tile
+constexpr int kTcBM = 64;           // rows (nodes) per tile: the M of one wgmma
 constexpr int kTcKC = 32;           // K elements per pipeline stage
-constexpr int kTcMaxNT = 128;       // columns per tile (two accumulators x two buffers = 512 TMEM columns)
-constexpr int kTcThreads = 480;     // 8 transform + 4 epilogue warps, A producer, MMA issuer, W producer
-constexpr int kTcXformThreads = 256; // two threads per row of a chunk (16 of its 32 k each)
-constexpr int kTcRawBytes = kTcBM * kTcKC * 4;            // 16 KB raw fp32 A chunk
-constexpr int kTcASliceBytes = kTcBM * kTcKC * 2;         // 8 KB per bf16 slice
+constexpr int kTcMaxNT = 128;       // columns per tile
+constexpr int kTcAccRegs = kTcMaxNT / 2;   // fp32 registers per thread of one m64nNTk16 accumulator at NT = 128
+constexpr int kTcThreads = 320;     // 4 transform warps, one MMA + epilogue warpgroup, A producer, W producer
+constexpr int kTcXformThreads = 128; // two threads per row of a chunk (16 of its 32 k each)
+constexpr int kTcMmaWarps = 4;
+constexpr int kTcRawBytes = kTcBM * kTcKC * 4;            // 8 KB raw fp32 A chunk
+constexpr int kTcASliceBytes = kTcBM * kTcKC * 2;         // 4 KB per bf16 slice
 constexpr int kTcBSliceBytes = kTcMaxNT * kTcKC * 2;      // 8 KB per bf16 slice (NT = 128)
 // three decoupled rings: raw A chunks (deep: the HBM/L2 round trip of the TMA loads is what has to be
-// hidden), sliced A operands and sliced W operands (both released by tcgen05.commit)
-constexpr int kTcRawStages = 5, kTcOpsStages = 2, kTcWStages = 3;
+// hidden), sliced A operands and sliced W operands (both released by the MMA warpgroup)
+constexpr int kTcRawStages = 8, kTcOpsStages = 3, kTcWStages = 3;
 constexpr int kTcOpsBytes = 3 * kTcASliceBytes, kTcWBytes = 3 * kTcBSliceBytes;
 constexpr int kTcRawOff = 0;
 constexpr int kTcOpsOff = kTcRawOff + kTcRawStages * kTcRawBytes;
 constexpr int kTcWOff = kTcOpsOff + kTcOpsStages * kTcOpsBytes;
-constexpr int kTcEpiOff = kTcWOff + kTcWStages * kTcWBytes;
-constexpr int kTcEpiBytes = 4 * 32 * 36 * 4;              // per-warp 32 x 36 transpose scratch (16-byte aligned rows)
-constexpr int kTcSmemBytes = kTcEpiOff + kTcEpiBytes + 1024 /*alignment slack*/;
+constexpr int kTcSmemBytes = kTcWOff + kTcWStages * kTcWBytes + 1024 /*alignment slack*/;
 constexpr int kTcZeroRow = -1000;   // row exponent of an all-zero row
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -95,8 +97,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // TMA: 3-D tiled tensor load (coordinates innermost first) completing on an mbarrier
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
@@ -113,44 +113,80 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
       : "memory");
 }
 
-// K-major, no-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1):
-// lbo = byte distance of core matrices adjacent in K, sbo = of 8-row groups adjacent in M/N.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;     // descriptor version for sm_100
-  return d;                   // base_offset = 0, lbo_mode = 0, layout_type = SWIZZLE_NONE
+// wgmma shared-memory matrix descriptor, K-major, no swizzle: the two 8-row x 16-byte core matrices of one
+// K = 16 step lie 128 bytes apart (leading byte offset), 8-row groups 512 bytes apart (stride byte offset).
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32);
 }
-// kind::f16 instruction descriptor: D = F32, A = B = BF16, both K-major, M = 128, N = n.
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTcBM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across a wgmma fence / wait
+__device__ __forceinline__ void acc_fence(float (&d)[kTcAccRegs]) {
+#pragma unroll
+  for (int i = 0; i < kTcAccRegs; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64, N] (+)= A[64, 16] * B[16, N]: bf16 operands from shared memory, fp32 accumulator fragment in the
+// first N/2 registers of d; scale_d = 0 overwrites D.
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_bf16<16>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <> __device__ __forceinline__ void wgmma_bf16<48>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<80>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<96>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<112>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %58, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[kTcAccRegs], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
 
 // 2^e as a float (e clamped to the normal range)
 __device__ __forceinline__ float exp2i(int e) {
@@ -254,18 +290,34 @@ __device__ __forceinline__ float4 lds128(uint32_t saddr) {
 __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
-__device__ __forceinline__ float lds32(uint32_t saddr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void sts32(uint32_t saddr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory");
-}
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<const uint32_t*>(&v);
+}
+
+// The 12 MMAs of one 32-wide K chunk (tile width N): ACC0 += A0*B0, ACC1 += the five cross terms
+template <int N>
+__device__ __forceinline__ void tc_mma_chunk(float (&acc0)[kTcAccRegs], float (&acc1)[kTcAccRegs], uint32_t sa,
+                                             uint32_t sb, bool first) {
+  constexpr uint32_t b_slice = (uint32_t)N * kTcKC * 2u;
+#pragma unroll
+  for (int j = 0; j < kTcKC / 16; ++j) {
+    const uint32_t ko = (uint32_t)j * 256u;     // two 16-byte K core matrices per MMA
+    const uint64_t dA0 = gmma_desc(sa + ko);
+    const uint64_t dA1 = gmma_desc(sa + kTcASliceBytes + ko);
+    const uint64_t dA2 = gmma_desc(sa + 2 * kTcASliceBytes + ko);
+    const uint64_t dB0 = gmma_desc(sb + ko);
+    const uint64_t dB1 = gmma_desc(sb + b_slice + ko);
+    const uint64_t dB2 = gmma_desc(sb + 2 * b_slice + ko);
+    const uint32_t acc = (!first || j > 0) ? 1u : 0u;
+    wgmma_bf16<N>(acc0, dA0, dB0, acc);
+    wgmma_bf16<N>(acc1, dA0, dB1, acc);
+    wgmma_bf16<N>(acc1, dA1, dB0, 1u);
+    wgmma_bf16<N>(acc1, dA0, dB2, 1u);
+    wgmma_bf16<N>(acc1, dA1, dB1, 1u);
+    wgmma_bf16<N>(acc1, dA2, dB0, 1u);
+  }
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1)
@@ -275,27 +327,17 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
   __shared__ uint64_t bar_raw_full[kTcRawStages], bar_raw_empty[kTcRawStages];
   __shared__ uint64_t bar_ops_full[kTcOpsStages], bar_ops_empty[kTcOpsStages];
   __shared__ uint64_t bar_w_full[kTcWStages], bar_w_empty[kTcWStages];
-  __shared__ uint64_t bar_acc_full[2], bar_acc_empty[2];
-  __shared__ uint32_t tmem_base_sh;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int trace_n = 0;
 
-  if (warp == 13) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_sh)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (tid == 0) {
     for (int s = 0; s < kTcRawStages; ++s) { mbar_init(&bar_raw_full[s], 1); mbar_init(&bar_raw_empty[s], kTcXformThreads); }
-    for (int s = 0; s < kTcOpsStages; ++s) { mbar_init(&bar_ops_full[s], kTcXformThreads); mbar_init(&bar_ops_empty[s], 1); }
-    for (int s = 0; s < kTcWStages; ++s) { mbar_init(&bar_w_full[s], 1); mbar_init(&bar_w_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&bar_acc_full[b], 1); mbar_init(&bar_acc_empty[b], 128); }
+    for (int s = 0; s < kTcOpsStages; ++s) { mbar_init(&bar_ops_full[s], kTcXformThreads); mbar_init(&bar_ops_empty[s], kTcMmaWarps); }
+    for (int s = 0; s < kTcWStages; ++s) { mbar_init(&bar_w_full[s], 1); mbar_init(&bar_w_empty[s], kTcMmaWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_sh;
 
   // tile t -> (block, node tile, component, n tile)
   auto decode = [&](int t, int& b, int& mt, int& ci, int& nt) {
@@ -322,7 +364,7 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
     return v;
   };
 
-  if (warp == 12) {
+  if (warp == 8) {
     // =================== TMA producer, A: raw fp32 chunks ===================
     if (lane == 0) {
       uint32_t it = 0;
@@ -339,7 +381,7 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         }
       }
     }
-  } else if (warp == 14) {
+  } else if (warp == 9) {
     // =================== TMA producer, W: pre-sliced bf16 chunks ===================
     if (lane == 0) {
       uint32_t it = 0;
@@ -359,10 +401,10 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         }
       }
     }
-  } else if (warp < 8) {
+  } else if (warp < 4) {
     // =================== transform: raw fp32 row -> three bf16 slices ===================
-    // thread (r, h): row r of the tile, k = 16 h .. 16 h + 15 of the chunk; packed fp32 arithmetic (FFMA2 ...)
-    const int r = tid & 127, h = tid >> 7;
+    // thread (r, h): row r of the tile, k = 16 h .. 16 h + 15 of the chunk
+    const int r = tid & (kTcBM - 1), h = tid / kTcBM;
     const uint32_t swz = a.swizzle ? (uint32_t)(r & 7) : 0u;
     const uint32_t row_off = (uint32_t)((r & 7) * 16 + (r >> 3) * 512);
     const V2 M2 = splat2(12582912.0f), nM2 = splat2(-12582912.0f);     // 1.5 * 2^23: (x + M) - M = rint(x)
@@ -417,139 +459,101 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         mbar_arrive(&bar_ops_full[o]);
       }
     }
-  } else if (warp == 13) {
-    // =================== MMA issuer ===================
-    if (lane == 0) {
-      uint32_t it = 0, tile_it = 0;
-      for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++tile_it) {
-        int b, mt, ci, nt;
-        decode(t, b, mt, ci, nt);
-        const TcLinBlock& B = a.blk[b];
-        const int n_kc = B.K / kTcKC;
-        const int buf = tile_it & 1;
-        mbar_wait(&bar_acc_empty[buf], ((tile_it >> 1) & 1) ^ 1);
-        TC_TRACE(2, 2, tile_it);   // MMA: accumulator buffer free
-        tc_fence_after();
-        const uint32_t acc0 = tmem_base + (uint32_t)(buf * 2 * kTcMaxNT)   /* fixed halves: tiles of different NT alternate */;
-        const uint32_t acc1 = acc0 + (uint32_t)B.NT;
-        const uint32_t idesc = umma_idesc_bf16(B.NT);
-        const uint32_t b_slice = (uint32_t)B.NT * kTcKC * 2u;
-        for (int kc = 0; kc < n_kc; ++kc, ++it) {
-          const int o = it % kTcOpsStages, w = it % kTcWStages;
-          mbar_wait(&bar_w_full[w], (it / kTcWStages) & 1);
-          TC_TRACE(2, 0, it);      // MMA: weights landed
-          mbar_wait(&bar_ops_full[o], (it / kTcOpsStages) & 1);
-          TC_TRACE(2, 1, it);      // MMA: operands ready, issuing
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + kTcOpsOff + (size_t)o * kTcOpsBytes);
-          const uint32_t sb = smem_u32(smem + kTcWOff + (size_t)w * kTcWBytes);
+  } else if (warp < 8) {
+    // =================== MMA + epilogue warpgroup (warps 4..7) ===================
+    // accumulator fragment of m64nNk16: warp w of the group holds rows 16 w + lane/4 (registers 4j, 4j+1) and
+    // 16 w + lane/4 + 8 (4j+2, 4j+3), columns 8 j + 2 (lane % 4) + {0, 1}
+    const int mw = warp - 4, q4 = lane & 3;
+    const int rl = 16 * mw + (lane >> 2);
+    float acc0[kTcAccRegs], acc1[kTcAccRegs];
 #pragma unroll
-          for (int j = 0; j < kTcKC / 16; ++j) {
-            const uint32_t ko = (uint32_t)j * 256u;     // two 16-byte K core matrices per MMA
-            const uint64_t dA0 = umma_desc(sa + ko, 128, 512);
-            const uint64_t dA1 = umma_desc(sa + kTcASliceBytes + ko, 128, 512);
-            const uint64_t dA2 = umma_desc(sa + 2 * kTcASliceBytes + ko, 128, 512);
-            const uint64_t dB0 = umma_desc(sb + ko, 128, 512);
-            const uint64_t dB1 = umma_desc(sb + b_slice + ko, 128, 512);
-            const uint64_t dB2 = umma_desc(sb + 2 * b_slice + ko, 128, 512);
-            const uint32_t acc = (kc > 0 || j > 0) ? 1u : 0u;
-            umma_bf16(acc0, dA0, dB0, idesc, acc);
-            umma_bf16(acc1, dA0, dB1, idesc, acc);
-            umma_bf16(acc1, dA1, dB0, idesc, 1u);
-            umma_bf16(acc1, dA0, dB2, idesc, 1u);
-            umma_bf16(acc1, dA1, dB1, idesc, 1u);
-            umma_bf16(acc1, dA2, dB0, idesc, 1u);
-          }
-          umma_commit(&bar_ops_empty[o]);                // both operand slots reusable once these MMAs have read them
-          umma_commit(&bar_w_empty[w]);
-        }
-        umma_commit(&bar_acc_full[buf]);                 // accumulators of this tile complete
-      }
-    }
-  } else if (warp < 12) {
-    // =================== epilogue (warps 8..11 <-> TMEM lanes 32*(warp-8) ..) ===================
-    const int ew = warp - 8;
-    const uint32_t scratch = smem_u32(smem + kTcEpiOff) + (uint32_t)ew * (32 * 36 * 4);
-    uint32_t tile_it = 0;
-    int Ea_next = row_exp(blockIdx.x, ew * 32 + lane);
+    for (int i = 0; i < kTcAccRegs; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+    uint32_t it = 0, tile_it = 0;
+    int Ea_next0 = row_exp(blockIdx.x, rl), Ea_next1 = row_exp(blockIdx.x, rl + 8);
     for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++tile_it) {
       int b, mt, ci, nt;
       decode(t, b, mt, ci, nt);
       const TcLinBlock& B = a.blk[b];
-      const int buf = tile_it & 1;
-      const int Ea = Ea_next;                                       // the row this thread holds in TMEM
-      Ea_next = row_exp(t + gridDim.x, ew * 32 + lane);
-      const float fa = (Ea == kTcZeroRow) ? 0.0f : exp2i(Ea - 7);
-      const uint32_t lane_base = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(buf * 2 * kTcMaxNT)   /* fixed halves: tiles of different NT alternate */;
-      const int col0 = nt * B.NT;
-      const int node0 = mt * kTcBM + ew * 32;
-      const int n_rows = min(32, a.n_nodes - node0);                // rows of this warp that exist (<= 0: none)
-      float* cbase = a.C + (size_t)node0 * a.ldc + B.c_off + (size_t)ci * B.c_cs + col0;
-      // One 32 x 32 slab at a time: thread = TMEM lane = row writes its 32 values as 8 x STS.128 into a
-      // [32][36]-float scratch (conflict-free), then the warp re-reads it as 4 rows x 8 column quads per pass
-      // (LDS.128) and writes C with 128-bit stores -- or 128-bit fire-and-forget reductions for C += ...:
-      // every element of C belongs to exactly one tile, so the single add per element is deterministic and no
-      // load latency enters the epilogue.
-      const int rsub = lane >> 3, g4 = (lane & 7) * 4;
-      bool waited = false;
-      for (int c = 0; c < B.NT; c += 32) {
-        const int cc = c + g4;                                      // first of this lane's 4 columns
-        const bool col_ok = cc < B.NT && col0 + cc < B.N;           // quads are all-in or all-out (NT, N multiples of 4)
-        float4 fb4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (col_ok) fb4 = __ldg(reinterpret_cast<const float4*>(B.fb + col0 + cc));
-        if (!waited) {
-          mbar_wait(&bar_acc_full[buf], (tile_it >> 1) & 1);
-          if (tid == 256) TC_TRACE(3, 0, tile_it);    // epilogue: accumulators complete
-          tc_fence_after();
-          waited = true;
-        }
-        {
-          uint32_t v0[32], v1[32];
-          tmem_ld32(lane_base + (uint32_t)c, v0);
-          tmem_ld32(lane_base + (uint32_t)(B.NT + c), v1);
-          tmem_ld_wait();
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float x0 = (__uint_as_float(v0[4 * q + 0]) + __uint_as_float(v1[4 * q + 0])) * fa;
-            const float x1 = (__uint_as_float(v0[4 * q + 1]) + __uint_as_float(v1[4 * q + 1])) * fa;
-            const float x2 = (__uint_as_float(v0[4 * q + 2]) + __uint_as_float(v1[4 * q + 2])) * fa;
-            const float x3 = (__uint_as_float(v0[4 * q + 3]) + __uint_as_float(v1[4 * q + 3])) * fa;
-            sts128(scratch + (uint32_t)(lane * 36 + 4 * q) * 4, __float_as_uint(x0), __float_as_uint(x1), __float_as_uint(x2), __float_as_uint(x3));
+      const int n_kc = B.K / kTcKC;
+      const int Ea0 = Ea_next0, Ea1 = Ea_next1;
+      Ea_next0 = row_exp(t + gridDim.x, rl);
+      Ea_next1 = row_exp(t + gridDim.x, rl + 8);
+      // the K loop of one tile, instantiated per tile width: the wgmma shape is an immediate, and a width
+      // dispatch inside the loop would make ptxas serialize the MMAs
+      auto mainloop = [&](auto width) {
+        constexpr int N = decltype(width)::value;
+        int prev_o = 0, prev_w = 0;
+        for (int kc = 0; kc < n_kc; ++kc, ++it) {
+          const int o = it % kTcOpsStages, w = it % kTcWStages;
+          mbar_wait(&bar_w_full[w], (it / kTcWStages) & 1);
+          if (tid == 128) TC_TRACE(2, 0, it);      // MMA: weights landed
+          mbar_wait(&bar_ops_full[o], (it / kTcOpsStages) & 1);
+          if (tid == 128) TC_TRACE(2, 1, it);      // MMA: operands ready, issuing
+          __syncwarp();
+          const uint32_t sa = smem_u32(smem + kTcOpsOff + (size_t)o * kTcOpsBytes);
+          const uint32_t sb = smem_u32(smem + kTcWOff + (size_t)w * kTcWBytes);
+          acc_fence(acc0);
+          acc_fence(acc1);
+          wgmma_fence();
+          tc_mma_chunk<N>(acc0, acc1, sa, sb, kc == 0);
+          wgmma_commit();
+          acc_fence(acc0);
+          acc_fence(acc1);
+          wgmma_wait<1>();             // the previous chunk's MMAs have read their operands: release its slots
+          if (kc > 0) {
+            __syncwarp();
+            if (lane == 0) { mbar_arrive(&bar_ops_empty[prev_o]); mbar_arrive(&bar_w_empty[prev_w]); }
           }
+          prev_o = o;
+          prev_w = w;
         }
+        wgmma_wait<0>();
+        acc_fence(acc0);
+        acc_fence(acc1);
         __syncwarp();
-        if (col_ok) {
-          float4 vals[8];
-#pragma unroll
-          for (int p8 = 0; p8 < 8; ++p8) vals[p8] = lds128(scratch + (uint32_t)((p8 * 4 + rsub) * 36 + g4) * 4);
-          float* p = cbase + (size_t)rsub * a.ldc + cc;
-          const size_t step = (size_t)4 * a.ldc;
-          if (a.accumulate) {
-#pragma unroll
-            for (int p8 = 0; p8 < 8; ++p8) {
-              if (p8 * 4 + rsub < n_rows)
-                atomicAdd(reinterpret_cast<float4*>(p + p8 * step), make_float4(vals[p8].x * fb4.x, vals[p8].y * fb4.y, vals[p8].z * fb4.z, vals[p8].w * fb4.w));
-            }
-          } else {
-#pragma unroll
-            for (int p8 = 0; p8 < 8; ++p8) {
-              if (p8 * 4 + rsub < n_rows)
-                *reinterpret_cast<float4*>(p + p8 * step) = make_float4(vals[p8].x * fb4.x, vals[p8].y * fb4.y, vals[p8].z * fb4.z, vals[p8].w * fb4.w);
-            }
-          }
-        }
-        __syncwarp();
+        if (lane == 0) { mbar_arrive(&bar_ops_empty[prev_o]); mbar_arrive(&bar_w_empty[prev_w]); }
+      };
+      switch (B.NT) {
+        case 16: mainloop(std::integral_constant<int, 16>()); break;
+        case 32: mainloop(std::integral_constant<int, 32>()); break;
+        case 48: mainloop(std::integral_constant<int, 48>()); break;
+        case 64: mainloop(std::integral_constant<int, 64>()); break;
+        case 80: mainloop(std::integral_constant<int, 80>()); break;
+        case 96: mainloop(std::integral_constant<int, 96>()); break;
+        case 112: mainloop(std::integral_constant<int, 112>()); break;
+        default: mainloop(std::integral_constant<int, 128>()); break;
       }
-      tc_fence_before();
-      if (tid == 256) TC_TRACE(3, 1, tile_it);        // epilogue: tile written
-      mbar_arrive(&bar_acc_empty[buf]);
-    }
-  }
+      if (tid == 160) TC_TRACE(3, 0, tile_it);    // epilogue: accumulators complete
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 13) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+      // every element of C belongs to exactly one tile, so the single add per element is deterministic
+      const float fa0 = (Ea0 == kTcZeroRow) ? 0.0f : exp2i(Ea0 - 7);
+      const float fa1 = (Ea1 == kTcZeroRow) ? 0.0f : exp2i(Ea1 - 7);
+      const int col0 = nt * B.NT;
+      const int node0 = mt * kTcBM + rl;
+      const bool ok0 = node0 < a.n_nodes, ok1 = node0 + 8 < a.n_nodes;
+      float* c0 = a.C + (size_t)node0 * a.ldc + B.c_off + (size_t)ci * B.c_cs + col0 + 2 * q4;
+      float* c1 = c0 + (size_t)8 * a.ldc;
+      const float* fbp = B.fb + col0 + 2 * q4;
+#pragma unroll
+      for (int j = 0; j < kTcMaxNT / 8; ++j) {
+        // column pairs are all-in or all-out (N a multiple of 4)
+        if (8 * j < B.NT && col0 + 8 * j + 2 * q4 < B.N) {
+          const float2 fb2 = __ldg(reinterpret_cast<const float2*>(fbp + 8 * j));
+          const float2 v0 = make_float2((acc0[4 * j + 0] + acc1[4 * j + 0]) * fa0 * fb2.x,
+                                        (acc0[4 * j + 1] + acc1[4 * j + 1]) * fa0 * fb2.y);
+          const float2 v1 = make_float2((acc0[4 * j + 2] + acc1[4 * j + 2]) * fa1 * fb2.x,
+                                        (acc0[4 * j + 3] + acc1[4 * j + 3]) * fa1 * fb2.y);
+          if (a.accumulate) {
+            if (ok0) atomicAdd(reinterpret_cast<float2*>(c0 + 8 * j), v0);
+            if (ok1) atomicAdd(reinterpret_cast<float2*>(c1 + 8 * j), v1);
+          } else {
+            if (ok0) *reinterpret_cast<float2*>(c0 + 8 * j) = v0;
+            if (ok1) *reinterpret_cast<float2*>(c1 + 8 * j) = v1;
+          }
+        }
+      }
+      if (tid == 160) TC_TRACE(3, 1, tile_it);        // epilogue: tile written
+    }
   }
 }
 

@@ -1,9 +1,9 @@
 // Scalar / packed-pair arithmetic used by the generated tensor-product code.
 //
-// On sm_100a `V2` is float2 and the operations map to Blackwell's packed FP32 instructions
-// (FFMA2 / FMUL2 / FADD2: two fp32 lanes per issue slot, with scalar-broadcast and immediate
-// operand forms), so one thread processes two channels per instruction.  When the same headers are
-// compiled by a host compiler (tests/cpu_harness) the pair type is emulated with plain floats.
+// `V2` is float2: one thread processes two channels.  sm_90a has no packed FP32 instructions, so each
+// operation is two scalar round-to-nearest FFMA / FMUL / FADD (bit-identical to a packed form).  When
+// the same headers are compiled by a host compiler (tests/cpu_harness) the pair type is emulated with
+// plain floats.
 #pragma once
 #include <cmath>
 
@@ -14,11 +14,11 @@
 #endif
 namespace s7b {
 using V2 = float2;
-S7B_HD V2 fma_(V2 a, V2 b, V2 c) { return __ffma2_rn(a, b, c); }
-S7B_HD V2 fma_(float s, V2 b, V2 c) { return __ffma2_rn(make_float2(s, s), b, c); }
-S7B_HD V2 mul_(V2 a, V2 b) { return __fmul2_rn(a, b); }
-S7B_HD V2 mul_(V2 a, float s) { return __fmul2_rn(a, make_float2(s, s)); }
-S7B_HD V2 add_(V2 a, V2 b) { return __fadd2_rn(a, b); }
+S7B_HD V2 fma_(V2 a, V2 b, V2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+S7B_HD V2 fma_(float s, V2 b, V2 c) { return make_float2(__fmaf_rn(s, b.x, c.x), __fmaf_rn(s, b.y, c.y)); }
+S7B_HD V2 mul_(V2 a, V2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+S7B_HD V2 mul_(V2 a, float s) { return make_float2(__fmul_rn(a.x, s), __fmul_rn(a.y, s)); }
+S7B_HD V2 add_(V2 a, V2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 S7B_HD V2 splat2(float s) { return make_float2(s, s); }
 }  // namespace s7b
 #else

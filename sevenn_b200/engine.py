@@ -1,4 +1,4 @@
-"""Python host side of the B200 engine: parameter repacking and a thin ctypes binding to the
+"""Python host side of the engine: parameter repacking and a thin ctypes binding to the
 C-ABI library ``sevenn_b200/lib/libsevenn_b200.so`` (``include/sevenn_b200.h``).
 
 PyTorch is used only for device memory, streams and (in ``parallel.py``) NCCL; every kernel on
@@ -205,7 +205,7 @@ def pack_table_pairs(tab: np.ndarray):
     ``table23`` [knots, W/2, 4] fp16 {a2e, a2o, a3e, a3o}  (|a2| <~ 1e-3, |a3| <~ 1e-5 of |w| <~ 60:
     half precision leaves w unchanged at the fp32 rounding level and dw/dr at ~2e-7 relative rms),
     returned bit-cast to float32 [knots, W/2, 2] for upload.  Every coefficient arrives as an aligned
-    (even, odd) pair for the packed FFMA2 Horner evaluation; 24 instead of 32 bytes per pair."""
+    (even, odd) pair for the channel-pair Horner evaluation; 24 instead of 32 bytes per pair."""
     K, W, _ = tab.shape
     pairs = tab.reshape(K, W // 2, 2, 4)                       # [k, pair, parity, coef]
     t01 = np.ascontiguousarray(pairs[..., 0:2].transpose(0, 1, 3, 2).reshape(K, W // 2, 4), dtype=np.float32)
@@ -311,7 +311,7 @@ class B200Engine:
                  knots: Optional[int] = None, device: Optional[int] = None, atomic_virial: bool = False):
         import torch
         if not torch.cuda.is_available():
-            raise RuntimeError('sevenn_b200 needs a CUDA device (sm_100a); there is no CPU path')
+            raise RuntimeError('sevenn_b200 needs a CUDA device (sm_90a); there is no CPU path')
         self.torch = torch
         self.lib = load_library()
         self.spec = build_spec(meta)

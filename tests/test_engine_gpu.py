@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box with `pytest -m gpu`): the CUDA engine, called through
+"""GPU parity tests (run on an H100 with `pytest -m gpu`): the CUDA engine, called through
 the C ABI (ctypes), against (a) the reference's own golden vectors and (b) the fp64 CPU oracle
 on the same inputs.
 

@@ -78,7 +78,7 @@ def test_tp_kind_forward_backward(lib, l1, lf, lo):
 
 @pytest.mark.parametrize('l1,lf,lo', KINDS)
 def test_tp_kind_packed_pair_instantiation_matches_scalar(lib, l1, lf, lo):
-    """The V2 (two channels per lane, FFMA2 on the GPU) instantiation of the generated code equals
+    """The V2 (two channels per lane on the GPU) instantiation of the generated code equals
     two independent scalar evaluations."""
     npath, nacc = ctypes.c_int(), ctypes.c_int()
     t = [np.zeros(16, np.int32) for _ in range(3)]

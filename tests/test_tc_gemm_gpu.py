@@ -1,4 +1,4 @@
-"""tcgen05 linear kernel (TMA-fed, error-free bf16x3 slices; csrc/tc_gemm.cuh) vs fp64 numpy, and vs the FP32
+"""Tensor-core (wgmma) linear kernel (TMA-fed, error-free bf16x3 slices; csrc/tc_gemm.cuh) vs fp64 numpy, and vs the FP32
 SIMT kernel inside the engine."""
 import ctypes
 

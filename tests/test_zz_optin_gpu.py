@@ -112,7 +112,10 @@ def test_gate_bwd_rows_option_matches_default(model):
         out = {k: v.cpu().numpy().copy() for k, v in eng.results().items()}
     finally:
         set_option('gate_bwd_rows', 0)
-    assert out['energy'][0] == ref['energy'][0]
+    # the per-atom energies are written without atomics: bit-identical.  The total is one fp64 atomicAdd per block
+    # of the readout, so its last bit follows the order in which the blocks finish
+    assert np.array_equal(out['atomic_energy'], ref['atomic_energy'])
+    assert abs(out['energy'][0] - ref['energy'][0]) <= 1e-14 * abs(ref['energy'][0])
     assert np.allclose(out['forces'], ref['forces'], atol=2e-6)
     assert np.allclose(out['virial'], ref['virial'], atol=1e-5)
 

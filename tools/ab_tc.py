@@ -1,4 +1,4 @@
-"""A/B of the node-linear kernels (tcgen05 3xTF32 vs FP32 SIMT): accuracy vs the fp64 oracle on the
+"""A/B of the node-linear kernels (tensor-core bf16x3 vs FP32 SIMT): accuracy vs the fp64 oracle on the
 64-atom cell and step time on the 12 000-atom cell."""
 import os, sys, time
 import numpy as np, torch

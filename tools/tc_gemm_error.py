@@ -1,5 +1,6 @@
-import sys, ctypes, numpy as np, torch
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tests')
+import os, sys, ctypes, numpy as np, torch
+ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..')
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 from sevenn_b200.engine import check, load_library
 lib = load_library()
 def run(rows, K, N, use_tc, scale=1.0, seed=0):
