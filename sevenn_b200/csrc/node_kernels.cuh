@@ -232,10 +232,15 @@ __device__ __forceinline__ void row_max_update(unsigned int* smax, int r, float 
   if (r >= 0 && lane == __ffs(peers) - 1) smax[r] = max(smax[r], mm);
   __syncwarp();
 }
+// Row exponent of the tensor-core linear from max |a| over a row: E with max |a| < 2^E.  zero_row for an all-zero
+// row, a row of subnormals (flushed: the row gives exactly 0) and a row holding Inf or NaN (the transform's a * 0
+// turns it into a NaN row).  E >= -104 keeps the slice scale 2^(23 - E) a normal float; a row whose maximum lies
+// below 2^-104 keeps 23 - (-104 - log2 max|a|) bits.  The same rule is restated in tc_gemm.cuh (row_exponent_kernel
+// and blocklin_tc_kernel's row_exp), each function self-contained (tests/test_simt_emulation.py compiles them one by one).
 __device__ __forceinline__ void row_exponents_store(const unsigned int* smax, int* E, int rows, int lane, int zero_row) {
   if (lane < rows) {
     const int ex = (int)(smax[lane] >> 23);
-    E[lane] = (ex < 30 || ex == 255) ? zero_row : ex - 126;
+    E[lane] = (ex == 0 || ex == 255) ? zero_row : max(ex - 126, -104);     // |a| < 2^(ex-126)
   }
 }
 

@@ -195,7 +195,7 @@ __device__ __forceinline__ float exp2i(int e) {
 }
 
 // ---- row exponents --------------------------------------------------------------------------------
-// E(n, i) with max_k |A[(n,i), k]| < 2^E  (kTcZeroRow for an all-zero / denormal row); one warp per row.
+// E(n, i) with max_k |A[(n,i), k]| < 2^E  (rule: row_exponents_store, node_kernels.cuh); one warp per row.
 struct RowExpArgs {
   const float* A;
   int* E;                 // [n_nodes, rows_per_node]
@@ -237,8 +237,8 @@ __global__ void row_exponent_kernel(const RowExpArgs a) {
   }
   __syncwarp();
   if (n < a.n_nodes && lane < a.rows_per_node) {
-    const int ex = (int)(smax[wib][lane] >> 23);
-    a.E[(size_t)n * a.rows_per_node + lane] = (ex < 30 || ex == 255) ? kTcZeroRow : ex - 126;     // |a| < 2^(ex-126)
+    const int ex = (int)(smax[wib][lane] >> 23);          // the rule of row_exponents_store (node_kernels.cuh)
+    a.E[(size_t)n * a.rows_per_node + lane] = (ex == 0 || ex == 255) ? kTcZeroRow : max(ex - 126, -104);
   }
 }
 
@@ -358,8 +358,8 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
     if (node >= a.n_nodes) return kTcZeroRow;
     int v = __ldg(a.E + (size_t)node * a.rows_per_node + a.blk[b].row_base + ci);
     if (a.e_bits) {
-      const int ex = v >> 23;
-      v = (ex < 30 || ex == 255) ? kTcZeroRow : ex - 126;          // |a| < 2^(ex-126)
+      const int ex = v >> 23;                              // the rule of row_exponents_store (node_kernels.cuh)
+      v = (ex == 0 || ex == 255) ? kTcZeroRow : max(ex - 126, -104);
     }
     return v;
   };

@@ -95,3 +95,12 @@ def test_positions_entry_matches_graph_entry(eng):
     assert abs(energy - float(r['energy'].cpu()[0])) < 2e-5      # different neighbour order within rows
     assert np.allclose(forces, r['forces'].cpu().numpy(), atol=2e-5)
     assert np.allclose(virial, r['virial'].cpu().numpy(), atol=2e-4)
+
+
+@pytest.mark.parametrize('fixture', ['dense', 'tiny_cell', 'many_species'])
+def test_nl_adversarial_fixtures(eng, fixture):
+    """rows of 85 neighbours (dense), a triclinic cell smaller than the cutoff (tiny_cell: many images of a
+    pair and of the atom itself), every species (tests/graphs.py)"""
+    import graphs
+    g = graphs.fixture(fixture, 'sevennet_0')
+    _check(eng, g.positions, g.cell, g.pbc, g.numbers)

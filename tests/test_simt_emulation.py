@@ -139,13 +139,19 @@ def gate_numpy(d, g, dh=None):
     return h, dg
 
 
+def exponents_of_bits(bits, zero_row=-1000):
+    """the row exponent the kernels derive from the bits of max |row| (node_kernels.cuh row_exponents_store):
+    zero_row for zero / subnormal / Inf / NaN maxima, otherwise max |row| < 2^E with E clamped at -104"""
+    ex = (np.asarray(bits, dtype=np.uint32) >> 23).astype(np.int64)
+    return np.where((ex == 0) | (ex == 255), zero_row, np.maximum(ex - 126, -104))
+
+
 def row_exponents(a, blocks, zero_row=-1000):
     """E[n, row_base + i] with max |row| < 2^E from the fp32 bit pattern, as tc_gemm.cuh defines it"""
     out = []
     for dcomp, K, off in blocks:
         rows = np.abs(a[:, off:off + dcomp * K]).reshape(len(a), dcomp, K).max(2).astype(np.float32)
-        ex = (rows.view(np.uint32) >> 23).astype(np.int64)
-        out.append(np.where((ex < 30) | (ex == 255), zero_row, ex - 126))
+        out.append(exponents_of_bits(rows.view(np.uint32), zero_row))
     return np.concatenate(out, 1)
 
 
@@ -193,6 +199,31 @@ def test_gate_kernels_and_row_exponents_on_the_emulator(emu, muls):
     emu.emu_gate_bwd_rows(ctypes.byref(d), _ptr(g), _ptr(dh), _ptr(dg1), n, _ptr(bits), rows, min(grid, 7))   # 7 blocks: grid-stride loop
     assert np.allclose(dg0, ref_dg, rtol=2e-5, atol=1e-6)
     assert np.array_equal(dg0, dg1)
-    ex = (bits >> 23).astype(np.int64)
-    E_bits = np.where((ex < 30) | (ex == 255), -1000, ex - 126)      # what tc_gemm.cuh's row_exp() makes of the bits
+    E_bits = exponents_of_bits(bits)                                 # what tc_gemm.cuh's row_exp() makes of the bits
     assert np.array_equal(E_bits, row_exponents(dg1, blocks_g))
+
+
+def test_row_exponents_across_the_float_range(emu):
+    """row_exponent_kernel on rows whose maxima span the whole fp32 range: zero and subnormal rows (and Inf / NaN)
+    are flagged, rows down to 2^-104 get their exact exponent, smaller normal rows the clamped -104 (never the
+    zero flag: the tensor-core linear must not drop them)."""
+    K = 8
+    exps = list(range(-125, 128, 3)) + [-104, -105, -97, -96, 127]       # 0.75 * 2^e is normal for e >= -125
+    A = [np.full(K, 0.75 * 2.0 ** e) for e in exps]
+    A += [np.zeros(K), np.full(K, 2.0 ** -140), np.full(K, 2.0 ** -149)]
+    inf_row, nan_row = np.ones(K), np.ones(K)
+    inf_row[3], nan_row[5] = np.inf, np.nan
+    A += [inf_row, nan_row]
+    A = np.ascontiguousarray(np.array(A, dtype=np.float32))
+    n = len(A)
+    a = RowExpArgs()
+    E = np.full((n, 1), 7777, np.int32)
+    a.A, a.E, a.lda, a.n_nodes, a.rows_per_node, a.nblocks = A.ctypes.data, E.ctypes.data, K, n, 1, 1
+    a.d[0], a.K[0], a.a_off[0], a.row_base[0] = 1, K, 0, 0
+    emu.emu_row_exponent(ctypes.byref(a))
+    E = E[:, 0]
+    m = len(exps)
+    want = np.array([max(e, -104) for e in exps])                  # 0.75 * 2^e < 2^e
+    assert np.array_equal(E[:m], want)
+    assert (E[m:] == -1000).all()
+    assert np.array_equal(E, exponents_of_bits(np.abs(A).max(1).view(np.uint32)))

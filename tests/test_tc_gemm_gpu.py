@@ -138,6 +138,8 @@ def _block_linear(n_nodes, a_K, c_N, accumulate, use_tc, seed=0, pad=(32, 64)):
     (515, [256, 64, 32, 32], [256, 480, 416, 352]),  # ... its transpose: column tiles of 128 / 96 / 32 / 32
     (300, [128, 64, 32, 32], [256, 64, 32, 32]),     # lmax 3 self connection
     (20000, [224, 384, 352], [224, 64, 32]),         # many tiles per CTA: the operand rings wrap many times
+    (333, [64, 32, 96], [48, 96, 40]),               # tile widths 48 / 96 / 48 (padded)
+    (129, [96, 64, 32], [180, 72, 100]),             # 2 x 96 (padded), 80 (padded), 112 (padded)
 ])
 def test_block_linear_tc_matches_fp64(n_nodes, a_K, c_N, accumulate):
     got, ref = _block_linear(n_nodes, a_K, c_N, accumulate, 1, seed=n_nodes)
@@ -153,3 +155,116 @@ def test_block_linear_tc_matches_fp64(n_nodes, a_K, c_N, accumulate):
         pad_cols[off:off + (2 * l + 1) * c_N[l]] = False
         off += (2 * l + 1) * c_N[l]
     assert np.array_equal(got[:, pad_cols], ref[:, pad_cols].astype(np.float32))
+
+
+# ---- every tile width of tc_pick_nt (16 .. 128 in steps of 16) and the padded last tile -------------------
+# N -> NT: 40 -> 48, 48 -> 48, 72 -> 80, 80 -> 80, 96 -> 96, 100 -> 112, 136 -> 2 x 80, 160 -> 2 x 80,
+# 180 -> 2 x 96, 260 -> 3 x 96 (asserted on the CPU in test_tc_pack_cpu.py)
+TILE_WIDTH_N = [40, 48, 72, 80, 96, 100, 136, 160, 180, 260]
+
+
+@pytest.mark.parametrize('N', TILE_WIDTH_N)
+def test_tc_dense_linear_every_tile_width(N):
+    got, ref = _dense(300, 96, N, 1, seed=N)
+    assert np.isfinite(got).all()
+    assert np.abs(got - ref).max() < 4e-7 * np.sqrt(96) * max(1.0, np.abs(ref).max())
+    simt, _ = _dense(300, 96, N, 0, seed=N)
+    assert np.abs(got - simt).max() < 6e-7 * np.sqrt(96) * max(1.0, np.abs(ref).max())
+
+
+def _linear_rows(A, W, C0, n_nodes, accumulate, use_tc):
+    """C[:n_nodes] (+)= A[:n_nodes] W through s7b_block_linear with one l = 0 block; A, C0 may hold more rows
+    (and C0 more columns) than the product touches.  Returns the whole C."""
+    import torch
+    from sevenn_b200.engine import check, load_library
+    lib = load_library()
+    K, N = W.shape
+    a_t, c_t = torch.tensor(A, device='cuda'), torch.tensor(C0, device='cuda')
+    i32 = lambda v: np.ascontiguousarray(v, dtype=np.int32)
+    ao, ak, co, cn = i32([0]), i32([K]), i32([0]), i32([N])
+    Wc = np.ascontiguousarray(W, dtype=np.float32)
+    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    check(lib.s7b_block_linear(a_t.data_ptr(), A.shape[1], n_nodes, 1, ao.ctypes.data, ak.ctypes.data, Wc.ctypes.data,
+                               c_t.data_ptr(), C0.shape[1], co.ctypes.data, cn.ctypes.data, int(accumulate), int(use_tc), st))
+    torch.cuda.synchronize()
+    return c_t.cpu().numpy()
+
+
+@pytest.mark.parametrize('accumulate', [False, True])
+@pytest.mark.parametrize('rows', [1, 63, 65, 129])
+@pytest.mark.parametrize('N', TILE_WIDTH_N)
+def test_tc_row_counts_leave_pads_and_extra_rows_alone(N, rows, accumulate):
+    rng = np.random.RandomState(N + rows)
+    K, extra, pad = 64, 70, 12
+    A = rng.normal(size=(rows + extra, K)).astype(np.float32)
+    W = (rng.normal(size=(K, N)) / np.sqrt(K)).astype(np.float32)
+    C0 = rng.normal(size=(rows + extra, N + pad)).astype(np.float32)
+    ref = (C0[:rows, :N].astype(np.float64) if accumulate else 0.0) + A[:rows].astype(np.float64) @ W.astype(np.float64)
+    for use_tc in (1, 0):
+        got = _linear_rows(A, W, C0, rows, accumulate, use_tc)
+        assert np.abs(got[:rows, :N] - ref).max() < 1e-6 * np.sqrt(K) * max(1.0, np.abs(ref).max()), use_tc
+        assert np.array_equal(got[:, N:], C0[:, N:])            # pad columns
+        assert np.array_equal(got[rows:], C0[rows:])            # rows beyond n_nodes
+
+
+def _wide_range_operands(K=64, N=80, seed=0):
+    """A: rows at scales 2^-100 .. 2^100, all-zero rows, rows of subnormals, rows with one dominant element;
+    W: an all-zero column and columns at scales 2^-20 .. 2^20"""
+    rng = np.random.RandomState(seed)
+    scales = [2.0 ** e for e in range(-100, 101, 5)]
+    A = [rng.normal(size=K) * s for s in scales]
+    A += [np.zeros(K), np.zeros(K)]
+    A += [rng.normal(size=K) * 2.0 ** -140, np.full(K, 2.0 ** -149)]         # subnormal rows
+    for e in (-60, 0, 60):
+        r = rng.normal(size=K) * 2.0 ** (e - 30)
+        r[rng.randint(K)] = 2.0 ** e                                          # one dominant element
+        A.append(r)
+    A = np.array(A, dtype=np.float32)
+    A = A[rng.permutation(len(A))]
+    W = rng.normal(size=(K, N)) / np.sqrt(K) * 2.0 ** rng.randint(-20, 21, size=N)[None, :]
+    W[:, 3] = 0.0
+    W[:, 7] *= 2.0 ** rng.randint(-30, 31, size=K)                            # one column with a wide spread
+    return A, W.astype(np.float32)
+
+
+@pytest.mark.parametrize('use_tc', [1, 0])
+def test_tc_linear_error_contract_over_the_exponent_range(use_tc):
+    """|C - A W| <= c 2^-24 max_k|A_ik| max_k|W_kj| sqrt(K) for every element; all-zero rows and rows of
+    subnormals give exactly 0 on the tensor-core path (the SIMT path multiplies them out within the same bound)."""
+    A, W = _wide_range_operands()
+    K, N = W.shape
+    rows = len(A)
+    got = _linear_rows(A, W, np.zeros((rows, N), np.float32), rows, False, use_tc).astype(np.float64)
+    ref = A.astype(np.float64) @ W.astype(np.float64)
+    amax = np.abs(A.astype(np.float64)).max(1)
+    bound = 8 * 2.0 ** -24 * np.outer(amax, np.abs(W.astype(np.float64)).max(0)) * np.sqrt(K)
+    assert np.isfinite(got).all()
+    tiny = amax < 2.0 ** -126
+    assert (amax[tiny] > 0).any() and (amax == 0).sum() == 2
+    if use_tc:
+        assert (got[tiny] == 0.0).all()
+    else:
+        assert (np.abs(got - ref)[tiny] <= bound[tiny] + K * 2.0 ** -149).all()     # K subnormal roundings
+    err = np.abs(got - ref)[~tiny]
+    assert (err <= bound[~tiny]).all(), (err / np.maximum(bound[~tiny], 1e-300)).max()
+    assert (got[:, 3] == 0.0).all()
+
+
+@pytest.mark.parametrize('use_tc', [1, 0])
+def test_tc_linear_non_finite_rows_stay_non_finite(use_tc):
+    """A row holding NaN or Inf gives a row of non-finite outputs on both paths (never finite numbers); the
+    other rows are unaffected."""
+    rng = np.random.RandomState(5)
+    rows, K, N = 130, 64, 96
+    A = rng.normal(size=(rows, K)).astype(np.float32)
+    W = (rng.normal(size=(K, N)) / np.sqrt(K)).astype(np.float32)
+    W[:, 5] = 0.0
+    bad = {3: np.nan, 64: np.inf, 65: -np.inf, 129: np.nan}
+    for i, v in bad.items():
+        A[i, rng.randint(K)] = v
+    got = _linear_rows(A, W, np.zeros((rows, N), np.float32), rows, False, use_tc)
+    for i in bad:
+        assert not np.isfinite(got[i]).any(), (i, got[i][np.isfinite(got[i])][:4])
+    good = np.setdiff1d(np.arange(rows), list(bad))
+    ref = A[good].astype(np.float64) @ W.astype(np.float64)
+    assert np.abs(got[good] - ref).max() < 1e-6 * np.sqrt(K) * np.abs(ref).max()

@@ -60,6 +60,21 @@ def _slice_rows(A):
     return q0.astype(np.float64), q1.astype(np.float64) / 256.0, q2.astype(np.float64) / 65536.0, fa
 
 
+# tile width tc_pick_nt chooses for N (fewest tiles of <= 128 columns, width a multiple of 16): the GPU tests of
+# tests/test_tc_gemm_gpu.py use these N to reach the wgmma widths 48 / 80 / 96 / 112 and a padded last tile
+TILE_WIDTHS = {40: 48, 48: 48, 72: 80, 80: 80, 96: 96, 100: 112, 136: 80, 160: 80, 180: 96, 260: 96,
+               16: 16, 32: 32, 64: 64, 128: 128, 224: 112, 384: 128}
+
+
+@pytest.mark.parametrize('N,NT', sorted(TILE_WIDTHS.items()))
+def test_pack_picks_the_tile_width(N, NT):
+    W = np.random.RandomState(N).normal(size=(64, N)).astype(np.float32)
+    sl, fb, nt = _pack(W)
+    assert nt == NT
+    rec = (sl.sum(0) * fb[:, None]).T
+    assert np.all(np.abs(rec - W) <= np.abs(W).max(axis=0) * 2.0 ** -23)
+
+
 @pytest.mark.parametrize('K,N', [(32, 32), (224, 224), (384, 64), (352, 32), (64, 384), (256, 256), (32, 352), (64, 480), (32, 416), (32, 24)])
 def test_pack_reproduces_weights(K, N):
     rng = np.random.RandomState(K + N)

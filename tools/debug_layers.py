@@ -1,87 +1,34 @@
 """GPU debugging aid: run the engine stage by stage and report, for every intermediate the
-oracle also produces, the max abs difference (engine vs fp64 oracle).  Usage:
+oracle also produces, the max abs difference (engine vs fp64 oracle), and the first stage that
+diverges.  Usage:
     python tools/debug_layers.py [sevennet_0|sevennet_l3i5] [table|mlp] [ncell]
 """
 import os
 import sys
 
 import numpy as np
-import torch
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..')
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
-from oracle.oracle import Oracle  # noqa: E402
-from sevenn_b200 import engine as eng  # noqa: E402
-from sevenn_b200.checkpoint import load_weights  # noqa: E402
+from helpers import first_divergence, format_stage_errors, model_weights, oracle, species_of, stage_errors  # noqa: E402
+from sevenn_b200.engine import B200Engine  # noqa: E402
 from sevenn_b200.neighbors import build_graph, diamond_si  # noqa: E402
-from sevenn_b200.spec import perm_cm_from_mulir  # noqa: E402
 
 
 def main():
     name = sys.argv[1] if len(sys.argv) > 1 else 'sevennet_0'
     radial = sys.argv[2] if len(sys.argv) > 2 else 'table'
     nc = int(sys.argv[3]) if len(sys.argv) > 3 else 2
-    meta, arrays = load_weights(os.path.join(ROOT, 'weights', f'{name}.npz'))
+    meta, arrays = model_weights(name)
     pos, cell, z = diamond_si(nc, nc, nc)
     ei, ev = build_graph(pos, cell, True, 5.0)
-    tm = {int(k): int(v) for k, v in meta['type_map'].items()}
-    species = np.array([tm[int(a)] for a in z])
-    o = Oracle(meta, arrays, dtype=torch.float64)
-    ref = o.forward(species, ei, ev, volume=abs(np.linalg.det(cell)), keep=True)
-    sv = ref['saved']
-    e = eng.B200Engine(meta, arrays, radial=radial)
-    e.set_graph(species, ei, ev)
-    spec = e.spec
-    N, E = len(species), ei.shape[1]
-
-    def report(tag, got, want):
-        got = got.detach().cpu().double().numpy()
-        want = np.asarray(want, dtype=np.float64)
-        d = np.abs(got - want).max() if got.size else 0.0
-        print(f'{tag:28s} max|diff| {d:.3e}   ref scale {np.abs(want).max() if want.size else 0:.3e}', flush=True)
-
-    e.run_stage(eng.STAGE_FWD_BEGIN)
-    torch.cuda.synchronize()
-    Y = e.buffer('edge_Y', shape=(E, -1) if False else None).reshape(E, -1)
-    report('edge sh (Y1..)', Y[:, :spec.n_sh - 1], sv['edge_attr'].numpy()[:, 1:])
-    report('edge length', e.buffer('edge_len'), np.linalg.norm(ev, axis=1))
-    if radial == 'mlp':
-        report('edge embedding', e.buffer('edge_emb').reshape(E, -1), sv['edge_embedding'].numpy())
-    for L in spec.layers:
-        t = L.t
-        px = perm_cm_from_mulir(list(L.x_muls))
-        report(f'{t}.x (after si1)', e.buffer('x', t).reshape(N, -1), sv[f'{t}.x_si1'].numpy()[:, px])
-        e.run_stage(eng.STAGE_FWD_LAYER, t)
-        torch.cuda.synchronize()
-        if radial == 'mlp':
-            report(f'{t}.radial weight', e.buffer('weight', t).reshape(E, -1), sv[f'{t}.weight'].numpy())
-        pm = L.mid_perm_cm_from_mulir()
-        den = float(arrays[f'{t}.den'][0])
-        report(f'{t}.mid / den', e.buffer('mid', t).reshape(N, -1) / den, sv[f'{t}.mid'].numpy()[:, pm])
-        pg = perm_cm_from_mulir(list(L.gate_muls))
-        report(f'{t}.gate_in', e.buffer('gate_in', t).reshape(N, -1), sv[f'{t}.gate_in'].numpy()[:, pg])
-        ph = perm_cm_from_mulir(list(L.out_muls))
-        report(f'{t}.gate_out', e.buffer('h', t).reshape(N, -1), sv[f'{t}.x_out'].numpy()[:, ph])
-    e.run_stage(eng.STAGE_FWD_END)
-    torch.cuda.synchronize()
-    report('atomic energy', e.buffer('atomic_energy'), ref['atomic_energy'].numpy())
-    print('energy engine', float(e.buffer('energy', dtype='f8')[0]), 'oracle', float(ref['energy']))
-    T = spec.n_layers
-    for t in range(T - 1, -1, -1):
-        e.run_stage(eng.STAGE_BWD_LAYER_A, t)
-        if t > 0:
-            e.run_stage(eng.STAGE_BWD_LAYER_B, t)
-    e.run_stage(eng.STAGE_BWD_END)
-    torch.cuda.synchronize()
-    perm = e._graph['perm']
-    fe = e.buffer('edge_force').reshape(E, 3)
-    want_fe = ref['edge_force'].numpy()
-    if perm is not None:
-        want_fe = want_fe[perm.cpu().numpy()]
-    report('edge force dE/d(edge_vec)', fe, want_fe)
-    report('forces', e.buffer('forces').reshape(N, 3), ref['forces'].numpy())
-    report('virial', e.buffer('virial', dtype='f8'), ref['virial'].numpy())
+    species = species_of(meta, z)
+    ref = oracle(name).forward(species, ei, ev, volume=abs(np.linalg.det(cell)), keep=True)
+    errors = stage_errors(B200Engine(meta, arrays, radial=radial), arrays, species, ei, ev, ref)
+    print(format_stage_errors(errors))
+    print('first divergence:', first_divergence(errors))
 
 
 if __name__ == '__main__':
