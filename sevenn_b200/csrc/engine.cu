@@ -545,6 +545,14 @@ static int launch_tc_linear(const TcWeights& w, const RowExp& re, const float* A
                             CU_TENSOR_MAP_INTERLEAVE_NONE, g_opt_tc_swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed (" + std::to_string((int)cr) + ")");
+    // C block viewed as (column, component, node): strides N*4 and ldc*4 bytes; the epilogue's TMA stores
+    const cuuint64_t cdim[3] = {(cuuint64_t)b.N, (cuuint64_t)b.d, (cuuint64_t)n_nodes};
+    const cuuint64_t cstr[2] = {(cuuint64_t)b.c_cs * 4, (cuuint64_t)ldc * 4};
+    const cuuint32_t cbox[3] = {(cuuint32_t)kTcCBox, 1, (cuuint32_t)kTcBM};
+    const CUresult cc = enc(&maps.c[t.nblocks], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)(C + c_off[l]), cdim, cstr, cbox, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cc != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed for C (" + std::to_string((int)cc) + ")");
     ++t.nblocks;
     ++bi;
   }

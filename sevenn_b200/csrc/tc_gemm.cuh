@@ -18,17 +18,18 @@
 //
 // Structure (persistent, one CTA per SM, 320 threads = 10 warps, tiles of 64 rows x NT <= 128 columns):
 //   warp 8   TMA producer A: per 32-wide K chunk one cp.async.bulk.tensor (3-D map over (k, component,
-//            node); 128B swizzle) for the raw fp32 A tile into an 8-deep ring (the HBM/L2 round trip of
-//            these loads is what has to be hidden: 64 KB in flight per SM)
-//   warp 9   producer W: one cp.async.bulk per chunk for the pre-sliced, pre-arranged W chunk (3-deep ring)
+//            node); 128B swizzle) for the raw fp32 A tile into a 4-deep ring (the HBM/L2 round trip of
+//            these loads is what has to be hidden: 32 KB in flight per SM)
+//   warp 9   producer W: one cp.async.bulk per chunk for the pre-sliced, pre-arranged W chunk (5-deep ring)
 //   warps 0-3 transform: two threads per row of a raw chunk (16 of its 32 k each) pull it into registers
 //            (freeing the raw slot), cut it into the three bf16 slices and write them in the canonical
 //            K-major no-swizzle core-matrix layout (8-row x 16-byte core matrices) into a 3-deep operand ring
 //   warps 4-7 one warpgroup: issues 12 wgmma.mma_async m64nNTk16 per chunk into its two register
 //            accumulators (64 x NT each, NT/2 + NT/2 registers per thread), releases a chunk's operand slots
 //            once the next chunk's MMAs are in flight (wgmma.wait_group 1), and after the tile's last chunk
-//            scales the accumulators and writes C straight from the fragments (8-byte stores per thread, a
-//            quad of lanes covers one 32-byte row segment), or RED.ADD.F32x2 when accumulating.
+//            scales the accumulators into a 64B-swizzled C tile in shared memory; one thread then issues TMA
+//            tensor stores (cp.reduce.async.bulk.tensor .add when accumulating) of 16-column boxes and the
+//            warpgroup moves on to the next tile while they drain.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -50,14 +51,20 @@ constexpr int kTcMmaWarps = 4;
 constexpr int kTcRawBytes = kTcBM * kTcKC * 4;            // 8 KB raw fp32 A chunk
 constexpr int kTcASliceBytes = kTcBM * kTcKC * 2;         // 4 KB per bf16 slice
 constexpr int kTcBSliceBytes = kTcMaxNT * kTcKC * 2;      // 8 KB per bf16 slice (NT = 128)
-// three decoupled rings: raw A chunks (deep: the HBM/L2 round trip of the TMA loads is what has to be
-// hidden), sliced A operands and sliced W operands (both released by the MMA warpgroup)
-constexpr int kTcRawStages = 8, kTcOpsStages = 3, kTcWStages = 3;
+// three decoupled rings -- raw A chunks (the HBM/L2 round trip of the TMA loads is what has to be hidden: 32 KB
+// in flight covers one H100 SM's share of HBM bandwidth x latency), sliced A operands and sliced W operands (both
+// released by the MMA warpgroup, one chunk late) -- and one C staging tile: 221 KB in all
+constexpr int kTcRawStages = 4, kTcOpsStages = 3, kTcWStages = 5;
 constexpr int kTcOpsBytes = 3 * kTcASliceBytes, kTcWBytes = 3 * kTcBSliceBytes;
+constexpr int kTcCBox = 16;                               // C columns per TMA store: one 64-byte swizzle row
+constexpr int kTcCBoxBytes = kTcBM * kTcCBox * 4;         // 4 KB
+constexpr int kTcCBytes = kTcBM * kTcMaxNT * 4;           // 32 KB staged C tile
 constexpr int kTcRawOff = 0;
 constexpr int kTcOpsOff = kTcRawOff + kTcRawStages * kTcRawBytes;
 constexpr int kTcWOff = kTcOpsOff + kTcOpsStages * kTcOpsBytes;
-constexpr int kTcSmemBytes = kTcWOff + kTcWStages * kTcWBytes + 1024 /*alignment slack*/;
+constexpr int kTcCOff = kTcWOff + kTcWStages * kTcWBytes;
+constexpr int kTcSmemBytes = kTcCOff + kTcCBytes + 1024 /*alignment slack*/;
+static_assert(kTcCOff % 1024 == 0, "the swizzled C staging tile must be 1024-byte aligned");
 constexpr int kTcZeroRow = -1000;   // row exponent of an all-zero row
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -111,6 +118,22 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
+}
+// TMA: 3-D tiled tensor store / reduce-add (one fp32 add per element) from shared memory, bulk-group completion
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%1, %2, %3}], [%4];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(src) : "memory");
+}
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%1, %2, %3}], [%4];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(src) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void mma_group_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // warps 4..7 only
+__device__ __forceinline__ void sts64(uint32_t saddr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(x), "f"(y) : "memory");
 }
 
 // wgmma shared-memory matrix descriptor, K-major, no swizzle: the two 8-row x 16-byte core matrices of one
@@ -278,7 +301,10 @@ struct TcLinArgs {
       }                                                                                           \
     }                                                                                             \
   } while (0)
-struct TcMaps { CUtensorMap m[kMaxL]; };   // per block: A viewed as (k, component, node), fp32
+// per block: A viewed as (k, component, node), fp32, 32 x 1 x 64 boxes, 128B swizzle; C viewed as
+// (column, component, node), fp32, 16 x 1 x 64 boxes, 64B swizzle (rows beyond n_nodes and columns beyond N are
+// clipped by the TMA unit, which masks the padded tiles)
+struct TcMaps { CUtensorMap m[kMaxL], c[kMaxL]; };
 
 // explicit shared-space accesses (the ring pointers are computed from an aligned base, which makes the compiler
 // fall back to generic LD/ST otherwise)
@@ -327,6 +353,7 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
   __shared__ uint64_t bar_raw_full[kTcRawStages], bar_raw_empty[kTcRawStages];
   __shared__ uint64_t bar_ops_full[kTcOpsStages], bar_ops_empty[kTcOpsStages];
   __shared__ uint64_t bar_w_full[kTcWStages], bar_w_empty[kTcWStages];
+  __shared__ __align__(16) float fb_s[kTcMaxNT];           // column scales of the tile in the epilogue
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int trace_n = 0;
@@ -463,8 +490,15 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
     // =================== MMA + epilogue warpgroup (warps 4..7) ===================
     // accumulator fragment of m64nNk16: warp w of the group holds rows 16 w + lane/4 (registers 4j, 4j+1) and
     // 16 w + lane/4 + 8 (4j+2, 4j+3), columns 8 j + 2 (lane % 4) + {0, 1}
-    const int mw = warp - 4, q4 = lane & 3;
+    const int mw = warp - 4, q4 = lane & 3, ct = tid - 128;
     const int rl = 16 * mw + (lane >> 2);
+    const uint32_t cst = smem_u32(smem + kTcCOff);
+    // staged C: box s = columns 16 s .. 16 s + 15, 64-byte rows, 16-byte granule g of row r at g ^ ((r >> 1) & 3)
+    // (the TMA 64B swizzle); a warp's 8-byte stores of 8 rows x 4 lanes then fill all 32 banks twice
+    auto c_addr = [&](int r, int j) -> uint32_t {
+      const int g = 2 * (j & 1) + (q4 >> 1);
+      return cst + (uint32_t)((j >> 1) * kTcCBoxBytes + r * 64 + ((g ^ ((r >> 1) & 3)) << 4) + (q4 & 1) * 8);
+    };
     float acc0[kTcAccRegs], acc1[kTcAccRegs];
 #pragma unroll
     for (int i = 0; i < kTcAccRegs; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
@@ -478,9 +512,12 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
       const int Ea0 = Ea_next0, Ea1 = Ea_next1;
       Ea_next0 = row_exp(t + gridDim.x, rl);
       Ea_next1 = row_exp(t + gridDim.x, rl + 8);
-      // the K loop of one tile, instantiated per tile width: the wgmma shape is an immediate, and a width
-      // dispatch inside the loop would make ptxas serialize the MMAs
-      auto mainloop = [&](auto width) {
+      const int col0 = nt * B.NT;
+      const float fb_t = (ct < B.NT && col0 + ct < B.N) ? __ldg(B.fb + col0 + ct) : 0.0f;   // in flight over the K loop
+      // the K loop and the staging of one tile, instantiated per tile width: the wgmma shape is an immediate (a
+      // width dispatch inside the loop would make ptxas serialize the MMAs), and with a runtime column bound the
+      // staging loop runs one branch per 8 columns, each waiting on its own shared-memory load
+      auto run_tile = [&](auto width) {
         constexpr int N = decltype(width)::value;
         int prev_o = 0, prev_w = 0;
         for (int kc = 0; kc < n_kc; ++kc, ++it) {
@@ -512,48 +549,50 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         acc_fence(acc1);
         __syncwarp();
         if (lane == 0) { mbar_arrive(&bar_ops_empty[prev_o]); mbar_arrive(&bar_w_empty[prev_w]); }
+        if (tid == 160) TC_TRACE(3, 0, tile_it);    // epilogue: accumulators complete
+
+        // the scaled tile goes to shared memory; one thread hands it to the TMA unit, whose stores (or
+        // reduce-adds, when accumulating) run while the next tile's MMAs are issued.  Every element of C belongs
+        // to exactly one tile, so the single add per element is deterministic.
+        const float fa0 = (Ea0 == kTcZeroRow) ? 0.0f : exp2i(Ea0 - 7);
+        const float fa1 = (Ea1 == kTcZeroRow) ? 0.0f : exp2i(Ea1 - 7);
+        if (tid == 128) bulk_wait_read_all();         // the previous tile's stores have read the staging tile
+        fb_s[ct] = fb_t;
+        mma_group_sync();
+        if (tid == 160) TC_TRACE(3, 2, tile_it);      // epilogue: staging tile free
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+          const float2 fb2 = *reinterpret_cast<const float2*>(&fb_s[8 * j + 2 * q4]);
+          sts64(c_addr(rl, j), (acc0[4 * j + 0] + acc1[4 * j + 0]) * fa0 * fb2.x,
+                (acc0[4 * j + 1] + acc1[4 * j + 1]) * fa0 * fb2.y);
+          sts64(c_addr(rl + 8, j), (acc0[4 * j + 2] + acc1[4 * j + 2]) * fa1 * fb2.x,
+                (acc0[4 * j + 3] + acc1[4 * j + 3]) * fa1 * fb2.y);
+        }
+        if (tid == 160) TC_TRACE(3, 3, tile_it);      // epilogue: tile staged
       };
       switch (B.NT) {
-        case 16: mainloop(std::integral_constant<int, 16>()); break;
-        case 32: mainloop(std::integral_constant<int, 32>()); break;
-        case 48: mainloop(std::integral_constant<int, 48>()); break;
-        case 64: mainloop(std::integral_constant<int, 64>()); break;
-        case 80: mainloop(std::integral_constant<int, 80>()); break;
-        case 96: mainloop(std::integral_constant<int, 96>()); break;
-        case 112: mainloop(std::integral_constant<int, 112>()); break;
-        default: mainloop(std::integral_constant<int, 128>()); break;
+        case 16: run_tile(std::integral_constant<int, 16>()); break;
+        case 32: run_tile(std::integral_constant<int, 32>()); break;
+        case 48: run_tile(std::integral_constant<int, 48>()); break;
+        case 64: run_tile(std::integral_constant<int, 64>()); break;
+        case 80: run_tile(std::integral_constant<int, 80>()); break;
+        case 96: run_tile(std::integral_constant<int, 96>()); break;
+        case 112: run_tile(std::integral_constant<int, 112>()); break;
+        default: run_tile(std::integral_constant<int, 128>()); break;
       }
-      if (tid == 160) TC_TRACE(3, 0, tile_it);    // epilogue: accumulators complete
-
-      // every element of C belongs to exactly one tile, so the single add per element is deterministic
-      const float fa0 = (Ea0 == kTcZeroRow) ? 0.0f : exp2i(Ea0 - 7);
-      const float fa1 = (Ea1 == kTcZeroRow) ? 0.0f : exp2i(Ea1 - 7);
-      const int col0 = nt * B.NT;
-      const int node0 = mt * kTcBM + rl;
-      const bool ok0 = node0 < a.n_nodes, ok1 = node0 + 8 < a.n_nodes;
-      float* c0 = a.C + (size_t)node0 * a.ldc + B.c_off + (size_t)ci * B.c_cs + col0 + 2 * q4;
-      float* c1 = c0 + (size_t)8 * a.ldc;
-      const float* fbp = B.fb + col0 + 2 * q4;
-#pragma unroll
-      for (int j = 0; j < kTcMaxNT / 8; ++j) {
-        // column pairs are all-in or all-out (N a multiple of 4)
-        if (8 * j < B.NT && col0 + 8 * j + 2 * q4 < B.N) {
-          const float2 fb2 = __ldg(reinterpret_cast<const float2*>(fbp + 8 * j));
-          const float2 v0 = make_float2((acc0[4 * j + 0] + acc1[4 * j + 0]) * fa0 * fb2.x,
-                                        (acc0[4 * j + 1] + acc1[4 * j + 1]) * fa0 * fb2.y);
-          const float2 v1 = make_float2((acc0[4 * j + 2] + acc1[4 * j + 2]) * fa1 * fb2.x,
-                                        (acc0[4 * j + 3] + acc1[4 * j + 3]) * fa1 * fb2.y);
-          if (a.accumulate) {
-            if (ok0) atomicAdd(reinterpret_cast<float2*>(c0 + 8 * j), v0);
-            if (ok1) atomicAdd(reinterpret_cast<float2*>(c1 + 8 * j), v1);
-          } else {
-            if (ok0) *reinterpret_cast<float2*>(c0 + 8 * j) = v0;
-            if (ok1) *reinterpret_cast<float2*>(c1 + 8 * j) = v1;
-          }
+      fence_async_smem();                             // generic-proxy writes -> visible to the TMA unit
+      mma_group_sync();
+      if (tid == 128) {
+        for (int s = 0; s < B.NT / kTcCBox && col0 + s * kTcCBox < B.N; ++s) {
+          const uint32_t src = cst + (uint32_t)(s * kTcCBoxBytes);
+          if (a.accumulate) tma_reduce_add_3d(&maps.c[b], src, col0 + s * kTcCBox, ci, mt * kTcBM);
+          else tma_store_3d(&maps.c[b], src, col0 + s * kTcCBox, ci, mt * kTcBM);
         }
+        bulk_commit();
       }
-      if (tid == 160) TC_TRACE(3, 1, tile_it);        // epilogue: tile written
+      if (tid == 160) TC_TRACE(3, 1, tile_it);        // epilogue: tile handed to the TMA unit
     }
+    if (tid == 128) bulk_wait_all();                  // the last stores complete before the CTA retires
   }
 }
 

@@ -8,7 +8,7 @@ from sevenn_b200.engine import check, load_library
 lib = load_library()
 ROLE = {0: 'prodA', 1: 'xform', 2: 'mma', 3: 'epi', 4: 'prodW'}
 EV = {(0, 0): 'issue', (1, 0): 'raw_landed', (1, 1): 'ops_free', (1, 2): 'written', (2, 0): 'w_landed', (2, 1): 'ops_ready',
-      (2, 2): 'acc_free', (3, 0): 'acc_full', (3, 1): 'tile_done', (4, 0): 'issue'}
+      (2, 2): 'acc_free', (3, 0): 'acc_full', (3, 1): 'tile_done', (3, 2): 'stage_free', (3, 3): 'staged', (4, 0): 'issue'}
 
 
 def run(n_nodes, a_K, c_N, acc, label, warm=True):
