@@ -361,7 +361,7 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
 
 // ---- tensor-core linear: host side --------------------------------------------------------------
 // Pre-sliced weights of one block-diagonal linear (see tc_gemm.cuh): per block l the three bf16 slices of
-// W^T in the canonical K-major core-matrix layout, cut into (n tile, 32-wide K chunk) blobs that one
+// W^T in the 64B-swizzled K-major layout, cut into (n tile, 32-wide K chunk) blobs that one
 // cp.async.bulk moves into a pipeline stage, plus the per-column scales 2^(Eb-7).
 struct TcWeights {
   DevBuf q, fb;
@@ -416,6 +416,21 @@ static void tc_pack_block(const float* W, int K, int N, int NT, uint16_t* q, flo
   }
 }
 
+// The device image of a packed block: every (n tile, K chunk, slice) piece of NT x 32 bf16 moves from the
+// canonical no-swizzle core-matrix order of tc_pack_block (8 rows x 16 bytes per core matrix, the four 8-k
+// granules of a row 128 bytes apart, 8-row groups 512 bytes apart) to the 64B-swizzled K-major rows that
+// blocklin_tc_kernel's wgmma descriptors read (tc_swz64, tc_gemm.cuh).
+static void tc_swizzle_block(uint16_t* q, size_t elems, int NT) {
+  const size_t piece = (size_t)NT * kTcKC;
+  std::vector<uint16_t> tmp(piece);
+  for (size_t p0 = 0; p0 < elems; p0 += piece) {
+    for (int r = 0; r < NT; ++r)
+      for (int g = 0; g < kTcKC / 8; ++g)
+        memcpy(tmp.data() + tc_swz64((uint32_t)r, (uint32_t)g) / 2, q + p0 + ((r & 7) * 16 + (r >> 3) * 512 + g * 128) / 2, 16);
+    memcpy(q + p0, tmp.data(), piece * sizeof(uint16_t));
+  }
+}
+
 static int tc_build_weights(TcWeights& w, const float* host, const int* Ks, const int* Ns, int n_l) {
   w.ok = false;
   w.nblocks = 0;
@@ -438,6 +453,7 @@ static int tc_build_weights(TcWeights& w, const float* host, const int* Ks, cons
     if (K == 0 || N == 0) continue;
     const TcWeights::Blk& b = w.blk[bi++];
     tc_pack_block(host + woff, K, N, b.NT, q.data() + b.q_off, fb.data() + b.fb_off);
+    tc_swizzle_block(q.data() + b.q_off, (size_t)3 * K * b.NT * tc_tiles(N, b.NT), b.NT);
     woff += (size_t)K * N;
   }
   if (w.q.ensure(q_total * sizeof(uint16_t) + 16) || w.fb.ensure(fb_total * sizeof(float) + 16)) return fail("cudaMalloc failed for tensor-core weights");

@@ -16,20 +16,24 @@
 // (the dropped A1*B2, A2*B1, A2*B2 are < 2^-24 relative).  Six bf16 MMAs per K = 16 step cost the same
 // tensor time as 3xTF32.  Emulated bit for bit on the CPU by tests/test_tc_pack_cpu.py.
 //
-// Structure (persistent, one CTA per SM, 320 threads = 10 warps, tiles of 64 rows x NT <= 128 columns):
-//   warp 8   TMA producer A: per 32-wide K chunk one cp.async.bulk.tensor (3-D map over (k, component,
+// Structure (persistent, one CTA per SM, 512 threads = four warpgroups, tiles of 64 rows x NT <= 128 columns;
+// setmaxnreg moves registers from the transform and producer warpgroups to the two MMA warpgroups):
+//   warps 0-3 transform: two threads per row of a raw chunk (16 of its 32 k each) pull it into registers
+//            (freeing the raw slot), cut it into the three bf16 slices and write them as 64-byte K-major rows
+//            with the 64B swizzle (tc_swz64) into a 3-deep operand ring
+//   warp 4   TMA producer A: per 32-wide K chunk one cp.async.bulk.tensor (3-D map over (k, component,
 //            node); 128B swizzle) for the raw fp32 A tile into a 4-deep ring (the HBM/L2 round trip of
 //            these loads is what has to be hidden: 32 KB in flight per SM)
-//   warp 9   producer W: one cp.async.bulk per chunk for the pre-sliced, pre-arranged W chunk (5-deep ring)
-//   warps 0-3 transform: two threads per row of a raw chunk (16 of its 32 k each) pull it into registers
-//            (freeing the raw slot), cut it into the three bf16 slices and write them in the canonical
-//            K-major no-swizzle core-matrix layout (8-row x 16-byte core matrices) into a 3-deep operand ring
-//   warps 4-7 one warpgroup: issues 12 wgmma.mma_async m64nNTk16 per chunk into its two register
-//            accumulators (64 x NT each, NT/2 + NT/2 registers per thread), releases a chunk's operand slots
-//            once the next chunk's MMAs are in flight (wgmma.wait_group 1), and after the tile's last chunk
-//            scales the accumulators into a 64B-swizzled C tile in shared memory; one thread then issues TMA
-//            tensor stores (cp.reduce.async.bulk.tensor .add when accumulating) of 16-column boxes and the
-//            warpgroup moves on to the next tile while they drain.
+//   warp 5   producer W: one cp.async.bulk per chunk for the pre-sliced W chunk, already in the swizzled
+//            operand layout (5-deep ring)
+//   warp 6   C store thread: issues the TMA tensor stores (cp.reduce.async.bulk.tensor .add when accumulating)
+//            of each staged tile in 16-column boxes and frees the staging tile once they have read it
+//   warps 8-11, 12-15  two MMA warpgroups on alternate tiles of the CTA.  Each issues 12 wgmma.mma_async
+//            m64nNTk16 per chunk into its own two register accumulators (64 x NT each, NT/2 + NT/2 registers
+//            per thread), releases a chunk's operand slots once the next chunk's MMAs are in flight
+//            (wgmma.wait_group 1), hands the rings to the other warpgroup after its tile's last chunk and then
+//            scales the accumulators into the shared 64B-swizzled C staging tile -- while the other warpgroup
+//            issues the next tile's MMAs.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -45,7 +49,9 @@ constexpr int kTcBM = 64;           // rows (nodes) per tile: the M of one wgmma
 constexpr int kTcKC = 32;           // K elements per pipeline stage
 constexpr int kTcMaxNT = 128;       // columns per tile
 constexpr int kTcAccRegs = kTcMaxNT / 2;   // fp32 registers per thread of one m64nNTk16 accumulator at NT = 128
-constexpr int kTcThreads = 320;     // 4 transform warps, one MMA + epilogue warpgroup, A producer, W producer
+constexpr int kTcThreads = 512;     // four warpgroups: transform; producers + C store; two MMA + epilogue
+// registers per thread after setmaxnreg (the launch gives 65536 / 512 = 128): 88 + 40 + 2 x 192 = 512 = 4 x 128
+constexpr int kTcXformRegs = 88, kTcProdRegs = 40, kTcMmaRegs = 192;
 constexpr int kTcXformThreads = 128; // two threads per row of a chunk (16 of its 32 k each)
 constexpr int kTcMmaWarps = 4;
 constexpr int kTcRawBytes = kTcBM * kTcKC * 4;            // 8 KB raw fp32 A chunk
@@ -53,7 +59,8 @@ constexpr int kTcASliceBytes = kTcBM * kTcKC * 2;         // 4 KB per bf16 slice
 constexpr int kTcBSliceBytes = kTcMaxNT * kTcKC * 2;      // 8 KB per bf16 slice (NT = 128)
 // three decoupled rings -- raw A chunks (the HBM/L2 round trip of the TMA loads is what has to be hidden: 32 KB
 // in flight covers one H100 SM's share of HBM bandwidth x latency), sliced A operands and sliced W operands (both
-// released by the MMA warpgroup, one chunk late) -- and one C staging tile: 221 KB in all
+// released by the MMA warpgroups, one chunk late) -- and one C staging tile that the two MMA warpgroups take in
+// turn (their epilogues never overlap): 221 KB in all
 constexpr int kTcRawStages = 4, kTcOpsStages = 3, kTcWStages = 5;
 constexpr int kTcOpsBytes = 3 * kTcASliceBytes, kTcWBytes = 3 * kTcBSliceBytes;
 constexpr int kTcCBox = 16;                               // C columns per TMA store: one 64-byte swizzle row
@@ -131,16 +138,24 @@ __device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* map, uint32
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void mma_group_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // warps 4..7 only
+// named barrier 1 + g: the 128 threads of MMA warpgroup g only
+__device__ __forceinline__ void mma_group_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void sts64(uint32_t saddr, float x, float y) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(x), "f"(y) : "memory");
 }
 
-// wgmma shared-memory matrix descriptor, K-major, no swizzle: the two 8-row x 16-byte core matrices of one
-// K = 16 step lie 128 bytes apart (leading byte offset), 8-row groups 512 bytes apart (stride byte offset).
+// wgmma shared-memory matrix descriptor, K-major, 64-byte swizzle (layout type 2): one operand row is the 32 k
+// of a chunk, 64 bytes, its 16-byte granule g stored at g ^ ((row >> 1) & 3) (tc_swz64); 8-row groups lie 512
+// bytes apart (stride byte offset); the leading byte offset is unused because a K = 16 step (32 bytes) stays
+// inside one swizzled row.  The K step j starts 32 j bytes into the rows; the swizzle is applied to the address
+// bits, so every operand slice starts on a 512-byte (here 1024-byte) boundary.
 __device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
 }
+// byte offset of 16-byte granule g (k = 8 g .. 8 g + 7) of operand row r in a 64B-swizzled K-major slice
+__host__ __device__ __forceinline__ uint32_t tc_swz64(uint32_t r, uint32_t g) { return r * 64u + ((g ^ ((r >> 1) & 3u)) << 4); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -283,14 +298,15 @@ struct TcLinArgs {
   int trace_cap;
   TcLinBlock blk[kMaxL];
 };
-// timeline events of CTA 0 (a.trace != nullptr): five roles, each traced by ONE thread that keeps its own
+// timeline events of CTA 0 (a.trace != nullptr): seven roles (A producer, transform, MMA and epilogue of
+// warpgroup 0, W producer, MMA and epilogue of warpgroup 1), each traced by ONE thread that keeps its own
 // record counter in a register and stores {event, index, clock64} with plain stores (no atomics: an atomic's
 // round trip would cost more than the stages being measured).  Layout: role r owns records
-// [r * trace_cap / 5, (r + 1) * trace_cap / 5); word 0 of the buffer is unused, counts are in words 1..5.
+// [r * trace_cap / 7, (r + 1) * trace_cap / 7); word 0 of the buffer is unused, counts are in words 1..7.
 #define TC_TRACE(role, ev, idx)                                                                   \
   do {                                                                                            \
     if (a.trace != nullptr && blockIdx.x == 0) {                                                  \
-      const int per = a.trace_cap / 5;                                                            \
+      const int per = a.trace_cap / 7;                                                            \
       if (trace_n < per) {                                                                        \
         long long* rec = a.trace + 8 + 3 * ((size_t)(role) * per + trace_n);                      \
         rec[0] = (ev);                                                                            \
@@ -329,7 +345,7 @@ __device__ __forceinline__ void tc_mma_chunk(float (&acc0)[kTcAccRegs], float (&
   constexpr uint32_t b_slice = (uint32_t)N * kTcKC * 2u;
 #pragma unroll
   for (int j = 0; j < kTcKC / 16; ++j) {
-    const uint32_t ko = (uint32_t)j * 256u;     // two 16-byte K core matrices per MMA
+    const uint32_t ko = (uint32_t)j * 32u;      // 16 k = 32 bytes into the swizzled rows
     const uint64_t dA0 = gmma_desc(sa + ko);
     const uint64_t dA1 = gmma_desc(sa + kTcASliceBytes + ko);
     const uint64_t dA2 = gmma_desc(sa + 2 * kTcASliceBytes + ko);
@@ -353,7 +369,9 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
   __shared__ uint64_t bar_raw_full[kTcRawStages], bar_raw_empty[kTcRawStages];
   __shared__ uint64_t bar_ops_full[kTcOpsStages], bar_ops_empty[kTcOpsStages];
   __shared__ uint64_t bar_w_full[kTcWStages], bar_w_empty[kTcWStages];
-  __shared__ __align__(16) float fb_s[kTcMaxNT];           // column scales of the tile in the epilogue
+  __shared__ uint64_t bar_c_full, bar_c_free[2];            // staging tile: written by a warpgroup / read by the stores
+  __shared__ uint64_t bar_turn[2];                          // MMA warpgroup g may start its next K loop
+  __shared__ __align__(16) float fb_s[2][kTcMaxNT];        // column scales of each MMA warpgroup's tile
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int trace_n = 0;
@@ -362,6 +380,11 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
     for (int s = 0; s < kTcRawStages; ++s) { mbar_init(&bar_raw_full[s], 1); mbar_init(&bar_raw_empty[s], kTcXformThreads); }
     for (int s = 0; s < kTcOpsStages; ++s) { mbar_init(&bar_ops_full[s], kTcXformThreads); mbar_init(&bar_ops_empty[s], kTcMmaWarps); }
     for (int s = 0; s < kTcWStages; ++s) { mbar_init(&bar_w_full[s], 1); mbar_init(&bar_w_empty[s], kTcMmaWarps); }
+    mbar_init(&bar_c_full, 1);
+    mbar_init(&bar_c_free[0], 1);
+    mbar_init(&bar_c_free[1], 1);
+    mbar_init(&bar_turn[0], kTcMmaWarps);
+    mbar_init(&bar_turn[1], kTcMmaWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -391,9 +414,11 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
     return v;
   };
 
-  if (warp == 8) {
+  if (warp >= 4 && warp < 8) {
+    // producer warpgroup: A producer (warp 4), W producer (warp 5), C store thread (warp 6); warp 7 is idle
+    setmaxnreg_dec<kTcProdRegs>();
+    if (warp == 4 && lane == 0) {
     // =================== TMA producer, A: raw fp32 chunks ===================
-    if (lane == 0) {
       uint32_t it = 0;
       for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x) {
         int b, mt, ci, nt;
@@ -407,10 +432,8 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
           tma_load_3d(smem + kTcRawOff + (size_t)s * kTcRawBytes, &maps.m[b], kc * kTcKC, ci, mt * kTcBM, &bar_raw_full[s]);
         }
       }
-    }
-  } else if (warp == 9) {
+    } else if (warp == 5 && lane == 0) {
     // =================== TMA producer, W: pre-sliced bf16 chunks ===================
-    if (lane == 0) {
       uint32_t it = 0;
       for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x) {
         int b, mt, ci, nt;
@@ -427,13 +450,35 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
           bulk_load(smem + kTcWOff + (size_t)s * kTcWBytes, wsrc + (size_t)kc * b_bytes, b_bytes, &bar_w_full[s]);
         }
       }
+    } else if (warp == 6 && lane == 0) {
+    // =================== C store thread: staged tiles -> TMA tensor stores, in tile order ===================
+      // owns every bulk group of the CTA, so it alone can wait for a tile's stores to have read the staging tile;
+      // it then hands the staging tile to the warpgroup of the next tile (c_free[(s + 1) & 1])
+      uint32_t s = 0;
+      for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++s) {
+        int b, mt, ci, nt;
+        decode(t, b, mt, ci, nt);
+        const TcLinBlock& B = a.blk[b];
+        const int col0 = nt * B.NT;
+        mbar_wait(&bar_c_full, s & 1);
+        const uint32_t cst = smem_u32(smem + kTcCOff);
+        for (int q = 0; q < B.NT / kTcCBox && col0 + q * kTcCBox < B.N; ++q) {
+          const uint32_t src = cst + (uint32_t)(q * kTcCBoxBytes);
+          if (a.accumulate) tma_reduce_add_3d(&maps.c[b], src, col0 + q * kTcCBox, ci, mt * kTcBM);
+          else tma_store_3d(&maps.c[b], src, col0 + q * kTcCBox, ci, mt * kTcBM);
+        }
+        bulk_commit();
+        bulk_wait_read_all();
+        mbar_arrive(&bar_c_free[(s + 1) & 1]);
+      }
+      bulk_wait_all();                                // the last stores complete before the CTA retires
     }
   } else if (warp < 4) {
     // =================== transform: raw fp32 row -> three bf16 slices ===================
     // thread (r, h): row r of the tile, k = 16 h .. 16 h + 15 of the chunk
+    setmaxnreg_dec<kTcXformRegs>();
     const int r = tid & (kTcBM - 1), h = tid / kTcBM;
     const uint32_t swz = a.swizzle ? (uint32_t)(r & 7) : 0u;
-    const uint32_t row_off = (uint32_t)((r & 7) * 16 + (r >> 3) * 512);
     const V2 M2 = splat2(12582912.0f), nM2 = splat2(-12582912.0f);     // 1.5 * 2^23: (x + M) - M = rint(x)
     uint32_t it = 0;
     int Ea_next = row_exp(blockIdx.x, r);
@@ -459,7 +504,7 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         const uint32_t a0 = smem_u32(smem + kTcOpsOff + (size_t)o * kTcOpsBytes);
         const uint32_t a1 = a0 + kTcASliceBytes, a2 = a1 + kTcASliceBytes;
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {                // 8 consecutive k = one 16-byte core-matrix row
+        for (int kk = 0; kk < 2; ++kk) {                // 8 consecutive k = one 16-byte granule of the row
           const V2 x[4] = {make_float2(v[2 * kk].x, v[2 * kk].y), make_float2(v[2 * kk].z, v[2 * kk].w),
                            make_float2(v[2 * kk + 1].x, v[2 * kk + 1].y), make_float2(v[2 * kk + 1].z, v[2 * kk + 1].w)};
           uint32_t p0[4], p1[4], p2[4];
@@ -476,7 +521,7 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
             p1[j] = pack_bf16(s1.x, s1.y);
             p2[j] = pack_bf16(s2.x, s2.y);
           }
-          const uint32_t off = row_off + (uint32_t)(2 * h + kk) * 128u;
+          const uint32_t off = tc_swz64((uint32_t)r, (uint32_t)(2 * h + kk));
           sts128(a0 + off, p0[0], p0[1], p0[2], p0[3]);
           sts128(a1 + off, p1[0], p1[1], p1[2], p1[3]);
           sts128(a2 + off, p2[0], p2[1], p2[2], p2[3]);
@@ -486,34 +531,38 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         mbar_arrive(&bar_ops_full[o]);
       }
     }
-  } else if (warp < 8) {
-    // =================== MMA + epilogue warpgroup (warps 4..7) ===================
+  } else {
+    // =================== two MMA + epilogue warpgroups (warps 8..11, 12..15) ===================
+    // warpgroup g takes the CTA's tiles tile_it = g, g + 2, ...; both walk the whole tile list so that they consume
+    // the operand and W rings in tile order.  While one stages its tile, the other issues MMAs.
     // accumulator fragment of m64nNk16: warp w of the group holds rows 16 w + lane/4 (registers 4j, 4j+1) and
     // 16 w + lane/4 + 8 (4j+2, 4j+3), columns 8 j + 2 (lane % 4) + {0, 1}
-    const int mw = warp - 4, q4 = lane & 3, ct = tid - 128;
+    setmaxnreg_inc<kTcMmaRegs>();
+    const int g = (warp - 8) >> 2, mw = (warp - 8) & 3, q4 = lane & 3, ct = tid & 127;
     const int rl = 16 * mw + (lane >> 2);
+    const bool tr_mma = (ct == 0), tr_epi = (ct == 32);   // the threads that trace this warpgroup's roles
+    const int role_mma = g ? 5 : 2, role_epi = g ? 6 : 3;
     const uint32_t cst = smem_u32(smem + kTcCOff);
+    float* fbs = fb_s[g];
     // staged C: box s = columns 16 s .. 16 s + 15, 64-byte rows, 16-byte granule g of row r at g ^ ((r >> 1) & 3)
     // (the TMA 64B swizzle); a warp's 8-byte stores of 8 rows x 4 lanes then fill all 32 banks twice
     auto c_addr = [&](int r, int j) -> uint32_t {
-      const int g = 2 * (j & 1) + (q4 >> 1);
-      return cst + (uint32_t)((j >> 1) * kTcCBoxBytes + r * 64 + ((g ^ ((r >> 1) & 3)) << 4) + (q4 & 1) * 8);
+      const int gr = 2 * (j & 1) + (q4 >> 1);
+      return cst + (uint32_t)((j >> 1) * kTcCBoxBytes + r * 64 + ((gr ^ ((r >> 1) & 3)) << 4) + (q4 & 1) * 8);
     };
     float acc0[kTcAccRegs], acc1[kTcAccRegs];
 #pragma unroll
     for (int i = 0; i < kTcAccRegs; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
-    uint32_t it = 0, tile_it = 0;
-    int Ea_next0 = row_exp(blockIdx.x, rl), Ea_next1 = row_exp(blockIdx.x, rl + 8);
+    uint32_t it = 0, tile_it = 0, mine = 0;
     for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++tile_it) {
       int b, mt, ci, nt;
       decode(t, b, mt, ci, nt);
       const TcLinBlock& B = a.blk[b];
       const int n_kc = B.K / kTcKC;
-      const int Ea0 = Ea_next0, Ea1 = Ea_next1;
-      Ea_next0 = row_exp(t + gridDim.x, rl);
-      Ea_next1 = row_exp(t + gridDim.x, rl + 8);
+      if ((int)(tile_it & 1) != g) { it += n_kc; continue; }     // the other warpgroup's tile
+      const int Ea0 = row_exp(t, rl), Ea1 = row_exp(t, rl + 8);   // in flight over the K loop, like fb_t
       const int col0 = nt * B.NT;
-      const float fb_t = (ct < B.NT && col0 + ct < B.N) ? __ldg(B.fb + col0 + ct) : 0.0f;   // in flight over the K loop
+      const float fb_t = (ct < B.NT && col0 + ct < B.N) ? __ldg(B.fb + col0 + ct) : 0.0f;
       // the K loop and the staging of one tile, instantiated per tile width: the wgmma shape is an immediate (a
       // width dispatch inside the loop would make ptxas serialize the MMAs), and with a runtime column bound the
       // staging loop runs one branch per 8 columns, each waiting on its own shared-memory load
@@ -523,9 +572,9 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         for (int kc = 0; kc < n_kc; ++kc, ++it) {
           const int o = it % kTcOpsStages, w = it % kTcWStages;
           mbar_wait(&bar_w_full[w], (it / kTcWStages) & 1);
-          if (tid == 128) TC_TRACE(2, 0, it);      // MMA: weights landed
+          if (tr_mma) TC_TRACE(role_mma, 0, it);      // MMA: weights landed
           mbar_wait(&bar_ops_full[o], (it / kTcOpsStages) & 1);
-          if (tid == 128) TC_TRACE(2, 1, it);      // MMA: operands ready, issuing
+          if (tr_mma) TC_TRACE(role_mma, 1, it);      // MMA: operands ready, issuing
           __syncwarp();
           const uint32_t sa = smem_u32(smem + kTcOpsOff + (size_t)o * kTcOpsBytes);
           const uint32_t sb = smem_u32(smem + kTcWOff + (size_t)w * kTcWBytes);
@@ -537,6 +586,7 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
           acc_fence(acc0);
           acc_fence(acc1);
           wgmma_wait<1>();             // the previous chunk's MMAs have read their operands: release its slots
+          if (tr_mma) TC_TRACE(role_mma, 2, it);      // MMA: the previous chunk has retired
           if (kc > 0) {
             __syncwarp();
             if (lane == 0) { mbar_arrive(&bar_ops_empty[prev_o]); mbar_arrive(&bar_w_empty[prev_w]); }
@@ -544,32 +594,41 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
           prev_o = o;
           prev_w = w;
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bar_turn[g ^ 1]);   // every chunk of this tile has landed: the other may go on
         wgmma_wait<0>();
         acc_fence(acc0);
         acc_fence(acc1);
         __syncwarp();
         if (lane == 0) { mbar_arrive(&bar_ops_empty[prev_o]); mbar_arrive(&bar_w_empty[prev_w]); }
-        if (tid == 160) TC_TRACE(3, 0, tile_it);    // epilogue: accumulators complete
+        if (tr_epi) TC_TRACE(role_epi, 0, tile_it);   // epilogue: accumulators complete
 
-        // the scaled tile goes to shared memory; one thread hands it to the TMA unit, whose stores (or
-        // reduce-adds, when accumulating) run while the next tile's MMAs are issued.  Every element of C belongs
-        // to exactly one tile, so the single add per element is deterministic.
+        // the scaled tile goes to the shared staging tile once the store thread has read the previous tile out of
+        // it (the other warpgroup's); the store thread hands it to the TMA unit, whose stores (or reduce-adds,
+        // when accumulating) run while both warpgroups go on.  Every element of C belongs to exactly one tile,
+        // so the single add per element is deterministic.
         const float fa0 = (Ea0 == kTcZeroRow) ? 0.0f : exp2i(Ea0 - 7);
         const float fa1 = (Ea1 == kTcZeroRow) ? 0.0f : exp2i(Ea1 - 7);
-        if (tid == 128) bulk_wait_read_all();         // the previous tile's stores have read the staging tile
-        fb_s[ct] = fb_t;
-        mma_group_sync();
-        if (tid == 160) TC_TRACE(3, 2, tile_it);      // epilogue: staging tile free
+        fbs[ct] = fb_t;
+        // this warpgroup's j-th tile is tile 2 j + g; it needs completion 2 j + g - 1 of the store thread's reads,
+        // which is arrival j - 1 + g on c_free[g] (none for tile 0: parity 1 passes on a fresh barrier)
+        mbar_wait(&bar_c_free[g], (mine & 1) ^ (uint32_t)(g ^ 1));
+        mma_group_sync(g);
+        if (tr_epi) TC_TRACE(role_epi, 2, tile_it);   // epilogue: staging tile free
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) {
-          const float2 fb2 = *reinterpret_cast<const float2*>(&fb_s[8 * j + 2 * q4]);
+          const float2 fb2 = *reinterpret_cast<const float2*>(&fbs[8 * j + 2 * q4]);
           sts64(c_addr(rl, j), (acc0[4 * j + 0] + acc1[4 * j + 0]) * fa0 * fb2.x,
                 (acc0[4 * j + 1] + acc1[4 * j + 1]) * fa0 * fb2.y);
           sts64(c_addr(rl + 8, j), (acc0[4 * j + 2] + acc1[4 * j + 2]) * fa1 * fb2.x,
                 (acc0[4 * j + 3] + acc1[4 * j + 3]) * fa1 * fb2.y);
         }
-        if (tid == 160) TC_TRACE(3, 3, tile_it);      // epilogue: tile staged
+        if (tr_epi) TC_TRACE(role_epi, 3, tile_it);   // epilogue: tile staged
       };
+      // the K loops take turns in tile order: a warpgroup waits on a ring slot only once every earlier chunk has
+      // landed, so the slot's barrier is never two phases behind the chunk it waits for (its parity would pass).
+      // This warpgroup's j-th tile waits for arrival j - 1 + g on bar_turn[g] (none for tile 0).
+      mbar_wait(&bar_turn[g], (mine & 1) ^ (uint32_t)(g ^ 1));
       switch (B.NT) {
         case 16: run_tile(std::integral_constant<int, 16>()); break;
         case 32: run_tile(std::integral_constant<int, 32>()); break;
@@ -581,18 +640,11 @@ blocklin_tc_kernel(const TcLinArgs a, const __grid_constant__ TcMaps maps) {
         default: run_tile(std::integral_constant<int, 128>()); break;
       }
       fence_async_smem();                             // generic-proxy writes -> visible to the TMA unit
-      mma_group_sync();
-      if (tid == 128) {
-        for (int s = 0; s < B.NT / kTcCBox && col0 + s * kTcCBox < B.N; ++s) {
-          const uint32_t src = cst + (uint32_t)(s * kTcCBoxBytes);
-          if (a.accumulate) tma_reduce_add_3d(&maps.c[b], src, col0 + s * kTcCBox, ci, mt * kTcBM);
-          else tma_store_3d(&maps.c[b], src, col0 + s * kTcCBox, ci, mt * kTcBM);
-        }
-        bulk_commit();
-      }
-      if (tid == 160) TC_TRACE(3, 1, tile_it);        // epilogue: tile handed to the TMA unit
+      mma_group_sync(g);                              // (also: every thread is done reading fbs)
+      if (ct == 0) mbar_arrive(&bar_c_full);
+      if (tr_epi) TC_TRACE(role_epi, 1, tile_it);     // epilogue: tile handed to the store thread
+      ++mine;
     }
-    if (tid == 128) bulk_wait_all();                  // the last stores complete before the CTA retires
   }
 }
 

@@ -6,9 +6,13 @@ ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..')
 sys.path.insert(0, ROOT)
 from sevenn_b200.engine import check, load_library
 lib = load_library()
-ROLE = {0: 'prodA', 1: 'xform', 2: 'mma', 3: 'epi', 4: 'prodW'}
+ROLE = {0: 'prodA', 1: 'xform', 2: 'mma0', 3: 'epi0', 4: 'prodW', 5: 'mma1', 6: 'epi1'}
 EV = {(0, 0): 'issue', (1, 0): 'raw_landed', (1, 1): 'ops_free', (1, 2): 'written', (2, 0): 'w_landed', (2, 1): 'ops_ready',
-      (2, 2): 'acc_free', (3, 0): 'acc_full', (3, 1): 'tile_done', (3, 2): 'stage_free', (3, 3): 'staged', (4, 0): 'issue'}
+      (2, 2): 'wait1_ret', (3, 0): 'acc_full', (3, 1): 'tile_done', (3, 2): 'stage_free', (3, 3): 'staged', (4, 0): 'issue'}
+EV.update({(5, e): EV[(2, e)] for e in range(3)})
+EV.update({(6, e): EV[(3, e)] for e in range(4)})
+MMA_WG = [(2, 3), (5, 6)]           # (MMA role, epilogue role) of each MMA warpgroup
+N_ROLES = 7
 
 
 def run(n_nodes, a_K, c_N, acc, label, warm=True):
@@ -38,9 +42,9 @@ def run(n_nodes, a_K, c_N, acc, label, warm=True):
     view = torch.as_tensor(_DevView(buf.value, (8 + 3 * cap,), '<i8'), device='cuda')
     host = view.cpu().numpy().copy()
     check(lib.s7b_tc_trace_enable(0, ctypes.byref(buf)))
-    per = cap // 5
+    per = cap // N_ROLES
     recs = []
-    for role in range(5):
+    for role in range(N_ROLES):
         n_r = int(min(host[1 + role], per))
         blk = host[8 + 3 * role * per: 8 + 3 * (role * per + n_r)].reshape(n_r, 3)
         recs.append(np.concatenate([np.full((n_r, 1), role, dtype=np.int64), blk], axis=1))
@@ -61,12 +65,35 @@ def run(n_nodes, a_K, c_N, acc, label, warm=True):
     def ev(role, e_):
         m = rec[(rec[:, 0] == role) & (rec[:, 1] == e_)]
         return dict(zip(m[:, 2].tolist(), (m[:, 3] - t0).tolist()))
-    issue, landed, free, written, ready = ev(0, 0), ev(1, 0), ev(1, 1), ev(1, 2), ev(2, 1)
+    issue, landed, free, written, ready = ev(0, 0), ev(1, 0), ev(1, 1), ev(1, 2), {**ev(2, 1), **ev(5, 1)}
     lat = [(k, landed[k] - issue[k], free[k] - landed[k], written[k] - free[k], ready[k] - written[k]) for k in sorted(issue) if k in landed and k in written and k in ready and k in free]
     arr = np.array(lat)
     if len(arr):
         print('   per chunk (mean clk): TMA issue->landed %.0f | landed->ops slot free %.0f | convert %.0f | written->MMA sees it %.0f' % tuple(arr[:, 1:].mean(0)))
         print('   first 10 chunks:', arr[:10].tolist())
+    # MMA warpgroup, per chunk: waiting in w_landed / ops_ready (from the warpgroup's previous event: the last
+    # chunk's wait_group 1 return, or the end of its previous epilogue), then ops_ready -> wait_group 1 returned
+    # (issuing this chunk and retiring the previous one); chunk interval = ops_ready to ops_ready inside a tile
+    for mma_role, epi_role in MMA_WG:
+        wl, rd, wt = ev(mma_role, 0), ev(mma_role, 1), ev(mma_role, 2)
+        marks = np.sort(np.array(list(wt.values()) + list(ev(epi_role, 1).values()), dtype=np.int64))
+        tile_ends = np.sort(np.array(list(ev(epi_role, 1).values()), dtype=np.int64))
+        rows = []
+        for k in sorted(rd):
+            if k not in wl or k not in wt:
+                continue
+            i = np.searchsorted(marks, wl[k]) - 1
+            if i < 0:
+                continue
+            prev_rd = rd.get(k - 1)
+            same_tile = prev_rd is not None and not np.any((tile_ends > prev_rd) & (tile_ends < rd[k]))
+            rows.append((wl[k] - marks[i], rd[k] - wl[k], wt[k] - rd[k], rd[k] - prev_rd if same_tile else -1))
+        if rows:
+            r = np.array(rows, dtype=np.float64)
+            iv = r[r[:, 3] >= 0, 3]
+            print(f'   {ROLE[mma_role]} per chunk (mean clk, {len(r)} chunks): wait w_landed {r[:, 0].mean():.0f} | wait ops_ready '
+                  f'{r[:, 1].mean():.0f} | ops_ready->wait_group 1 returned {r[:, 2].mean():.0f} | chunk interval in a tile '
+                  f'{iv.mean() if len(iv) else 0:.0f} (median {np.median(iv) if len(iv) else 0:.0f})')
 
 
 run(12000, [128, 64, 32], [128, 64, 32], False, 'self_interaction_1')
