@@ -6,8 +6,12 @@ reference are 4.5e-5 / 1.8e-5 (relative) smaller in magnitude than the fp64 sums
 ~130 000 lattice images of every atom pair in a float (``disp_local``, pair_d3_for_ase.cu:1560,1700), and the
 far images (each ~6e-8 of the running sum, i.e. at the fp32 rounding threshold) are partly absorbed.  The
 oracle keeps the exact sum; the test bounds the difference and checks its sign."""
-import numpy as np
+import os
 
+import numpy as np
+import pytest
+
+import d3_cells as C
 from oracle.d3_oracle import ase_results, d3_reference
 
 NACL = dict(numbers=[11, 17], positions=[[0.0, 0.0, 0.0], [2.815, 0.0, 0.0]],
@@ -59,3 +63,23 @@ def test_forces_are_the_energy_gradient():
             assert abs(fd - base['forces'][a, k]) < 2e-6, (damping, a, k, fd, base['forces'][a, k])
         assert np.abs(base['forces'].sum(0)).max() < 1e-12
         assert np.allclose(base['sigma'], base['sigma'].T, atol=1e-12)
+
+
+@pytest.mark.parametrize('fixture,damping,functional', C.GOLDEN_CASES)
+def test_matches_compiled_reference_edge_cells(fixture, damping, functional):
+    """The oracle against stored outputs of the reference's compiled D3 (tools/make_d3_golden.py) on a sheared
+    cell, a slab, a compressed Cs cell (weight sums below 1e-300) and 16 species, each with a functional at an
+    extreme of the table.  Measured: energy within 1.8e-6 (relative), forces within 2.7e-6 and stress within
+    2.0e-6 of their largest component; the reference's fp32 image sums (see the module docstring) account for
+    that, most on the 5.75 A Cs cell with its ~12 000 lattice images.  Bounds 1e-5."""
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'd3_compiled_reference.npz'))
+    k = C.golden_key(fixture, damping, functional)
+    z, pos, cell, pbc = C.FIXTURES[fixture]()
+    assert np.array_equal(pos, g[k + '_positions'])
+    r = d3_reference(z, pos, cell, pbc, damping=damping, functional=functional)
+    s = r['sigma']
+    s6 = np.array([s[0, 0], s[1, 1], s[2, 2], s[0, 1], s[0, 2], s[1, 2]])
+    f_ref, s_ref = g[k + '_forces'], g[k + '_stress']
+    assert abs(r['energy'] / float(g[k + '_energy']) - 1.0) < 1e-5
+    assert np.abs(r['forces'] - f_ref).max() < 1e-5 * np.abs(f_ref).max()
+    assert np.abs(s6 - s_ref).max() < 1e-5 * np.abs(s_ref).max()
