@@ -167,7 +167,8 @@ S7B_API int s7b_engine_compute(S7bEngine* eng, void* stream);
 
 /* Device pointer to an engine-owned buffer (valid until the next set_graph that grows it):
  * "x" (layer t input after self_interaction_1, [n_nodes, dim_x(t)]), "dx", "gate_in", "mid",
- * "h", "energy" (double[1]), "atomic_energy" [n_local], "forces" [n_nodes,3], "edge_force" [E,3],
+ * "h", "energy" (double[1]), "atomic_energy" [n_local], "atomic_energy_f64" (double[n_local], the same
+ * per-atom energies before their rounding to float), "forces" [n_nodes,3], "edge_force" [E,3],
  * "virial" (double[6], = -sum r (x) f), "edge_Y", "edge_rec".  *numel receives the element count. */
 S7B_API void* s7b_engine_buffer(S7bEngine* eng, const char* name, int layer, size_t* numel);
 
@@ -216,6 +217,27 @@ S7B_API int s7b_engine_compute_positions_host(S7bEngine* eng, int32_t n_atoms, c
 S7B_API int s7b_engine_neighbor_rows_host(S7bEngine* eng, int32_t n_atoms, const int32_t* species, const double* positions,
                                           const double* cell9, const int32_t* pbc3, int32_t n_centres,
                                           const int32_t* centres, int64_t* n_edges_out, void* stream);
+
+/* B independent structures; atoms of structure b are [atom_ptr[b], atom_ptr[b+1]) (host, B+1 entries,
+ * atom_ptr[0] = 0, non-decreasing; empty structures are legal).  species [n] and positions [n,3] (double)
+ * are DEVICE pointers; cells [B,9] (rows = lattice vectors) and pbc [B,3] are host arrays.
+ * Builds every structure's neighbour list in one pass, with the semantics of s7b_engine_set_positions_host
+ * per structure, and installs the union graph (no cross-structure edges).  Each structure gets the cell-list
+ * grid it would get alone, so its CSR rows are those of s7b_engine_set_positions_host with offsets.  Kernel
+ * launches and host synchronisations do not depend on B.  Bad arguments (atom_ptr, a zero lattice vector or
+ * singular cell along a periodic direction -- the message names the structure) fail before the device is
+ * touched.  The graph lives in engine-owned buffers, so a following call whose edge count stays within
+ * their headroom replays the captured step of s7b_engine_compute. */
+S7B_API int s7b_engine_set_positions_batch(S7bEngine* eng, int32_t n_systems, const int32_t* atom_ptr,
+                                           const int32_t* d_species, const double* d_positions,
+                                           const double* cells9, const int32_t* pbc3,
+                                           int64_t* n_edges_out, void* stream);
+
+/* After s7b_engine_compute on a graph from s7b_engine_set_positions_batch: per-structure energy [B] and
+ * virial [B,6] (xx,yy,zz,xy,yz,zx of -sum r (x) f), fp64, device pointers, deterministic given edge forces.
+ * The energy sums the fp64 per-atom energies (engine buffer "atomic_energy_f64").  Fails when the current
+ * graph was not installed by s7b_engine_set_positions_batch. */
+S7B_API int s7b_engine_system_results(S7bEngine* eng, double* d_energy, double* d_virial, void* stream);
 
 /* Per-kernel timing with CUDA events recorded on the launching stream around every kernel (or
  * kernel group) of the stage sequence; labels like "conv_bwd.t2.l1".  Enable, run steps, then read. */

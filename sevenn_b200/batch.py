@@ -4,8 +4,10 @@ The reference evaluates a batch as one disjoint-union graph: ``AtomGraphSequenti
 ``is_batch_data`` (``sevenn/nn/sequential.py:99-108,143``), per-graph energy from ``AtomReduce``
 (``nn/linear.py:127-141``) and per-graph stress from the per-atom virial scattered by ``batch``
 (``nn/force_output.py:216-228``).  The engine works on any CSR graph, so a batch is the concatenation
-of the per-structure graphs with node offsets; the per-structure reductions run as torch segment sums
-on the device (plumbing).  ``SevenNetModel`` mirrors the TorchSim adapter ``sevenn/torchsim.py:56-292``:
+of the per-structure graphs with node offsets.  ``BatchedEvaluator`` builds it structure by structure from
+host arrays, with torch segment sums for the per-structure results.  ``DeviceBatch`` keeps a batch on the
+device: one batched neighbour list (``s7b_engine_set_positions_batch``) and per-structure energy / virial
+reduced in fp64 by a kernel (``s7b_engine_system_results``).  ``SevenNetModel`` mirrors the TorchSim adapter ``sevenn/torchsim.py:56-292``:
 same constructor keywords, ``forward(state) -> {'energy' [B], 'forces' [n,3], 'stress' [B,3,3]}``
 with the sign / Voigt handling of ``torchsim.py:286-290``.  ``torch_sim`` is not installed here, so
 ``state`` is duck-typed: ``positions, row_vector_cell (or cell), pbc, atomic_numbers, system_idx``.
@@ -89,6 +91,69 @@ class BatchedEvaluator:
         return res
 
 
+class DeviceBatch:
+    """Structures given as flat device-resident arrays, the layout of a TorchSim state, evaluated in one engine
+    pass without a host copy of the positions: only the atom counts, cells and pbc (O(B) values) cross to the
+    host, with one readback per call for the checks."""
+
+    def __init__(self, engine: B200Engine):
+        self.engine = engine
+        torch = engine.torch
+        tm = engine.spec.type_map
+        lut = torch.full((max(tm) + 1,), -1, dtype=torch.int32)
+        for z, s in tm.items():
+            lut[z] = s
+        self._lut = lut.to(engine.device)
+
+    def set_batch(self, numbers, positions, cells, pbc, system_idx):
+        """numbers [n] atomic numbers, positions [n,3], cells [B,3,3] (rows = lattice vectors), pbc (bool, [3] or
+        [B,3]), system_idx [n] (sorted structure index of every atom): torch tensors on any device, or numpy
+        arrays.  Builds the union graph on the device."""
+        eng, torch = self.engine, self.engine.torch
+        dev = eng.device
+        z = torch.as_tensor(numbers).to(dev, torch.int64).reshape(-1)
+        si = torch.as_tensor(system_idx).to(dev, torch.int64).reshape(-1)
+        cells = torch.as_tensor(cells).detach().to('cpu', torch.float64).reshape(-1, 3, 3)
+        B, n = int(cells.shape[0]), int(z.shape[0])
+        if B < 1:
+            raise ValueError('empty batch')
+        if si.shape[0] != n:
+            raise ValueError(f'system_idx has {si.shape[0]} entries for {n} atoms')
+        lut = self._lut
+        known = (z >= 0) & (z < lut.shape[0])
+        species = torch.where(known, lut[z.clamp(0, lut.shape[0] - 1)], -1)
+        # one readback: any unknown atomic number, the first one, system_idx unsorted, out of range; then atom_ptr [B+1]
+        flags = torch.zeros(4, dtype=torch.int64, device=dev)
+        if n > 0:
+            bad = species < 0
+            flags[0] = bad.any()
+            flags[1] = z[bad.to(torch.int8).argmax()]
+            flags[2] = (si[1:] < si[:-1]).any()
+            flags[3] = (si.min() < 0) | (si.max() >= B)
+        counts = torch.bincount(si.clamp(0, B - 1), minlength=B)
+        h = torch.cat([flags, torch.zeros(1, dtype=torch.int64, device=dev), torch.cumsum(counts, 0)]).cpu().numpy()
+        if h[0]:
+            raise ValueError(f'atomic number {int(h[1])} is not known to this model')
+        if h[2]:
+            raise ValueError('system_idx must be sorted')
+        if h[3]:
+            raise ValueError(f'system_idx must lie in [0, {B}): one structure per cell')
+        eng.set_positions_batch(species, positions, h[4:], cells, pbc)
+        return self
+
+    def compute(self, numbers, positions, cells, pbc, system_idx) -> dict:
+        """-> dict of device tensors, as ``BatchedEvaluator.compute``: energy [B] f64 (fp64 sum of the per-atom
+        energies), atomic_energy [n], forces [n,3], virial [B,6] f64 (= -sum r (x) f per structure, order
+        xx,yy,zz,xy,yz,zx), n_edges."""
+        self.set_batch(numbers, positions, cells, pbc, system_idx)
+        eng = self.engine
+        eng.compute()
+        energy, virial = eng.system_results()
+        ae = eng.buffer('atomic_energy', shape=(eng.n_local,)).clone()
+        forces = eng.buffer('forces', shape=(eng.n_nodes, 3)).clone()
+        return dict(energy=energy, atomic_energy=ae, forces=forces, virial=virial, n_edges=eng.n_edges)
+
+
 class SevenNetModel:
     """TorchSim-style model wrapper (``sevenn/torchsim.py:56``): ``model(state)`` evaluates all systems of
     the state in one engine pass."""
@@ -118,7 +183,7 @@ class SevenNetModel:
         self.type_map = self.engine.spec.type_map
         self.modal = None
         self.implemented_properties = ['energy', 'forces', 'stress']
-        self._batch = BatchedEvaluator(self.engine)
+        self._batch = DeviceBatch(self.engine)
 
     @property
     def device(self):
@@ -130,20 +195,11 @@ class SevenNetModel:
 
     def forward(self, state, **kwargs):
         torch = self.engine.torch
-        pos = torch.as_tensor(state.positions).detach().cpu().double().numpy()
         cells = getattr(state, 'row_vector_cell', None)
         if cells is None:   # SimState.cell holds column vectors
             cells = torch.as_tensor(state.cell).transpose(-1, -2)
-        cells = torch.as_tensor(cells).detach().cpu().double().numpy().reshape(-1, 3, 3)
-        numbers = torch.as_tensor(state.atomic_numbers).cpu().numpy()
-        sys_idx = torch.as_tensor(state.system_idx).cpu().numpy()
-        pbc = np.broadcast_to(np.asarray(torch.as_tensor(state.pbc).cpu().numpy(), dtype=bool), (3,))
-        B = int(sys_idx.max()) + 1
-        if np.any(np.diff(sys_idx) < 0):
-            raise ValueError('system_idx must be sorted')
-        systems = [dict(numbers=numbers[sys_idx == b], positions=pos[sys_idx == b], cell=cells[b], pbc=pbc)
-                   for b in range(B)]
-        out = self._batch.compute(systems)
+        cells = torch.as_tensor(cells).detach().to('cpu', torch.float64).reshape(-1, 3, 3).numpy()
+        out = self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
         vol = torch.as_tensor(np.abs(np.linalg.det(cells)), device=self._device)
         s = (out['virial'] / vol[:, None])                      # 'inferred_stress', (xx,yy,zz,xy,yz,zx)
         v = -s[:, [0, 1, 2, 4, 5, 3]]                           # ASE Voigt, sign of torchsim.py:286-290

@@ -49,7 +49,7 @@ struct S7bD3 {
   NLGrid grid;
   int3 R_vdw, R_cn;
   D3Buf r0ab, c6ref, cnref, mxc;
-  D3Buf pos, wrapped, type, key, key_sorted, idx, idx_sorted, bin_start, tmp;
+  D3Buf pos, wrapped, type, key, key_sorted, idx, idx_sorted, bin_start, tmp, grid_dev, batch1, sys;
   D3Buf xs, ts, bin_of, W, dW, logD, near_, cn, dc6i, force, energy, sigma, out_force;
   std::vector<double> host_force;      // reference ABI: pair_get_force returns a pointer
   double host_energy = 0.0, host_sigma[6] = {0, 0, 0, 0, 0, 0};
@@ -96,7 +96,7 @@ void s7b_d3_destroy(S7bD3* d) {
   if (!d) return;
   D3Buf* bufs[] = {&d->r0ab, &d->c6ref, &d->cnref, &d->mxc, &d->pos, &d->wrapped, &d->type, &d->key, &d->key_sorted, &d->idx,
                    &d->idx_sorted, &d->bin_start, &d->tmp, &d->xs, &d->ts, &d->bin_of, &d->W, &d->dW, &d->logD, &d->near_,
-                   &d->cn, &d->dc6i, &d->force, &d->energy, &d->sigma, &d->out_force};
+                   &d->cn, &d->dc6i, &d->force, &d->energy, &d->sigma, &d->out_force, &d->grid_dev, &d->batch1, &d->sys};
   for (D3Buf* b : bufs) b->release();
   delete d;
 }
@@ -203,11 +203,17 @@ int s7b_d3_set_system(S7bD3* d, int32_t n, const int32_t* types, const double* p
   rc |= d->W.ensure(N * 20); rc |= d->dW.ensure(N * 20); rc |= d->logD.ensure(N * 4); rc |= d->near_.ensure(N * 4);
   rc |= d->cn.ensure(N * 8); rc |= d->dc6i.ensure(N * 8); rc |= d->force.ensure(N * 24); rc |= d->out_force.ensure(N * 24);
   rc |= d->energy.ensure(8); rc |= d->sigma.ensure(72);
+  rc |= d->grid_dev.ensure(sizeof(NLGrid)); rc |= d->batch1.ensure(4 * sizeof(int)); rc |= d->sys.ensure(N * 4);
   if (rc) return d3_fail("cudaMalloc failed for the D3 system");
   S7B_CUDA_CHECK(cudaMemcpyAsync(d->pos.p, x.data(), N * 24, cudaMemcpyHostToDevice, st));
   S7B_CUDA_CHECK(cudaMemcpyAsync(d->type.p, types, N * 4, cudaMemcpyHostToDevice, st));
+  // the binning of the model's neighbour list, as a batch of one structure: atom_ptr = {0, n}, bin_off = {0, nbins}
+  const int batch1[4] = {0, n, 0, (int)nbins};
+  S7B_CUDA_CHECK(cudaMemcpyAsync(d->grid_dev.p, &g, sizeof(NLGrid), cudaMemcpyHostToDevice, st));
+  S7B_CUDA_CHECK(cudaMemcpyAsync(d->batch1.p, batch1, sizeof(batch1), cudaMemcpyHostToDevice, st));
   const int blk = 128, grd = (n + blk - 1) / blk;
-  nl_bin_kernel<<<grd, blk, 0, st>>>(g, d->pos.as<double>(), n, d->key.as<int>(), d->idx.as<int>(), d->wrapped.as<double>());
+  nl_bin_kernel<<<grd, blk, 0, st>>>(d->grid_dev.as<NLGrid>(), d->batch1.as<int>(), d->batch1.as<int>() + 2, 1, d->pos.as<double>(), n,
+                                     d->key.as<int>(), d->idx.as<int>(), d->wrapped.as<double>(), d->sys.as<int>());
   S7B_CUDA_CHECK(cudaGetLastError());
   size_t tmp_sort = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, d->key.as<int>(), d->key_sorted.as<int>(), d->idx.as<int>(), d->idx_sorted.as<int>(), n, 0, 32, st);

@@ -173,14 +173,20 @@ struct S7bEngine {
   std::vector<DevBuf> x, g, wbuf, z1, z2, h1, h2;   // per layer (wbuf.. exact-MLP mode only)
   DevBuf mid, h, dh, dg, dx, dwbuf, tmpA, tmpB;
   RowExp re_mid, re_h, re_dg, re_dx;      // row exponents of the tensor-core GEMM inputs
-  DevBuf energy, atomic_energy, forces, virial, atomic_virial;
+  DevBuf energy, atomic_energy, atomic_energy64, forces, virial, atomic_virial;
   bool want_atomic_virial = false;
   // host staging for compute_host
   DevBuf hs_species, hs_rowptr, hs_src, hs_vec, hs_centre, hs_flag;
   // device neighbour list (positions -> CSR)
   DevBuf nl_pos, nl_wrapped, nl_key, nl_key_sorted, nl_idx, nl_idx_sorted, nl_bin_start, nl_count, nl_tmp, nl_centres;
+  DevBuf nl_species, nl_grids, nl_atom_ptr, nl_bin_off, nl_lohi, nl_sys, nl_total;
+  std::vector<NLGrid> nl_grids_host;
+  std::vector<int> nl_bin_off_host;
   int nl_n_centres = 0;
   int64_t nl_n_edges = 0;
+  // structures of the current graph when s7b_engine_set_positions_batch installed it (0 otherwise)
+  int n_systems = 0;
+  DevBuf sys_atom_ptr;
   Profiler prof;
   // side streams: the per-l1 convolution kernels of one layer are independent (disjoint outputs) and
   // stress different units (l1 = 0: L1/L2 latency, l1 >= 1: FP32 pipe), so they are co-scheduled
@@ -891,7 +897,9 @@ void s7b_engine_destroy(S7bEngine* e) {
                     &e->mid, &e->h, &e->dh, &e->dg, &e->dx, &e->dwbuf, &e->tmpA, &e->tmpB, &e->energy,
                     &e->atomic_energy, &e->forces, &e->virial, &e->atomic_virial, &e->hs_species, &e->hs_rowptr, &e->hs_src,
                     &e->hs_vec, &e->hs_centre, &e->hs_flag, &e->nl_pos, &e->nl_wrapped, &e->nl_key, &e->nl_key_sorted,
-                    &e->nl_idx, &e->nl_idx_sorted, &e->nl_bin_start, &e->nl_count, &e->nl_tmp, &e->nl_centres};
+                    &e->nl_idx, &e->nl_idx_sorted, &e->nl_bin_start, &e->nl_count, &e->nl_tmp, &e->nl_centres,
+                    &e->nl_species, &e->nl_grids, &e->nl_atom_ptr, &e->nl_bin_off, &e->nl_lohi, &e->nl_sys, &e->nl_total,
+                    &e->sys_atom_ptr, &e->atomic_energy64};
   for (DevBuf* b : bufs) b->release();
   for (auto* v : {&e->x, &e->g, &e->wbuf, &e->z1, &e->z2, &e->h1, &e->h2})
     for (auto& b : *v) b.release();
@@ -965,6 +973,7 @@ int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t
   e->d_rowptr = d_rowptr;
   e->d_src = d_src;
   e->d_edge_vec = d_edge_vec;
+  e->n_systems = 0;
   const bool table = e->desc.table_knots > 0;
   if (n_edges > e->E_cap || 2 * n_edges < e->E_cap)   // a little headroom, so MD-step fluctuations keep the capacity
     e->E_cap = (n_edges + n_edges / 32 + 1024) / 1024 * 1024;
@@ -1020,6 +1029,7 @@ int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t
   rc |= e->energy.ensure(sizeof(double));
   rc |= e->virial.ensure(6 * sizeof(double));
   rc |= e->atomic_energy.ensure(Nl * sizeof(float));
+  rc |= e->atomic_energy64.ensure(Nl * sizeof(double));
   rc |= e->forces.ensure(Nn * 3 * sizeof(float));
   if (e->want_atomic_virial) rc |= e->atomic_virial.ensure(Nn * 6 * sizeof(float));
   if (rc) return fail("cudaMalloc failed while sizing step buffers");
@@ -1211,7 +1221,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
       if (Nl > 0) {
         const int blk = 256;
         ProfScope ps(e->prof, st, "readout");
-        readout_kernel<<<(Nl * 32 + blk - 1) / blk, blk, 0, st>>>(e->h.as<float>(), wr, gparam(e, "readout_lo"), scale, shift, e->d_species, Nl, L.dim_h, e->atomic_energy.as<float>(), e->energy.as<double>(), e->dh.as<float>());
+        readout_kernel<<<(Nl * 32 + blk - 1) / blk, blk, 0, st>>>(e->h.as<float>(), wr, gparam(e, "readout_lo"), scale, shift, e->d_species, Nl, L.dim_h, e->atomic_energy.as<float>(), e->atomic_energy64.as<double>(), e->energy.as<double>(), e->dh.as<float>());
         S7B_LAUNCH_CHECK();
       }
       return 0;
@@ -1499,6 +1509,7 @@ void* s7b_engine_buffer(S7bEngine* e, const char* name, int layer, size_t* numel
   else if (nm == "energy") { p = e->energy.p; n = 1; }
   else if (nm == "virial") { p = e->virial.p; n = 6; }
   else if (nm == "atomic_energy") { p = e->atomic_energy.p; n = (size_t)e->n_local; }
+  else if (nm == "atomic_energy_f64") { p = e->atomic_energy64.p; n = (size_t)e->n_local; }
   else if (nm == "atomic_virial" && e->want_atomic_virial) { p = e->atomic_virial.p; n = (size_t)e->n_nodes * 6; }
   else if (nm == "forces") { p = e->forces.p; n = (size_t)e->n_nodes * 3; }
   else if (nm == "edge_force") { p = e->fedge.p; n = (size_t)e->n_edges * 3; }
@@ -1572,49 +1583,35 @@ static int invert3(const double* m, double* inv) {
   return 0;
 }
 
-// Neighbour list of `n_centres` centre atoms (centres == nullptr: all n_atoms atoms) against all atoms;
-// leaves species / rowptr [n_centres + 1] / src (indices into the n_atoms atoms) / edge_vec in the hs_* buffers.
-static int build_neighbor_list(S7bEngine* e, int32_t n_atoms, const int32_t* species, const double* positions,
-                               const double* cell9, const int32_t* pbc3, int32_t n_centres, const int32_t* centres_host,
-                               int64_t* n_edges_out, void* stream) {
-  if (!e) return fail("null engine");
-  if (n_atoms < 0 || (n_atoms > 0 && (!species || !positions))) return fail("bad arguments");
-  if (centres_host == nullptr) n_centres = n_atoms;
-  if (n_centres < 0 || n_centres > n_atoms) return fail("bad centre count");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  NLGrid g;
+// Cell-list grid of one structure (b = its index in the batch, for messages), in two steps.  nl_grid_cell:
+// lattice (missing vectors of non-periodic directions completed), inverse and plane heights -- everything
+// that does not depend on the positions.  nl_grid_bins: binned fractional range of the non-periodic
+// directions from the bounding box lo/hi (nullptr: fully periodic or no atoms), bins and search radii.
+static int nl_grid_cell(NLGrid& g, double height[3], const double* cell9, const int32_t* pbc3, double cutoff, int b) {
   memset(&g, 0, sizeof(g));
-  const double cutoff = (double)e->desc.cutoff;
   g.cutoff2 = cutoff * cutoff;
   for (int a = 0; a < 3; ++a) g.pbc[a] = (pbc3 && pbc3[a]) ? 1 : 0;
   for (int k = 0; k < 9; ++k) g.cell[k] = cell9 ? cell9[k] : 0.0;
   for (int a = 0; a < 3; ++a) {      // complete missing lattice vectors of non-periodic directions
     const double* v = g.cell + 3 * a;
     if (v[0] * v[0] + v[1] * v[1] + v[2] * v[2] < 1e-20) {
-      if (g.pbc[a]) return fail("periodic direction with a zero lattice vector");
+      if (g.pbc[a]) return fail("periodic direction with a zero lattice vector (structure " + std::to_string(b) + ")");
       g.cell[3 * a + a] = 1.0;
     }
   }
-  if (invert3(g.cell, g.inv)) return fail("singular cell");
-  // plane spacings
-  double height[3];
+  if (invert3(g.cell, g.inv)) return fail("singular cell (structure " + std::to_string(b) + ")");
   for (int a = 0; a < 3; ++a) {      // |row a of inv^T| = 1 / height_a
     const double nx = g.inv[0 * 3 + a], ny = g.inv[1 * 3 + a], nz = g.inv[2 * 3 + a];
     height[a] = 1.0 / sqrt(nx * nx + ny * ny + nz * nz);
   }
-  // fractional bounding range of non-periodic directions (host pass over the caller's positions)
   for (int a = 0; a < 3; ++a) { g.fmin[a] = 0.0; g.fspan[a] = 1.0; }
-  if (!(g.pbc[0] && g.pbc[1] && g.pbc[2]) && n_atoms > 0) {
-    double lo[3] = {1e300, 1e300, 1e300}, hi[3] = {-1e300, -1e300, -1e300};
-    for (int i = 0; i < n_atoms; ++i)
-      for (int a = 0; a < 3; ++a) {
-        const double f = positions[3 * i] * g.inv[0 * 3 + a] + positions[3 * i + 1] * g.inv[1 * 3 + a] + positions[3 * i + 2] * g.inv[2 * 3 + a];
-        lo[a] = std::min(lo[a], f);
-        hi[a] = std::max(hi[a], f);
-      }
+  return 0;
+}
+
+static long long nl_grid_bins(NLGrid& g, const double height[3], const double* lo, const double* hi, double cutoff) {
+  if (lo)
     for (int a = 0; a < 3; ++a)
       if (!g.pbc[a]) { g.fmin[a] = lo[a]; g.fspan[a] = std::max(hi[a] - lo[a], 1e-9) * (1.0 + 1e-9); }
-  }
   long long nbins = 1;
   for (int a = 0; a < 3; ++a) {
     const double extent = height[a] * g.fspan[a];
@@ -1625,21 +1622,83 @@ static int build_neighbor_list(S7bEngine* e, int32_t n_atoms, const int32_t* spe
     if (g.R[a] < 0) g.R[a] = 0;
     nbins *= nb;
   }
-  if (nbins > (1LL << 26)) return fail("neighbour grid too large");
+  return nbins;
+}
+
+// Neighbour lists of a batch of B structures (atoms of structure b: [atom_ptr[b], atom_ptr[b+1]), host array),
+// species / positions on the device; rows of `n_centres` centre atoms (centres_host == nullptr: all atoms)
+// against the atoms of their own structure.  Leaves species / rowptr [n_centres + 1] / src (indices into all
+// atoms) / edge_vec in the hs_* buffers.  Launches and host synchronisations do not depend on B: one readback of
+// the bounding boxes (only when a structure has a non-periodic direction) and one of the edge total.  Every
+// argument is checked before the device is touched.
+static int build_neighbor_list(S7bEngine* e, int32_t B, const int32_t* atom_ptr, const int32_t* d_species,
+                               const double* d_positions, const double* cells9, const int32_t* pbc3, int32_t n_centres,
+                               const int32_t* centres_host, int64_t* n_edges_out, void* stream) {
+  if (!e) return fail("null engine");
+  if (B < 1 || !atom_ptr) return fail("bad arguments: need at least one structure and atom_ptr");
+  if (atom_ptr[0] != 0) return fail("atom_ptr[0] must be 0");
+  for (int b = 0; b < B; ++b)
+    if (atom_ptr[b + 1] < atom_ptr[b]) return fail("atom_ptr must be non-decreasing (structure " + std::to_string(b) + ")");
+  const int32_t n_atoms = atom_ptr[B];
+  if (n_atoms > 0 && (!d_species || !d_positions)) return fail("bad arguments");
+  if (centres_host == nullptr) n_centres = n_atoms;
+  if (n_centres < 0 || n_centres > n_atoms) return fail("bad centre count");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const double cutoff = (double)e->desc.cutoff;
+  std::vector<NLGrid>& grids = e->nl_grids_host;
+  std::vector<double> heights(3 * (size_t)B);
+  grids.resize(B);
+  bool need_bbox = false;
+  for (int b = 0; b < B; ++b) {
+    if (nl_grid_cell(grids[b], &heights[3 * (size_t)b], cells9 ? cells9 + 9 * (size_t)b : nullptr,
+                     pbc3 ? pbc3 + 3 * (size_t)b : nullptr, cutoff, b)) return 1;
+    need_bbox |= !(grids[b].pbc[0] && grids[b].pbc[1] && grids[b].pbc[2]) && atom_ptr[b + 1] > atom_ptr[b];
+  }
   const size_t N = (size_t)std::max(n_atoms, 1);
   int rc = 0;
-  rc |= e->hs_species.ensure(N * sizeof(int));
-  rc |= e->hs_rowptr.ensure((N + 1) * sizeof(int));
-  rc |= e->nl_pos.ensure(N * 3 * sizeof(double));
+  rc |= e->nl_grids.ensure((size_t)B * sizeof(NLGrid));
+  rc |= e->nl_atom_ptr.ensure(((size_t)B + 1) * sizeof(int));
+  rc |= e->nl_bin_off.ensure(((size_t)B + 1) * sizeof(int));
+  rc |= e->nl_lohi.ensure((size_t)B * 6 * sizeof(double));
+  rc |= e->nl_sys.ensure(N * sizeof(int));
   rc |= e->nl_wrapped.ensure(N * 3 * sizeof(double));
   rc |= e->nl_key.ensure(N * sizeof(int));
   rc |= e->nl_key_sorted.ensure(N * sizeof(int));
   rc |= e->nl_idx.ensure(N * sizeof(int));
   rc |= e->nl_idx_sorted.ensure(N * sizeof(int));
-  rc |= e->nl_bin_start.ensure(((size_t)nbins + 1) * sizeof(int));
   rc |= e->nl_count.ensure((N + 1) * sizeof(int));
+  rc |= e->nl_total.ensure(sizeof(int64_t));
   rc |= e->nl_centres.ensure(N * sizeof(int));
   if (rc) return fail("cudaMalloc failed for the neighbour list");
+  S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_atom_ptr.p, atom_ptr, ((size_t)B + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  std::vector<double> lohi;
+  if (need_bbox) {    // fractional bounding boxes of all structures, one launch and one readback
+    S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_grids.p, grids.data(), (size_t)B * sizeof(NLGrid), cudaMemcpyHostToDevice, st));
+    nl_bbox_kernel<<<B, 256, 0, st>>>(e->nl_grids.as<NLGrid>(), e->nl_atom_ptr.as<int>(), d_positions, e->nl_lohi.as<double>());
+    S7B_LAUNCH_CHECK();
+    lohi.resize(6 * (size_t)B);
+    S7B_CUDA_CHECK(cudaMemcpyAsync(lohi.data(), e->nl_lohi.p, lohi.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    S7B_CUDA_CHECK(cudaStreamSynchronize(st));
+  }
+  std::vector<int>& bin_off = e->nl_bin_off_host;
+  bin_off.assign((size_t)B + 1, 0);
+  long long nbins = 0;
+  for (int b = 0; b < B; ++b) {
+    NLGrid& g = grids[b];
+    const bool box = need_bbox && !(g.pbc[0] && g.pbc[1] && g.pbc[2]) && atom_ptr[b + 1] > atom_ptr[b];
+    double lo[3], hi[3];
+    for (int a = 0; a < 3; ++a) { lo[a] = box ? lohi[6 * (size_t)b + 2 * a] : 0.0; hi[a] = box ? lohi[6 * (size_t)b + 2 * a + 1] : 0.0; }
+    const long long nb = nl_grid_bins(g, &heights[3 * (size_t)b], box ? lo : nullptr, box ? hi : nullptr, cutoff);
+    if (nb > (1LL << 26)) return fail("neighbour grid too large (structure " + std::to_string(b) + ")");
+    nbins += nb;
+    if (nbins > (1LL << 26)) return fail("neighbour grids of the batch too large: more than 2^26 bins in all");
+    bin_off[b + 1] = (int)nbins;
+  }
+  if (e->nl_bin_start.ensure(((size_t)nbins + 1) * sizeof(int)) || e->hs_species.ensure(N * sizeof(int)) ||
+      e->hs_rowptr.ensure((N + 1) * sizeof(int)))
+    return fail("cudaMalloc failed for the neighbour list");
+  S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_grids.p, grids.data(), (size_t)B * sizeof(NLGrid), cudaMemcpyHostToDevice, st));
+  S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_bin_off.p, bin_off.data(), ((size_t)B + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
   int64_t n_edges = 0;
   const int* d_centres = nullptr;
   if (centres_host != nullptr && n_centres > 0) {
@@ -1647,35 +1706,43 @@ static int build_neighbor_list(S7bEngine* e, int32_t n_atoms, const int32_t* spe
     d_centres = e->nl_centres.as<int>();
   }
   if (n_atoms > 0) {
-    S7B_CUDA_CHECK(cudaMemcpyAsync(e->hs_species.p, species, (size_t)n_atoms * sizeof(int), cudaMemcpyHostToDevice, st));
-    S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_pos.p, positions, (size_t)n_atoms * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (d_species != e->hs_species.as<int>())
+      S7B_CUDA_CHECK(cudaMemcpyAsync(e->hs_species.p, d_species, (size_t)n_atoms * sizeof(int), cudaMemcpyDeviceToDevice, st));
     const int blk = 128, grd = (n_atoms + blk - 1) / blk;
-    nl_bin_kernel<<<grd, blk, 0, st>>>(g, e->nl_pos.as<double>(), n_atoms, e->nl_key.as<int>(), e->nl_idx.as<int>(), e->nl_wrapped.as<double>());
+    const NLGrid* d_grids = e->nl_grids.as<NLGrid>();
+    const int* d_bin_off = e->nl_bin_off.as<int>();
+    nl_bin_kernel<<<grd, blk, 0, st>>>(d_grids, e->nl_atom_ptr.as<int>(), d_bin_off, B, d_positions, n_atoms, e->nl_key.as<int>(),
+                                       e->nl_idx.as<int>(), e->nl_wrapped.as<double>(), e->nl_sys.as<int>());
     S7B_LAUNCH_CHECK();
-    size_t tmp_sort = 0, tmp_scan = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, e->nl_key.as<int>(), e->nl_key_sorted.as<int>(), e->nl_idx.as<int>(), e->nl_idx_sorted.as<int>(), n_atoms, 0, 32, st);
+    int end_bit = 1;                   // keys are < nbins <= 2^26
+    while ((1LL << end_bit) < nbins) ++end_bit;
+    size_t tmp_sort = 0, tmp_scan = 0, tmp_sum = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, e->nl_key.as<int>(), e->nl_key_sorted.as<int>(), e->nl_idx.as<int>(), e->nl_idx_sorted.as<int>(), n_atoms, 0, end_bit, st);
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, e->nl_count.as<int>(), e->hs_rowptr.as<int>(), n_atoms + 1, st);
-    if (e->nl_tmp.ensure(std::max(tmp_sort, tmp_scan) + 256)) return fail("cudaMalloc failed for cub workspace");
+    cub::DeviceReduce::Sum(nullptr, tmp_sum, e->nl_count.as<int>(), e->nl_total.as<int64_t>(), n_atoms, st);
+    if (e->nl_tmp.ensure(std::max(std::max(tmp_sort, tmp_scan), tmp_sum) + 256)) return fail("cudaMalloc failed for cub workspace");
     size_t tmp = e->nl_tmp.bytes;
-    S7B_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(e->nl_tmp.p, tmp, e->nl_key.as<int>(), e->nl_key_sorted.as<int>(), e->nl_idx.as<int>(), e->nl_idx_sorted.as<int>(), n_atoms, 0, 32, st));
+    S7B_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(e->nl_tmp.p, tmp, e->nl_key.as<int>(), e->nl_key_sorted.as<int>(), e->nl_idx.as<int>(), e->nl_idx_sorted.as<int>(), n_atoms, 0, end_bit, st));
     ++g_launches;
     nl_bin_start_kernel<<<(n_atoms + 1 + 255) / 256, 256, 0, st>>>(e->nl_key_sorted.as<int>(), n_atoms, (int)nbins, e->nl_bin_start.as<int>());
     S7B_LAUNCH_CHECK();
     S7B_CUDA_CHECK(cudaMemsetAsync(e->nl_count.p, 0, ((size_t)n_atoms + 1) * sizeof(int), st));
     const int grd_c = std::max(1, (n_centres + blk - 1) / blk);
-    nl_pairs_kernel<false><<<grd_c, blk, 0, st>>>(g, e->nl_wrapped.as<double>(), e->nl_key.as<int>(), e->nl_idx_sorted.as<int>(), e->nl_bin_start.as<int>(), n_centres, e->nl_count.as<int>(), nullptr, nullptr, nullptr, d_centres);
+    nl_pairs_kernel<false><<<grd_c, blk, 0, st>>>(d_grids, d_bin_off, e->nl_sys.as<int>(), e->nl_wrapped.as<double>(), e->nl_key.as<int>(), e->nl_idx_sorted.as<int>(), e->nl_bin_start.as<int>(), n_centres, e->nl_count.as<int>(), nullptr, nullptr, nullptr, d_centres);
     S7B_LAUNCH_CHECK();
     tmp = e->nl_tmp.bytes;
     S7B_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(e->nl_tmp.p, tmp, e->nl_count.as<int>(), e->hs_rowptr.as<int>(), n_centres + 1, st));
     ++g_launches;
-    int total = 0;
-    S7B_CUDA_CHECK(cudaMemcpyAsync(&total, e->hs_rowptr.as<int>() + n_centres, sizeof(int), cudaMemcpyDeviceToHost, st));
+    tmp = e->nl_tmp.bytes;             // the int32 scan wraps past 2^31 edges: the total is also summed in int64
+    S7B_CUDA_CHECK(cub::DeviceReduce::Sum(e->nl_tmp.p, tmp, e->nl_count.as<int>(), e->nl_total.as<int64_t>(), n_centres, st));
+    ++g_launches;
+    S7B_CUDA_CHECK(cudaMemcpyAsync(&n_edges, e->nl_total.p, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     S7B_CUDA_CHECK(cudaStreamSynchronize(st));
-    n_edges = total;
+    if (n_edges >= ((int64_t)1 << 31)) return fail("more than 2^31-1 edges per GPU are not supported");
     const size_t E = (size_t)std::max<int64_t>(n_edges, 1);
     if (e->hs_src.ensure(E * sizeof(int)) || e->hs_vec.ensure(E * 3 * sizeof(float))) return fail("cudaMalloc failed for the edge list");
     if (n_edges > 0) {
-      nl_pairs_kernel<true><<<grd_c, blk, 0, st>>>(g, e->nl_wrapped.as<double>(), e->nl_key.as<int>(), e->nl_idx_sorted.as<int>(), e->nl_bin_start.as<int>(), n_centres, nullptr, e->hs_rowptr.as<int>(), e->hs_src.as<int>(), e->hs_vec.as<float>(), d_centres);
+      nl_pairs_kernel<true><<<grd_c, blk, 0, st>>>(d_grids, d_bin_off, e->nl_sys.as<int>(), e->nl_wrapped.as<double>(), e->nl_key.as<int>(), e->nl_idx_sorted.as<int>(), e->nl_bin_start.as<int>(), n_centres, nullptr, e->hs_rowptr.as<int>(), e->hs_src.as<int>(), e->hs_vec.as<float>(), d_centres);
       S7B_LAUNCH_CHECK();
     }
   } else {
@@ -1685,6 +1752,24 @@ static int build_neighbor_list(S7bEngine* e, int32_t n_atoms, const int32_t* spe
   e->nl_n_edges = n_edges;
   if (n_edges_out) *n_edges_out = n_edges;
   return 0;
+}
+
+// The host-array entry points are a batch of one: positions / species are uploaded to scratch buffers first.
+static int build_neighbor_list_host(S7bEngine* e, int32_t n_atoms, const int32_t* species, const double* positions,
+                                    const double* cell9, const int32_t* pbc3, int32_t n_centres, const int32_t* centres_host,
+                                    int64_t* n_edges_out, void* stream) {
+  if (!e) return fail("null engine");
+  if (n_atoms < 0 || (n_atoms > 0 && (!species || !positions))) return fail("bad arguments");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t N = (size_t)std::max(n_atoms, 1);
+  if (e->nl_pos.ensure(N * 3 * sizeof(double)) || e->nl_species.ensure(N * sizeof(int))) return fail("cudaMalloc failed for the neighbour list");
+  if (n_atoms > 0) {
+    S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_species.p, species, (size_t)n_atoms * sizeof(int), cudaMemcpyHostToDevice, st));
+    S7B_CUDA_CHECK(cudaMemcpyAsync(e->nl_pos.p, positions, (size_t)n_atoms * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  }
+  const int32_t atom_ptr[2] = {0, n_atoms};
+  return build_neighbor_list(e, 1, atom_ptr, e->nl_species.as<int>(), e->nl_pos.as<double>(), cell9, pbc3, n_centres,
+                             centres_host, n_edges_out, stream);
 }
 
 // ---- host-staged pieces of the stage protocol (a LAMMPS pair style without CUDA headers: pair_e3gnn_parallel.cpp
@@ -1768,8 +1853,34 @@ int s7b_engine_read_scalars_host(S7bEngine* e, double* energy, double* virial6, 
 int s7b_engine_set_positions_host(S7bEngine* e, int32_t n_atoms, const int32_t* species, const double* positions,
                                   const double* cell9, const int32_t* pbc3, void* stream) {
   int64_t n_edges = 0;
-  if (build_neighbor_list(e, n_atoms, species, positions, cell9, pbc3, n_atoms, nullptr, &n_edges, stream)) return 1;
+  if (build_neighbor_list_host(e, n_atoms, species, positions, cell9, pbc3, n_atoms, nullptr, &n_edges, stream)) return 1;
   return s7b_engine_set_graph(e, n_atoms, n_atoms, n_edges, e->hs_species.as<int>(), e->hs_rowptr.as<int>(), e->hs_src.as<int>(), e->hs_vec.as<float>(), stream);
+}
+
+int s7b_engine_set_positions_batch(S7bEngine* e, int32_t n_systems, const int32_t* atom_ptr, const int32_t* d_species,
+                                   const double* d_positions, const double* cells9, const int32_t* pbc3,
+                                   int64_t* n_edges_out, void* stream) {
+  int64_t n_edges = 0;
+  if (build_neighbor_list(e, n_systems, atom_ptr, d_species, d_positions, cells9, pbc3, 0, nullptr, &n_edges, stream)) return 1;
+  const int32_t n = atom_ptr[n_systems];
+  if (e->sys_atom_ptr.ensure(((size_t)n_systems + 1) * sizeof(int))) return fail("cudaMalloc failed");
+  if (s7b_engine_set_graph(e, n, n, n_edges, e->hs_species.as<int>(), e->hs_rowptr.as<int>(), e->hs_src.as<int>(), e->hs_vec.as<float>(), stream)) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  S7B_CUDA_CHECK(cudaMemcpyAsync(e->sys_atom_ptr.p, e->nl_atom_ptr.p, ((size_t)n_systems + 1) * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  e->n_systems = n_systems;
+  if (n_edges_out) *n_edges_out = n_edges;
+  return 0;
+}
+
+int s7b_engine_system_results(S7bEngine* e, double* d_energy, double* d_virial, void* stream) {
+  if (!e) return fail("null engine");
+  if (e->n_systems < 1) return fail("the current graph was not built by s7b_engine_set_positions_batch");
+  if (!d_energy || !d_virial) return fail("null output");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  system_sums_kernel<<<e->n_systems, kSysBlock, 0, st>>>(e->sys_atom_ptr.as<int>(), e->d_rowptr, e->atomic_energy64.as<double>(),
+                                                         e->d_edge_vec, e->fedge.as<float>(), d_energy, d_virial);
+  S7B_LAUNCH_CHECK();
+  return 0;
 }
 
 // Multi-GPU front-end (SURVEY 8(f), pair_e3gnn_parallel.cpp:194-340): the rows of a SUBSET of centre atoms
@@ -1780,7 +1891,7 @@ int s7b_engine_neighbor_rows_host(S7bEngine* e, int32_t n_atoms, const int32_t* 
                                   const double* cell9, const int32_t* pbc3, int32_t n_centres, const int32_t* centres,
                                   int64_t* n_edges_out, void* stream) {
   if (!centres && n_centres > 0) return fail("null centre list");
-  return build_neighbor_list(e, n_atoms, species, positions, cell9, pbc3, n_centres, centres, n_edges_out, stream);
+  return build_neighbor_list_host(e, n_atoms, species, positions, cell9, pbc3, n_centres, centres, n_edges_out, stream);
 }
 
 int s7b_engine_compute_positions_host(S7bEngine* e, int32_t n_atoms, const int32_t* species, const double* positions,

@@ -36,11 +36,66 @@ __device__ __forceinline__ void nl_frac(const NLGrid& g, const double* p, double
   for (int a = 0; a < 3; ++a) f[a] = p[0] * g.inv[0 * 3 + a] + p[1] * g.inv[1 * 3 + a] + p[2] * g.inv[2 * 3 + a];
 }
 
-// bin key per atom + wrapped cartesian position
-static __global__ void nl_bin_kernel(const NLGrid g, const double* __restrict__ pos, int n, int* __restrict__ key,
-                              int* __restrict__ idx, double* __restrict__ wrapped) {
+// A batch is B independent structures; the atoms of structure b are [atom_ptr[b], atom_ptr[b+1]) and its bins
+// are [bin_off[b], bin_off[b+1]) of one key space, so one stable sort and one bin_start cover the whole batch
+// and no bin holds atoms of two structures.  A single structure is a batch of one.
+
+// structure of atom i: the last b with atom_ptr[b] <= i (empty structures are skipped)
+__device__ __forceinline__ int nl_system_of(const int* __restrict__ atom_ptr, int B, int i) {
+  int lo = 0, hi = B;   // atom_ptr[lo] <= i < atom_ptr[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(atom_ptr + mid) <= i) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// Fractional bounding box [B, 6] = (lo_a, hi_a) per direction of every structure, one block per structure.
+// Each fractional coordinate is rounded as the plain host expression p0*i0a + p1*i1a + p2*i2a (no FMA
+// contraction), so a structure's grid does not depend on where or with what its bounding box was taken.
+static __global__ void nl_bbox_kernel(const NLGrid* __restrict__ grids, const int* __restrict__ atom_ptr,
+                                      const double* __restrict__ pos, double* __restrict__ lohi) {
+  const int b = blockIdx.x;
+  const int a0 = atom_ptr[b], a1 = atom_ptr[b + 1];
+  const double* inv = grids[b].inv;
+  double lo[3] = {1e300, 1e300, 1e300}, hi[3] = {-1e300, -1e300, -1e300};
+  for (int i = a0 + threadIdx.x; i < a1; i += blockDim.x) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const double f = __dadd_rn(__dadd_rn(__dmul_rn(pos[3 * i], inv[0 * 3 + a]), __dmul_rn(pos[3 * i + 1], inv[1 * 3 + a])),
+                                 __dmul_rn(pos[3 * i + 2], inv[2 * 3 + a]));
+      lo[a] = f < lo[a] ? f : lo[a];
+      hi[a] = f > hi[a] ? f : hi[a];
+    }
+  }
+  __shared__ double sm[6][256];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) { sm[2 * a][threadIdx.x] = lo[a]; sm[2 * a + 1][threadIdx.x] = hi[a]; }
+  __syncthreads();
+  for (int s = blockDim.x >> 1; s > 0; s >>= 1) {
+    if (threadIdx.x < s) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        const double l = sm[2 * a][threadIdx.x + s], h = sm[2 * a + 1][threadIdx.x + s];
+        if (l < sm[2 * a][threadIdx.x]) sm[2 * a][threadIdx.x] = l;
+        if (h > sm[2 * a + 1][threadIdx.x]) sm[2 * a + 1][threadIdx.x] = h;
+      }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x < 6) lohi[6 * (size_t)b + threadIdx.x] = sm[threadIdx.x][0];
+}
+
+// bin key per atom (bin_off[b] + local bin) + wrapped cartesian position + structure index
+static __global__ void nl_bin_kernel(const NLGrid* __restrict__ grids, const int* __restrict__ atom_ptr,
+                                     const int* __restrict__ bin_off, int B, const double* __restrict__ pos, int n,
+                                     int* __restrict__ key, int* __restrict__ idx, double* __restrict__ wrapped,
+                                     int* __restrict__ sys) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  const int sb = nl_system_of(atom_ptr, B, i);
+  const NLGrid g = grids[sb];
   const double p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
   double f[3];
   nl_frac(g, p, f);
@@ -53,8 +108,9 @@ static __global__ void nl_bin_kernel(const NLGrid g, const double* __restrict__ 
   }
 #pragma unroll
   for (int c = 0; c < 3; ++c) wrapped[3 * i + c] = f[0] * g.cell[0 * 3 + c] + f[1] * g.cell[1 * 3 + c] + f[2] * g.cell[2 * 3 + c];
-  key[i] = (b[0] * g.nb[1] + b[1]) * g.nb[2] + b[2];
+  key[i] = bin_off[sb] + (b[0] * g.nb[1] + b[1]) * g.nb[2] + b[2];
   idx[i] = i;
+  sys[i] = sb;
 }
 
 // first sorted position of every bin (bin_start[nbins] = n)
@@ -69,17 +125,22 @@ static __global__ void nl_bin_start_kernel(const int* __restrict__ key_sorted, i
 // One thread per centre atom (centre c = centres[tid], or tid itself when centres == nullptr; original
 // numbering).  FILL = false: count[tid] = neighbours; FILL = true: write src / edge_vec at rowptr[tid] +
 // running offset.  A centre subset is what a rank of the multi-GPU runner asks for: the rows of its own atoms.
+// Only the centre's own structure's bins are visited, so a batch has no cross-structure edges.
 template <bool FILL>
-__global__ void nl_pairs_kernel(const NLGrid g, const double* __restrict__ wrapped, const int* __restrict__ key,
-                                const int* __restrict__ idx_sorted, const int* __restrict__ bin_start, int n,
-                                int* __restrict__ count, const int* __restrict__ rowptr,
-                                int* __restrict__ src, float* __restrict__ edge_vec,
+__global__ void nl_pairs_kernel(const NLGrid* __restrict__ grids, const int* __restrict__ bin_off,
+                                const int* __restrict__ sys, const double* __restrict__ wrapped,
+                                const int* __restrict__ key, const int* __restrict__ idx_sorted,
+                                const int* __restrict__ bin_start, int n, int* __restrict__ count,
+                                const int* __restrict__ rowptr, int* __restrict__ src, float* __restrict__ edge_vec,
                                 const int* __restrict__ centres = nullptr) {
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
   if (tid >= n) return;
   const int i = centres != nullptr ? centres[tid] : tid;
+  const int sb = sys[i];
+  const NLGrid g = grids[sb];
+  const int boff = bin_off[sb];
   const double xi = wrapped[3 * i], yi = wrapped[3 * i + 1], zi = wrapped[3 * i + 2];
-  const int k = key[i];
+  const int k = key[i] - boff;
   const int b2 = k % g.nb[2], b1 = (k / g.nb[2]) % g.nb[1], b0 = k / (g.nb[2] * g.nb[1]);
   int out = FILL ? rowptr[tid] : 0;
   for (int d0 = -g.R[0]; d0 <= g.R[0]; ++d0) {
@@ -97,7 +158,7 @@ __global__ void nl_pairs_kernel(const NLGrid g, const double* __restrict__ wrapp
         const double sx = s0 * g.cell[0] + s1 * g.cell[3] + s2 * g.cell[6];
         const double sy = s0 * g.cell[1] + s1 * g.cell[4] + s2 * g.cell[7];
         const double sz = s0 * g.cell[2] + s1 * g.cell[5] + s2 * g.cell[8];
-        const int nbin = (q0 * g.nb[1] + q1) * g.nb[2] + q2;
+        const int nbin = boff + (q0 * g.nb[1] + q1) * g.nb[2] + q2;
         const bool same_image = (s0 == 0 && s1 == 0 && s2 == 0);
         for (int s = bin_start[nbin]; s < bin_start[nbin + 1]; ++s) {
           const int j = idx_sorted[s];
@@ -117,6 +178,41 @@ __global__ void nl_pairs_kernel(const NLGrid g, const double* __restrict__ wrapp
     }
   }
   if (!FILL) count[tid] = out;
+}
+
+// Per-structure results of a batch, one block per structure, in a fixed order (deterministic): energy[b] = sum
+// of the fp64 per-atom energies of [atom_ptr[b], atom_ptr[b+1]); virial[b] = -sum over the structure's edges
+// [rowptr[atom_ptr[b]], rowptr[atom_ptr[b+1]]) of (r_x f_x, r_y f_y, r_z f_z, r_x f_y, r_y f_z, r_z f_x), each
+// product in double.  The edges of a structure are contiguous: the CSR is by centre and structures are
+// contiguous atom ranges.
+constexpr int kSysBlock = 256;
+static __global__ void __launch_bounds__(kSysBlock) system_sums_kernel(
+    const int* __restrict__ atom_ptr, const int* __restrict__ rowptr, const double* __restrict__ atomic_energy,
+    const float* __restrict__ edge_vec, const float* __restrict__ fedge, double* __restrict__ energy,
+    double* __restrict__ virial) {
+  const int b = blockIdx.x;
+  const int a0 = atom_ptr[b], a1 = atom_ptr[b + 1];
+  const int e0 = rowptr[a0], e1 = rowptr[a1];
+  double v[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int i = a0 + threadIdx.x; i < a1; i += kSysBlock) v[0] += atomic_energy[i];
+  for (int k = e0 + threadIdx.x; k < e1; k += kSysBlock) {
+    const double rx = edge_vec[3 * (size_t)k], ry = edge_vec[3 * (size_t)k + 1], rz = edge_vec[3 * (size_t)k + 2];
+    const double fx = fedge[3 * (size_t)k], fy = fedge[3 * (size_t)k + 1], fz = fedge[3 * (size_t)k + 2];
+    v[1] += rx * fx; v[2] += ry * fy; v[3] += rz * fz;
+    v[4] += rx * fy; v[5] += ry * fz; v[6] += rz * fx;
+  }
+  __shared__ double sm[7][kSysBlock];
+#pragma unroll
+  for (int q = 0; q < 7; ++q) sm[q][threadIdx.x] = v[q];
+  __syncthreads();
+  for (int s = kSysBlock >> 1; s > 0; s >>= 1) {
+    if (threadIdx.x < s)
+#pragma unroll
+      for (int q = 0; q < 7; ++q) sm[q][threadIdx.x] += sm[q][threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) energy[b] = sm[0][0];
+  if (threadIdx.x < 6) virial[6 * (size_t)b + threadIdx.x] = -sm[1 + threadIdx.x][0];
 }
 
 }  // namespace s7b

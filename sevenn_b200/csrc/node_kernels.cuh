@@ -373,8 +373,8 @@ __global__ void readout_kernel(const float* __restrict__ h, const float* __restr
                                const float* __restrict__ wr_lo,
                                const float* __restrict__ scale, const float* __restrict__ shift,
                                const int* __restrict__ species, int n_nodes, int width,
-                               float* __restrict__ atomic_energy, double* __restrict__ energy,
-                               float* __restrict__ dh) {
+                               float* __restrict__ atomic_energy, double* __restrict__ atomic_energy64,
+                               double* __restrict__ energy, float* __restrict__ dh) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   double e_atom = 0.0;
@@ -394,6 +394,7 @@ __global__ void readout_kernel(const float* __restrict__ h, const float* __restr
     const double ea = fma((double)sc, acc, (double)__ldg(shift + s));
     if (lane == 0) {
       atomic_energy[warp] = (float)ea;
+      atomic_energy64[warp] = ea;
       e_atom = ea;
     }
   }

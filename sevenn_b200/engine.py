@@ -59,6 +59,7 @@ EXPORTS = [
     's7b_engine_read_rows_host', 's7b_engine_write_rows_host', 's7b_engine_read_scalars_host', 's7b_engine_set_profiling',
     's7b_engine_profile_count', 's7b_engine_profile_entry', 's7b_conv_plan_create',
     's7b_conv_plan_destroy', 's7b_conv_plan_dims', 's7b_conv_forward', 's7b_conv_backward',
+    's7b_engine_set_positions_batch', 's7b_engine_system_results',
 ]
 
 
@@ -108,6 +109,8 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_compute_host.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.s7b_engine_set_positions_host.argtypes = [vp, i32, vp, vp, vp, vp, vp]
     lib.s7b_engine_compute_positions_host.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.s7b_engine_set_positions_batch.argtypes = [vp, i32, vp, vp, vp, vp, vp, ctypes.POINTER(i64), vp]
+    lib.s7b_engine_system_results.argtypes = [vp, vp, vp, vp]
     lib.s7b_engine_set_profiling.argtypes = [vp, ctypes.c_int]
     lib.s7b_engine_profile_count.argtypes = [vp]
     lib.s7b_engine_profile_entry.argtypes = [vp, ctypes.c_int, ctypes.c_char_p, sz,
@@ -293,6 +296,11 @@ def model_desc(spec: ModelSpec, knots: int) -> S7bModelDesc:
             d.muls[t][l] = m
     d.table_knots = knots
     return d
+
+
+def _host(a):
+    """numpy view of a host array, or a host copy of a torch tensor on any device"""
+    return a.detach().cpu().numpy() if hasattr(a, 'detach') else np.asarray(a)
 
 
 class _DevView:
@@ -512,6 +520,44 @@ class B200Engine:
         self.lib.s7b_engine_buffer(self._h, b'graph_src', 0, ctypes.byref(n))
         self.n_edges = int(n.value)
         return self
+
+    def set_positions_batch(self, species, positions, atom_ptr, cells, pbc):
+        """Neighbour lists of B structures built in one pass on the device, installed as one union graph (C ABI
+        ``s7b_engine_set_positions_batch``).  species [n] (indices), positions [n,3], atom_ptr [B+1] (atoms of
+        structure b: [atom_ptr[b], atom_ptr[b+1])), cells [B,3,3] (rows = lattice vectors, zeros where a structure
+        has none), pbc broadcastable to [B,3]: torch tensors on any device, or numpy arrays.  Species and
+        positions go to (or stay on) the device; atom_ptr, cells and pbc are read on the host."""
+        torch = self.torch
+        ap = np.ascontiguousarray(_host(atom_ptr), dtype=np.int32).ravel()
+        B = len(ap) - 1
+        if B < 1:
+            raise ValueError('atom_ptr needs B + 1 >= 2 entries')
+        c = np.ascontiguousarray(_host(cells), dtype=np.float64).reshape(B, 9)
+        pb = np.ascontiguousarray(np.broadcast_to(np.asarray(_host(pbc), dtype=bool), (B, 3)).astype(np.int32))
+        sp = torch.as_tensor(species).detach().to(self.device, torch.int32).contiguous().reshape(-1)
+        pos = torch.as_tensor(positions).detach().to(self.device, torch.float64).contiguous().reshape(-1, 3)
+        if sp.shape[0] != pos.shape[0] or sp.shape[0] != int(ap[-1]):
+            raise ValueError(f'species ({sp.shape[0]}) and positions ({pos.shape[0]}) need atom_ptr[-1] = {int(ap[-1])} rows')
+        ne = ctypes.c_int64()
+        with torch.cuda.device(self.device):
+            check(self.lib.s7b_engine_set_positions_batch(self._h, B, ap.ctypes.data, sp.data_ptr(), pos.data_ptr(),
+                                                          c.ctypes.data, pb.ctypes.data, ctypes.byref(ne), self._stream()))
+        self._graph = dict(perm=None, n_systems=B)
+        self.n_nodes = self.n_local = int(ap[-1])
+        self.n_edges = int(ne.value)
+        return self
+
+    def system_results(self):
+        """(energy [B], virial [B,6]) float64 device tensors of the last ``compute`` on a graph from
+        ``set_positions_batch``: fp64 sums of the per-atom energies, virial = -sum r (x) f per structure
+        (xx,yy,zz,xy,yz,zx).  C ABI ``s7b_engine_system_results``."""
+        torch = self.torch
+        B = (self._graph or {}).get('n_systems', 0)
+        energy = torch.empty(B, dtype=torch.float64, device=self.device)
+        virial = torch.empty(B, 6, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self.lib.s7b_engine_system_results(self._h, energy.data_ptr(), virial.data_ptr(), self._stream()))
+        return energy, virial
 
     def neighbor_rows(self, species, positions, cell, pbc, centres):
         """Device neighbour rows of the atoms `centres` (indices) against all atoms: torch views
