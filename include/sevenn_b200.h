@@ -297,15 +297,38 @@ S7B_API int s7b_d3_set_params(S7bD3* d3, int32_t ntypes, const double* rcov, con
 /* damping: 0 = zero, 1 = Becke-Johnson; cutoffs are squared distances in bohr^2 (reference defaults 9000 / 1600) */
 S7B_API int s7b_d3_set_damping(S7bD3* d3, int32_t damping, double s6, double s8, double a1, double a2, double alp6,
                                double alp8, double vdw_cutoff_au2, double cn_cutoff_au2);
+/* types / positions / cell9 / pbc3 are host arrays; they are copied before the call returns (it synchronises stream) */
 S7B_API int s7b_d3_set_system(S7bD3* d3, int32_t n_atoms, const int32_t* types, const double* positions,
                               const double* cell9, const int32_t* pbc3, void* stream);
 S7B_API int s7b_d3_run_stage(S7bD3* d3, int32_t stage, int32_t i_begin, int32_t i_end, void* stream);
 /* device buffers in bin-sorted order: "cn", "dc6i" double[n]; "force" double[n,3] (hartree/bohr); "energy"
- * double[1]; "sigma" double[6]; "order" int32[n] (sorted position -> caller's atom index) */
+ * double[B]; "sigma" double[B,6]; "order" int32[n] (sorted position -> caller's atom index); "type" int32[n] (after
+ * s7b_d3_set_system_batch: Z - 1 | local type << 8, the local type being the rank of Z among the elements of the
+ * atom's structure; after s7b_d3_set_system: the type index).  B = 1 after
+ * s7b_d3_set_system.  Stage 2 sets energy / sigma to the pair sums of its range, stage 3 adds its virial. */
 S7B_API void* s7b_d3_buffer(S7bD3* d3, const char* name, size_t* numel);
-/* energy (eV), forces [n,3] (eV/A, caller's atom order), sigma6 (eV: xx,yy,zz,xy,xz,yz of sum f (x) r) */
+/* energy (eV), forces [n,3] (eV/A, caller's atom order), sigma6 (eV: xx,yy,zz,xy,xz,yz of sum f (x) r); one structure */
 S7B_API int s7b_d3_results_host(S7bD3* d3, double* energy, double* forces, double* sigma6, void* stream);
 S7B_API int s7b_d3_compute_host(S7bD3* d3, double* energy, double* forces, double* sigma6, void* stream);
+
+/* Batches.  The full element tables, rows indexed by Z - 1: rcov [94], r2r4 [94], r0ab [94*94] (Angstrom),
+ * c6ref [94*94*25], cnref [94*5], mxc [94].  Uploaded once per handle. */
+S7B_API int s7b_d3_set_element_tables(S7bD3* d3, const double* rcov, const double* r2r4, const double* r0ab,
+                                      const double* c6ref, const double* cnref, const int32_t* mxc);
+/* B structures in one pass: atoms of structure b are [atom_ptr[b], atom_ptr[b+1]) (host, [B+1]); d_numbers (device
+ * int32 [n], atomic numbers 1..94) and d_positions (device double [n,3], Angstrom) stay on the device; cells9 (host
+ * double [B,9], rows) and pbc3 (host int32 [B,3]).  Every structure has its own cell list, wrap and local element
+ * types (at most 16 elements per structure, any number in the batch).  Empty structures are allowed and give zeros.
+ * An atomic number outside 1..94, more than 16 elements in a structure, a singular cell or a decreasing atom_ptr is
+ * refused with a message naming the structure, before the current system is touched.  One small readback.  Then run
+ * the three stages over [0, n). */
+S7B_API int s7b_d3_set_system_batch(S7bD3* d3, int32_t n_systems, const int32_t* atom_ptr, const int32_t* d_numbers,
+                                    const double* d_positions, const double* cells9, const int32_t* pbc3, void* stream);
+/* After the three stages over [0, n): energy [B] (eV), forces [n,3] (eV/A, caller's atom order) and virial [B,6]
+ * (eV; xx,yy,zz,xy,yz,zx of -sum r (x) dE/dr, the order and sign of s7b_engine_system_results, so the two add), fp64
+ * device pointers, no synchronisation.  Per-structure sums in a fixed order: deterministic, and independent of the
+ * other structures of the batch. */
+S7B_API int s7b_d3_system_results(S7bD3* d3, double* d_energy, double* d_forces, double* d_virial, void* stream);
 
 /* The reference's own D3 entry points (pair_d3_for_ase.cu:2034-2082; ctypes signatures sevenn/calculator.py:430-483),
  * same names / arguments / call order, so its D3Calculator can load this library in place of pair_d3.so.

@@ -11,6 +11,7 @@ reduced in fp64 by a kernel (``s7b_engine_system_results``).  ``SevenNetModel`` 
 same constructor keywords, ``forward(state) -> {'energy' [B], 'forces' [n,3], 'stress' [B,3,3]}``
 with the sign / Voigt handling of ``torchsim.py:286-290``.  ``torch_sim`` is not installed here, so
 ``state`` is duck-typed: ``positions, row_vector_cell (or cell), pbc, atomic_numbers, system_idx``.
+``SevenNetD3Model`` adds D3 dispersion of the whole batch (``d3.D3Batch``).
 """
 from __future__ import annotations
 
@@ -138,7 +139,8 @@ class DeviceBatch:
             raise ValueError('system_idx must be sorted')
         if h[3]:
             raise ValueError(f'system_idx must lie in [0, {B}): one structure per cell')
-        eng.set_positions_batch(species, positions, h[4:], cells, pbc)
+        self.atom_ptr = h[4:]
+        eng.set_positions_batch(species, positions, self.atom_ptr, cells, pbc)
         return self
 
     def compute(self, numbers, positions, cells, pbc, system_idx) -> dict:
@@ -193,19 +195,54 @@ class SevenNetModel:
     def dtype(self):
         return self._dtype
 
-    def forward(self, state, **kwargs):
+    def _cells(self, state):
+        """host float64 [B,3,3] cells of the state, rows = lattice vectors"""
         torch = self.engine.torch
         cells = getattr(state, 'row_vector_cell', None)
         if cells is None:   # SimState.cell holds column vectors
             cells = torch.as_tensor(state.cell).transpose(-1, -2)
-        cells = torch.as_tensor(cells).detach().to('cpu', torch.float64).reshape(-1, 3, 3).numpy()
-        out = self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
+        return torch.as_tensor(cells).detach().to('cpu', torch.float64).reshape(-1, 3, 3).numpy()
+
+    def _stress(self, virial, cells):
+        """[B,3,3] stress from the virial [B,6] (xx,yy,zz,xy,yz,zx) and the cells"""
+        torch = self.engine.torch
         vol = torch.as_tensor(np.abs(np.linalg.det(cells)), device=self._device)
-        s = (out['virial'] / vol[:, None])                      # 'inferred_stress', (xx,yy,zz,xy,yz,zx)
+        s = (virial / vol[:, None])                             # 'inferred_stress', (xx,yy,zz,xy,yz,zx)
         v = -s[:, [0, 1, 2, 4, 5, 3]]                           # ASE Voigt, sign of torchsim.py:286-290
-        stress = torch.stack([torch.stack([v[:, 0], v[:, 5], v[:, 4]], -1),
-                              torch.stack([v[:, 5], v[:, 1], v[:, 3]], -1),
-                              torch.stack([v[:, 4], v[:, 3], v[:, 2]], -1)], -2)
+        return torch.stack([torch.stack([v[:, 0], v[:, 5], v[:, 4]], -1),
+                            torch.stack([v[:, 5], v[:, 1], v[:, 3]], -1),
+                            torch.stack([v[:, 4], v[:, 3], v[:, 2]], -1)], -2)
+
+    def forward(self, state, **kwargs):
+        cells = self._cells(state)
+        out = self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
+        stress = self._stress(out['virial'], cells)
         return {'energy': out['energy'].to(self._dtype), 'forces': out['forces'], 'stress': stress.to(self._dtype)}
+
+    __call__ = forward
+
+
+class SevenNetD3Model(SevenNetModel):
+    """``SevenNetModel`` + D3 dispersion (``d3.D3Batch``), the batched counterpart of ``d3.SevenNetD3Calculator``:
+    ``model(state)`` evaluates the network and D3 of all systems of the state on the current stream and returns
+    their sums, energy [B], forces [n,3] and stress [B,3,3] (fp64 sums, returned in float32).  The stress of both
+    terms uses the state's cells.  A structure without a cell (all zeros) gets ``D3Calculator``'s generated cell for
+    the D3 term (``self.d3.cells``); its energy and forces are those of the isolated structure, but it has no volume,
+    so its stress is not finite (inf / nan), as in ``SevenNetModel``.  Keywords: those of ``SevenNetModel`` and of
+    ``SevenNetD3Calculator``'s D3 part."""
+
+    def __init__(self, model='7net-0', *, damping_type: str = 'damp_bj', functional_name: str = 'pbe',
+                 vdw_cutoff: float = 9000, cn_cutoff: float = 1600, **kwargs):
+        super().__init__(model, **kwargs)
+        from .d3 import D3Batch
+        self.d3 = D3Batch(damping_type, functional_name, vdw_cutoff, cn_cutoff, device=self._device.index)
+
+    def forward(self, state, **kwargs):
+        cells = self._cells(state)
+        out = self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
+        d3 = self.d3.compute(state.atomic_numbers, state.positions, cells, state.pbc, atom_ptr=self._batch.atom_ptr)
+        stress = self._stress(out['virial'] + d3['virial'], cells)
+        return {'energy': (out['energy'] + d3['energy']).to(self._dtype),
+                'forces': (out['forces'].double() + d3['forces']).to(self._dtype), 'stress': stress.to(self._dtype)}
 
     __call__ = forward

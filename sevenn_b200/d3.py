@@ -1,7 +1,8 @@
 """D3 dispersion front-end: ``D3Calculator`` / ``SevenNetD3Calculator`` with the constructor and result
 keys of the reference (``sevenn/calculator.py:236-314, 387-618``) on top of the cell-list CUDA kernels of
 ``csrc/d3_kernels.cuh`` (C ABI ``s7b_d3_*``), plus the multi-GPU driver the reference does not have
-(its D3 is single-GPU and limited to 46 340 atoms, ``docs/source/user_guide/d3.md:7,53``).
+(its D3 is single-GPU and limited to 46 340 atoms, ``docs/source/user_guide/d3.md:7,53``), and ``D3Batch``: many
+structures in one pass from device-resident arrays, the layout of a TorchSim state (``batch.SevenNetD3Model``).
 
 Unlike the reference binding there is no LAMMPS-frame rotation: the library takes lattice vectors in any
 orientation, so forces and the virial come back in the caller's frame.
@@ -15,7 +16,7 @@ from typing import Optional
 
 import numpy as np
 
-from .engine import check, load_library
+from .engine import _host, check, load_library
 
 _PARAMS = None
 AU_TO_ANG = 0.52917726
@@ -72,6 +73,10 @@ class D3Engine:
     def _stream(self):
         return ctypes.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)
 
+    def _set_damping(self):
+        check(self.lib.s7b_d3_set_damping(self._h, self.damping, self.par['s6'], self.par['s8'], self.par['a1'],
+                                          self.par['a2'], self.par['alp6'], self.par['alp8'], self.rthr, self.cnthr))
+
     def set_system(self, numbers, positions, cell, pbc=(True, True, True)):
         """numbers [n] atomic numbers, positions [n,3] and cell rows in Angstrom."""
         numbers = np.asarray(numbers, dtype=np.int64)
@@ -86,8 +91,7 @@ class D3Engine:
             with self.torch.cuda.device(self.device):
                 check(self.lib.s7b_d3_set_params(self._h, len(uniq), rcov.ctypes.data, r2r4.ctypes.data, r0.ctypes.data,
                                                  c6.ctypes.data, cr.ctypes.data, mxc.ctypes.data))
-                check(self.lib.s7b_d3_set_damping(self._h, self.damping, self.par['s6'], self.par['s8'], self.par['a1'],
-                                                  self.par['a2'], self.par['alp6'], self.par['alp8'], self.rthr, self.cnthr))
+                self._set_damping()
             self._numbers = uniq
         lut = {zz: i for i, zz in enumerate(uniq)}
         types = np.ascontiguousarray([lut[int(a)] for a in numbers], dtype=np.int32)
@@ -155,6 +159,103 @@ def distributed_d3(engine: D3Engine, numbers, positions, cell, pbc=(True, True, 
     for name in ('energy', 'sigma'):
         dist.all_reduce(engine.buffer(name), group=group)
     return engine.results()
+
+
+def batch_inputs(torch, device, numbers, positions, cells, pbc, system_idx=None, atom_ptr=None, max_cutoff=None):
+    """Host logic of ``D3Batch.compute``: (numbers int32 [n] and positions float64 [n,3] on ``device``, atom_ptr int32
+    [B+1], cells float64 [B,3,3], pbc int32 [B,3]; the last three on the host).  atom_ptr is taken as given, else
+    derived from system_idx (one readback), else the batch is one structure.  A non-empty structure with an
+    all-zero cell gets ``D3Calculator``'s cell: an orthogonal box of its extent + max_cutoff + 1 A, periodic; the
+    extents are a device min / max, read back only when such a structure is present."""
+    z = torch.as_tensor(numbers).detach().to(device, torch.int32).contiguous().reshape(-1)
+    pos = torch.as_tensor(positions).detach().to(device, torch.float64).contiguous().reshape(-1, 3)
+    c = np.array(_host(cells), dtype=np.float64).reshape(-1, 3, 3)
+    B, n = int(c.shape[0]), int(z.shape[0])
+    if B < 1:
+        raise ValueError('empty batch')
+    if pos.shape[0] != n:
+        raise ValueError(f'numbers ({n}) and positions ({pos.shape[0]}) need the same number of rows')
+    pb = np.array(np.broadcast_to(np.asarray(_host(pbc), dtype=bool), (B, 3)))
+    if atom_ptr is not None:
+        ap = np.array(_host(atom_ptr), dtype=np.int64).ravel()
+        if ap.shape[0] != B + 1 or ap[0] != 0 or ap[-1] != n or (np.diff(ap) < 0).any():
+            raise ValueError(f'atom_ptr must be non-decreasing, [B+1] = [{B + 1}], from 0 to {n}')
+    elif system_idx is not None:
+        si = torch.as_tensor(system_idx).detach().to(device, torch.int64).reshape(-1)
+        if si.shape[0] != n:
+            raise ValueError(f'system_idx has {si.shape[0]} entries for {n} atoms')
+        flags = torch.zeros(2, dtype=torch.int64, device=device)
+        if n > 0:                 # one readback: unsorted, out of range, then atom_ptr
+            flags[0] = (si[1:] < si[:-1]).any()
+            flags[1] = (si.min() < 0) | (si.max() >= B)
+        counts = torch.bincount(si.clamp(0, B - 1), minlength=B)
+        h = torch.cat([flags, torch.zeros(1, dtype=torch.int64, device=device), torch.cumsum(counts, 0)]).cpu().numpy()
+        if h[0]:
+            raise ValueError('system_idx must be sorted')
+        if h[1]:
+            raise ValueError(f'system_idx must lie in [0, {B}): one structure per cell')
+        ap = h[2:]
+    elif B == 1:
+        ap = np.array([0, n])
+    else:
+        raise ValueError('a batch of several structures needs system_idx or atom_ptr')
+    zero = np.flatnonzero((c.reshape(B, 9) == 0).all(1) & (ap[1:] > ap[:-1]))
+    if zero.size:
+        sys = torch.repeat_interleave(torch.arange(B, device=device), torch.as_tensor(np.diff(ap), device=device))
+        idx = sys[:, None].expand(-1, 3)
+        lo = torch.full((B, 3), np.inf, dtype=torch.float64, device=device).scatter_reduce(0, idx, pos, 'amin')
+        hi = torch.full((B, 3), -np.inf, dtype=torch.float64, device=device).scatter_reduce(0, idx, pos, 'amax')
+        zi = torch.as_tensor(zero, device=device)
+        lohi = torch.stack([lo[zi], hi[zi]], 1).cpu().numpy()
+        for k, b in enumerate(zero):       # D3Calculator.calculate, for this structure alone
+            c[b] = np.eye(3) * (lohi[k, 1] - lohi[k, 0] + max_cutoff + 1.0)
+            pb[b] = True
+    return z, pos, np.ascontiguousarray(ap, dtype=np.int32), c, np.ascontiguousarray(pb.astype(np.int32))
+
+
+class D3Batch:
+    """D3 of B structures in one pass on one GPU (C ABI ``s7b_d3_set_system_batch``): atomic numbers and positions
+    stay on the device, the full element tables are uploaded once, every structure has its own cell list and at most
+    16 elements (any number in the batch).  Damping and functional as ``D3Engine``; ``engine`` is that D3Engine,
+    whose ``buffer`` views show the per-atom values of the last batch (bin-sorted order, ``order`` maps them)."""
+
+    def __init__(self, damping_type: str = 'damp_bj', functional_name: str = 'pbe', vdw_cutoff: float = 9000.0,
+                 cn_cutoff: float = 1600.0, device: Optional[int] = None):
+        self.engine = eng = D3Engine(damping_type, functional_name, vdw_cutoff, cn_cutoff, device=device)
+        self.torch, self.device = eng.torch, eng.device
+        self.max_cutoff = np.sqrt(max(eng.rthr, eng.cnthr)) * AU_TO_ANG        # D3Calculator's zero-cell rule
+        T = d3_tables()
+        f8 = lambda a: np.ascontiguousarray(a, dtype=np.float64)
+        self._tables = [f8(T['rcov']), f8(T['r2r4']), f8(T['r0ab']), f8(T['c6ref']), f8(T['cnref']),
+                        np.ascontiguousarray(T['mxc'], dtype=np.int32)]
+        with self.torch.cuda.device(self.device):
+            check(eng.lib.s7b_d3_set_element_tables(eng._h, *[a.ctypes.data for a in self._tables]))
+            eng._set_damping()
+        self.cells = self.pbc = None
+
+    def compute(self, numbers, positions, cells, pbc, system_idx=None, atom_ptr=None) -> dict:
+        """numbers [n] atomic numbers, positions [n,3] (Angstrom, float32 or float64), cells [B,3,3] (rows), pbc
+        ([3] or [B,3]), and system_idx [n] (sorted) or atom_ptr [B+1]: torch tensors on any device, or numpy arrays.
+        -> dict of float64 device tensors: energy [B] (eV), forces [n,3] (eV/A), virial [B,6] (eV; xx,yy,zz,xy,yz,zx,
+        the order and sign of ``DeviceBatch``'s virial).  ``self.cells`` / ``self.pbc`` hold the cells used."""
+        torch, eng = self.torch, self.engine
+        z, pos, ap, c, pb = batch_inputs(torch, self.device, numbers, positions, cells, pbc, system_idx, atom_ptr,
+                                         self.max_cutoff)
+        B, n = len(ap) - 1, int(ap[-1])
+        self.cells, self.pbc = c, pb.astype(bool)
+        cc = np.ascontiguousarray(c.reshape(B, 9))
+        energy = torch.empty(B, dtype=torch.float64, device=self.device)
+        forces = torch.empty(n, 3, dtype=torch.float64, device=self.device)
+        virial = torch.empty(B, 6, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            st = eng._stream()
+            check(eng.lib.s7b_d3_set_system_batch(eng._h, B, ap.ctypes.data, z.data_ptr(), pos.data_ptr(), cc.ctypes.data,
+                                                  pb.ctypes.data, st))
+            eng.n = n
+            for stage in (1, 2, 3):
+                check(eng.lib.s7b_d3_run_stage(eng._h, stage, 0, n, st))
+            check(eng.lib.s7b_d3_system_results(eng._h, energy.data_ptr(), forces.data_ptr(), virial.data_ptr(), st))
+        return dict(energy=energy, forces=forces, virial=virial)
 
 
 try:

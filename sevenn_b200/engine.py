@@ -60,6 +60,7 @@ EXPORTS = [
     's7b_engine_profile_count', 's7b_engine_profile_entry', 's7b_conv_plan_create',
     's7b_conv_plan_destroy', 's7b_conv_plan_dims', 's7b_conv_forward', 's7b_conv_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
+    's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results',
 ]
 
 
@@ -100,6 +101,9 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_d3_buffer.restype = vp
     lib.s7b_d3_results_host.argtypes = [vp, vp, vp, vp, vp]
     lib.s7b_d3_compute_host.argtypes = [vp, vp, vp, vp, vp]
+    lib.s7b_d3_set_element_tables.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.s7b_d3_set_system_batch.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]
+    lib.s7b_d3_system_results.argtypes = [vp, vp, vp, vp, vp]
     lib.s7b_engine_set_param.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, vp, sz]
     lib.s7b_engine_set_graph.argtypes = [vp, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.s7b_engine_run_stage.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]
