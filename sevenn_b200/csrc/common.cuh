@@ -28,21 +28,31 @@ S7B_HD float dsilu_n(float z) {
 struct ConvRole {
   int x_off;                  // offset of the l1 block inside a node row of x   (cm layout)
   int mul;                    // channels of l1 == component stride inside the block
-  int w_off[kMaxPaths];       // per path: first column in weight[E, W] / table row
+  int tab_off;                // first channel pair of this role's radial table image (table mode, see ConvArgs::table)
+  int w_off[kMaxPaths];       // per path: first column in weight[E, W]
   int out_off[kMaxPaths];     // per path: offset inside a mid row of element (k = 0, u = 0)
   int out_stride[kMaxPaths];  // per path: K_l3 (component stride in the fused mid block)
 };
 
+// Floats per edge of the stored harmonics Y_1 .. Y_{NY-1} (Y_0 = 1 is implicit), padded to whole float4s.
+__host__ __device__ constexpr int y_stride(int ny) { return (ny - 1 + 3) / 4 * 4; }
+
+// Return code of the per-group convolution dispatch (conv_dispatch.cuh) for a role whose multiplicity is not
+// the one its kernels were compiled for (kConvMul, conv_kernels.cuh).
+constexpr int kConvWrongMul = 3;
+
 struct ConvArgs {
   const int* rowptr;          // [n_dst + 1] CSR over destination (centre) atoms
   const int4* rec;            // [E] {src, table interval, frac bits, 0}
-  const float* Y;             // [E, ny_stride]  Y_1 .. Y_{NY-1} (Y_0 = 1 implicit), zero padded
+  const float* Y;             // [E, y_stride(NY)]  Y_1 .. Y_{NY-1} (Y_0 = 1 implicit), zero padded
   const float* x;             // [n_nodes, dim_x]
-  const float4* table;        // [knots, W/2] {a0e,a0o,a1e,a1o}: value and slope*h of the cubic, per channel pair
-  const uint2* table23;       // [knots, W/2] {half2(a2e,a2o), half2(a3e,a3o)}: the two small cubic terms in fp16
+  // Radial tables: one image per l1 role at ConvRole::tab_off, laid out [knot][path of the role][channel pair]
+  // (engine.cu role_table_images), so that one edge reaches all paths of its role from one address.
+  const float4* table;        // {a0e,a0o,a1e,a1o}: value and slope*h of the cubic, per channel pair
+  const uint2* table23;       // {half2(a2e,a2o), half2(a3e,a3o)}: the two small cubic terms in fp16
   const float* w;             // [E, W] stored weights (operator boundary / exact-MLP mode)
   int n_begin, n_dst;        // centre atoms [n_begin, n_dst) of this launch (multi-GPU: interior / boundary ranges)
-  int dim_x, dim_mid, w_numel, ny_stride;
+  int dim_x, dim_mid, w_numel;
   float inv_h;                // 1 / table interval
   unsigned int* row_max;      // optional [n_dst, rows_per_node]: running max |out| bits of every (l3, k) row of the mid
   int rows_per_node;          // features (row l3^2 + k), for the tensor-core linear that consumes them (tc_gemm.cuh)

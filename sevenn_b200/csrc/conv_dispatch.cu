@@ -24,6 +24,7 @@ int launch_conv_fwd(int l1, int lf, int lo, bool table, const ConvArgs& a, const
   else if (lf == 3 && lo == 3) rc = launch_conv_fwd_3_3(l1, table, a, role, out, st);
   else if (lf == 3 && lo == 0) rc = launch_conv_fwd_3_0(l1, table, a, role, out, st);
   if (rc == 2) { set_error(__FILE__, __LINE__, "no tensor-product kind compiled for this (lmax_filter, lmax_out)"); return 1; }
+  if (rc == kConvWrongMul) { set_error(__FILE__, __LINE__, "no convolution kernel compiled for this l1 multiplicity"); return 1; }
   if (rc) { set_error(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError())); return 1; }
   ++g_conv_launches;
   return 0;
@@ -39,6 +40,7 @@ int launch_conv_bwd(int l1, int lf, int lo, bool table, bool need_dx, const Conv
   else if (lf == 3 && lo == 3) rc = launch_conv_bwd_3_3(l1, table, need_dx, a, role, gout, dx, dY_acc, dEdr_acc, dw, st);
   else if (lf == 3 && lo == 0) rc = launch_conv_bwd_3_0(l1, table, need_dx, a, role, gout, dx, dY_acc, dEdr_acc, dw, st);
   if (rc == 2) { set_error(__FILE__, __LINE__, "no tensor-product kind compiled for this (lmax_filter, lmax_out)"); return 1; }
+  if (rc == kConvWrongMul) { set_error(__FILE__, __LINE__, "no convolution kernel compiled for this l1 multiplicity"); return 1; }
   if (rc) { set_error(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError())); return 1; }
   ++g_conv_launches;
   return 0;

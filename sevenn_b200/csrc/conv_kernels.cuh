@@ -26,14 +26,19 @@
 namespace s7b {
 
 constexpr int kConvWarpsPerBlock = 4;
+// Channels of the l1 = 0..3 blocks of x that the kernels are compiled for (those of SevenNet-0 and
+// SevenNet-l3i5).  The multiplicity is a template parameter, so that the component stride of x and the
+// table offsets are immediates; a model with other widths is refused when its layers are configured.
+constexpr int kConvMul[kMaxL] = {128, 64, 32, 32};
 // Register budget, as the min-resident-CTAs argument of __launch_bounds__ (128-thread CTAs: 4 -> 128
 // registers, 3 -> 168, 1 -> 255).  Chosen by A/B timing on the previous GPU generation (7net-0, 12k atoms;
 // not re-tuned on H100):
 //  * forward: an explicit 1 lets ptxas keep more gathers in flight for the l1 = 0 kernels (96 -> 128
 //    registers, -22 % time); the l1 >= 1 kernels do not change;
 //  * backward: l1 = 0 is fastest at 3 (-6 %), l1 = 1 at 4 (128 registers; 168 or 220 are 3-4 % slower),
-//    l1 >= 2 at 3 (what ptxas picks by itself).  The lmax = 3 kinds need > 168 registers (they spill
-//    otherwise) and are left at 2.
+//    l1 >= 2 at 3 (what ptxas picks by itself).  The l1 = 0 kernel without dx (first layer) at 4: it fits
+//    in 122 registers without spilling; at 3 it took 138 and 0.245 instead of 0.22 ms (H100, 700 W).  The
+//    lmax = 3 kinds need > 168 registers (they spill otherwise) and are left at 2.
 #ifndef S7B_FWD_MINBLOCKS
 #define S7B_FWD_MINBLOCKS 1
 #endif
@@ -41,7 +46,7 @@ constexpr int kConvWarpsPerBlock = 4;
 #ifdef S7B_BWD_MINBLOCKS
 #define S7B_BWD_BOUNDS __launch_bounds__(32 * kConvWarpsPerBlock, S7B_BWD_MINBLOCKS)
 #else
-#define S7B_BWD_BOUNDS __launch_bounds__(32 * kConvWarpsPerBlock, (Kind::NY != 9) ? 2 : ((Kind::D1 == 3) ? 4 : 3))
+#define S7B_BWD_BOUNDS __launch_bounds__(32 * kConvWarpsPerBlock, (Kind::NY != 9) ? 2 : ((Kind::D1 == 3 || !NEED_DX) ? 4 : 3))
 #endif
 #ifndef S7B_COOP_REC
 #define S7B_COOP_REC 1   // lanes of a group fetch the records of LPN consecutive edges at once (see EdgeRecs)
@@ -59,7 +64,7 @@ struct EdgeRecs {
   __device__ __forceinline__ void fill(const ConvArgs& a, int e0, int len, int it, int sl) {
     const int ei = it + sl;
     int4 r = make_int4(0, 0, 0, 0);
-    if (ei < len) r = __ldg(a.rec + e0 + ei);
+    if (ei < len) r = __ldg(a.rec + (unsigned)(e0 + ei));
     cx = r.x; cy = r.y; cz = r.z;
   }
   __device__ __forceinline__ int4 get(int it) const {
@@ -111,6 +116,9 @@ __device__ __forceinline__ void load_Y(const float* __restrict__ Yrow, float (&Y
   }
 }
 
+// i * stride for a non-negative row index and stride (node, edge): one 32 x 32 -> 64-bit multiply
+__device__ __forceinline__ size_t row_offset(int i, int stride) { return (size_t)(unsigned)i * (unsigned)stride; }
+
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
 // Per-lane value type: V2 = two adjacent channels (float2 math), float = one channel.
@@ -122,11 +130,10 @@ template <> struct VT<V2> {
   static __device__ __forceinline__ void store(float* p, V2 v) { *reinterpret_cast<float2*>(p) = v; }
   static __device__ __forceinline__ float hsum(V2 v) { return v.x + v.y; }
   static __device__ __forceinline__ float amax(V2 v) { return fmaxf(fabsf(v.x), fabsf(v.y)); }
-  // cubic coefficients of the channel pair starting at (even) column c of table row tk
-  static __device__ __forceinline__ void coef(const ConvArgs& a, int tk, int c, V2& a0, V2& a1, V2& a2, V2& a3) {
-    const size_t ti = (size_t)tk * (a.w_numel >> 1) + (c >> 1);
-    const float4 c01 = __ldg(a.table + ti);
-    const uint2 c23 = __ldg(a.table23 + ti);
+  // cubic coefficients of the channel pair at t01 / t23
+  static __device__ __forceinline__ void coef(const float4* t01, const uint2* t23, bool, V2& a0, V2& a1, V2& a2, V2& a3) {
+    const float4 c01 = __ldg(t01);
+    const uint2 c23 = __ldg(t23);
     a0 = make_float2(c01.x, c01.y);
     a1 = make_float2(c01.z, c01.w);
     a2 = __half22float2(*reinterpret_cast<const __half2*>(&c23.x));
@@ -140,13 +147,12 @@ template <> struct VT<float> {
   static __device__ __forceinline__ void store(float* p, float v) { *p = v; }
   static __device__ __forceinline__ float hsum(float v) { return v; }
   static __device__ __forceinline__ float amax(float v) { return fabsf(v); }
-  static __device__ __forceinline__ void coef(const ConvArgs& a, int tk, int c, float& a0, float& a1, float& a2, float& a3) {
-    const size_t ti = (size_t)tk * (a.w_numel >> 1) + (c >> 1);
-    const float4 c01 = __ldg(a.table + ti);
-    const uint2 c23 = __ldg(a.table23 + ti);
+  // the odd or even channel of the pair at t01 / t23
+  static __device__ __forceinline__ void coef(const float4* t01, const uint2* t23, bool odd, float& a0, float& a1, float& a2, float& a3) {
+    const float4 c01 = __ldg(t01);
+    const uint2 c23 = __ldg(t23);
     const float2 h2 = __half22float2(*reinterpret_cast<const __half2*>(&c23.x));
     const float2 h3 = __half22float2(*reinterpret_cast<const __half2*>(&c23.y));
-    const bool odd = (c & 1) != 0;
     a0 = odd ? c01.y : c01.x;
     a1 = odd ? c01.w : c01.z;
     a2 = odd ? h2.y : h2.x;
@@ -179,12 +185,15 @@ struct LaneMap {
 
 // ------------------------------------------------------------------------------------------
 // forward:  out[n, path block] = sum_{e in row n} w_e * CG(x[src_e], Y_e)
-// grid = (ceil(n_dst / (kConvWarpsPerBlock * 32/LPN)), mul / (2*LPN*NV)), block = 32*kConvWarpsPerBlock
+// grid = (ceil(n_dst / (kConvWarpsPerBlock * 32/LPN)), MUL / (CH*LPN*NV)), block = 32*kConvWarpsPerBlock
+// MUL (= role.mul) is a compile-time constant: the component stride of x and the table offsets of the paths
+// become immediates, and each edge costs one x address and one table address per lane.
 // ------------------------------------------------------------------------------------------
-template <class Kind, int NV, int LPN, bool TABLE, class V>
+template <class Kind, int MUL, int NV, int LPN, bool TABLE, class V>
 __global__ void S7B_FWD_BOUNDS
 conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) {
   constexpr int CH = VT<V>::CH;
+  static_assert(MUL % (CH * LPN * NV) == 0, "channels must fill whole lane groups");
   const LaneMap<NV, LPN, CH> m(a);
   if (m.nmax == 0 && !m.node_ok) return;      // whole warp beyond the last node (uniform)
 
@@ -194,6 +203,9 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
 #pragma unroll
     for (int q = 0; q < Kind::NACC; ++q) acc[c][q] = VT<V>::zero();
 
+  const unsigned xlane = role.x_off + m.uc0;               // this lane's first element in a row of x
+  const unsigned tlane = role.tab_off + (m.uc0 >> 1);       // ... and its first pair in a knot row of the table
+  const bool odd = (m.uc0 & 1) != 0;
   EdgeRecs<LPN> recs;
   for (int it = 0; it < m.nmax; ++it) {
     const bool valid = (LPN == 32) || (it < m.len);
@@ -205,23 +217,26 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
     const int4 rec = __ldg(a.rec + e);
 #endif
     float Y[Kind::NY];
-    load_Y<Kind>(a.Y + (size_t)e * a.ny_stride, Y);
-    const float* __restrict__ xrow = a.x + (size_t)rec.x * a.dim_x + role.x_off;
+    load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
+    const float* __restrict__ xrow = a.x + (row_offset(rec.x, a.dim_x) + xlane);
+    const unsigned ti = tlane + rec.y * (Kind::NPATH * MUL / 2);   // knot row of the role's table image
+    const float4* __restrict__ k01 = a.table + ti;
+    const uint2* __restrict__ k23 = a.table23 + ti;
     const float tt = __int_as_float(rec.z);
 #pragma unroll
     for (int c = 0; c < NV; ++c) {
-      const int u = m.uc0 + CH * LPN * c;
+      const int u = CH * LPN * c;                        // channel offset from m.uc0
       V x[Kind::D1], w[Kind::NPATH];
 #pragma unroll
-      for (int i = 0; i < Kind::D1; ++i) x[i] = VT<V>::load(xrow + i * role.mul + u);
+      for (int i = 0; i < Kind::D1; ++i) x[i] = VT<V>::load(xrow + i * MUL + u);
 #pragma unroll
       for (int p = 0; p < Kind::NPATH; ++p) {
         if (TABLE) {
           V a0, a1, a2, a3;
-          VT<V>::coef(a, rec.y, role.w_off[p] + u, a0, a1, a2, a3);
+          VT<V>::coef(k01 + (p * (MUL / 2) + u / 2), k23 + (p * (MUL / 2) + u / 2), odd, a0, a1, a2, a3);
           w[p] = fma_(tt, fma_(tt, fma_(tt, a3, a2), a1), a0);
         } else {
-          w[p] = VT<V>::load(a.w + (size_t)e * a.w_numel + role.w_off[p] + u);
+          w[p] = VT<V>::load(a.w + (size_t)e * a.w_numel + role.w_off[p] + m.uc0 + u);
         }
         if (LPN != 32 && !valid) w[p] = VT<V>::zero();
       }
@@ -272,13 +287,16 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
 //   !TABLE: dw[e, :]     = dE/dw                                          (plug-in boundary)
 //   dY_acc[e, 1..]      += sum_u dE/dY                                    (group reduction)
 //   dx[src_e, :]        += dE/dx                                          (RED.ADD.F32x2, NEED_DX)
-// dY_acc / dEdr_acc / dw rows are owned by exactly one group of one launch: plain read-modify-write.
+// dY_acc / dEdr_acc / dw rows are owned by exactly one group of one launch: plain read-modify-write,
+// unless the role's channels are spread over several CTAs (SPLIT, gridDim.y > 1): then they are added atomically.
 // ------------------------------------------------------------------------------------------
-template <class Kind, int NV, int LPN, bool TABLE, bool NEED_DX, bool SPLIT>
+template <class Kind, int MUL, int NV, int LPN, bool TABLE, bool NEED_DX>
 __global__ void S7B_BWD_BOUNDS
 conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__ gout,
                 float* __restrict__ dx, float* __restrict__ dY_acc, float* __restrict__ dEdr_acc,
                 float* __restrict__ dw) {
+  static_assert(MUL % (2 * LPN * NV) == 0, "channels must fill whole lane groups");
+  constexpr bool SPLIT = MUL > 2 * LPN * NV;
   const LaneMap<NV, LPN, 2> m(a);
   if (m.nmax == 0) return;                    // uniform: no edges in any row of this warp
 
@@ -302,6 +320,8 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
   const int idx = (m.sl / PER) % NR;                      // which reduced value ends up in this lane
   const bool is_dY = idx + 1 < Kind::NY;
   const bool writer = (m.sl % PER) == 0 && (is_dY || (RIDE && idx == NR - 1));
+  const unsigned xlane = role.x_off + m.uc0;               // this lane's first element in a row of x / dx
+  const unsigned tlane = role.tab_off + (m.uc0 >> 1);       // ... and its first pair in a knot row of the table
   EdgeRecs<LPN> recs;
   for (int it = 0; it < m.nmax; ++it) {
     const bool valid = (LPN == 32) || (it < m.len);
@@ -313,8 +333,11 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
     const int4 rec = __ldg(a.rec + e);
 #endif
     float Y[Kind::NY];
-    load_Y<Kind>(a.Y + (size_t)e * a.ny_stride, Y);
-    const float* __restrict__ xrow = a.x + (size_t)rec.x * a.dim_x + role.x_off;
+    load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
+    const size_t xo = row_offset(rec.x, a.dim_x) + xlane;
+    const unsigned ti = tlane + rec.y * (Kind::NPATH * MUL / 2);   // knot row of the role's table image
+    const float4* __restrict__ k01 = a.table + ti;
+    const uint2* __restrict__ k23 = a.table23 + ti;
     const float tt = __int_as_float(rec.z);
     V2 dY[Kind::NY];
 #pragma unroll
@@ -322,23 +345,22 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
     V2 dEdr2 = splat2(0.0f);
 #pragma unroll
     for (int c = 0; c < NV; ++c) {
-      const int u = m.uc0 + 2 * LPN * c;
+      const int u = 2 * LPN * c;                         // channel offset from m.uc0
       V2 x[Kind::D1], w[Kind::NPATH], wd[Kind::NPATH], dwv[Kind::NPATH], dxv[Kind::D1];
 #pragma unroll
-      for (int i = 0; i < Kind::D1; ++i) x[i] = ldg2(xrow + i * role.mul + u);
+      for (int i = 0; i < Kind::D1; ++i) x[i] = ldg2(a.x + xo + (i * MUL + u));
 #pragma unroll
       for (int p = 0; p < Kind::NPATH; ++p) {
         if (TABLE) {
-          const size_t ti = (size_t)rec.y * (a.w_numel >> 1) + ((role.w_off[p] + u) >> 1);
-          const float4 c01 = __ldg(a.table + ti);
-          const uint2 c23 = __ldg(a.table23 + ti);
+          const float4 c01 = __ldg(k01 + (p * (MUL / 2) + u / 2));
+          const uint2 c23 = __ldg(k23 + (p * (MUL / 2) + u / 2));
           const V2 a0 = make_float2(c01.x, c01.y), a1 = make_float2(c01.z, c01.w);
           const V2 a2 = __half22float2(*reinterpret_cast<const __half2*>(&c23.x));
           const V2 a3 = __half22float2(*reinterpret_cast<const __half2*>(&c23.y));
           w[p] = fma_(tt, fma_(tt, fma_(tt, a3, a2), a1), a0);
           wd[p] = mul_(fma_(tt, fma_(3.0f * tt, a3, mul_(a2, 2.0f)), a1), a.inv_h);
         } else {
-          w[p] = ldg2(a.w + (size_t)e * a.w_numel + role.w_off[p] + u);
+          w[p] = ldg2(a.w + (size_t)e * a.w_numel + role.w_off[p] + m.uc0 + u);
         }
       }
       Kind::bwd(x, Y, w, ga[c], dwv, dxv, dY);
@@ -346,13 +368,12 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
 #pragma unroll
         for (int p = 0; p < Kind::NPATH; ++p) {
           if (TABLE) dEdr2 = fma_(dwv[p], wd[p], dEdr2);
-          else *reinterpret_cast<float2*>(dw + (size_t)e * a.w_numel + role.w_off[p] + u) = dwv[p];
+          else *reinterpret_cast<float2*>(dw + (size_t)e * a.w_numel + role.w_off[p] + m.uc0 + u) = dwv[p];
         }
         if (NEED_DX) {
-          float* __restrict__ dxrow = dx + (size_t)rec.x * a.dim_x + role.x_off;
 #pragma unroll
           for (int i = 0; i < Kind::D1; ++i)
-            atomicAdd(reinterpret_cast<float2*>(dxrow + i * role.mul + u), dxv[i]);
+            atomicAdd(reinterpret_cast<float2*>(dx + xo + (i * MUL + u)), dxv[i]);
         }
       }
     }
@@ -364,9 +385,9 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
     if (RIDE) red[NR - 1] = dEdr;
     group_reduce_multi<NR, LPN>(red, m.sl);
     // a (node, l1) role normally belongs to one group -> plain read-modify-write (deterministic);
-    // SPLIT (launched with gridDim.y > 1: the role's channels are spread over several CTAs) adds atomically
+    // SPLIT (the role's channels are spread over several CTAs) adds atomically
     if (valid && writer) {
-      float* dst = is_dY ? dY_acc + (size_t)e * a.ny_stride + idx : dEdr_acc + e;
+      float* dst = is_dY ? dY_acc + row_offset(e, y_stride(Kind::NY)) + idx : dEdr_acc + e;
       if (SPLIT) atomicAdd(dst, red[0]);
       else *dst += red[0];      // (requesting the old value at the top of the iteration was measured 1 % slower)
     }

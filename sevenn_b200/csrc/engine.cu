@@ -230,15 +230,18 @@ static int irreps_dim(const int* muls, int n_l) {
   return d;
 }
 
-// Restates build_layer() of sevenn_b200/spec.py (reference convolution.py:61-82 path order).
+// Restates build_layer() of sevenn_b200/spec.py (reference convolution.py:61-82 path order).  knots: rows of the
+// radial table (0 without one), which places the per-role table images (ConvRole::tab_off).
 static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* out_muls, int n_lo,
-                           int lmax_filter) {
+                           int lmax_filter, int knots) {
   L.n_lx = n_lx;
   L.n_lg = n_lo;
   L.lmax_out = n_lo - 1;
   int off = 0;
   for (int l = 0; l < n_lx; ++l) {
-    if (x_muls[l] % 32 != 0 || x_muls[l] <= 0) return fail("multiplicities must be positive multiples of 32");
+    if (x_muls[l] != kConvMul[l])
+      return fail("the convolution kernels are compiled for " + std::to_string(kConvMul[l]) + " channels of l = " +
+                  std::to_string(l) + " in x, not " + std::to_string(x_muls[l]) + " (conv_kernels.cuh kConvMul)");
     L.x_muls[l] = x_muls[l];
     L.x_off[l] = off;
     off += (2 * l + 1) * x_muls[l];
@@ -289,12 +292,14 @@ static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* 
     off += (2 * l + 1) * k_run[l];
   }
   L.dim_mid = off;
-  // conv roles: per l1 the paths in slot order
+  // conv roles: per l1 the paths in slot order; the role's table image follows those of the smaller l1
+  int tab_off = 0;
   for (int l1 = 0; l1 < n_lx; ++l1) {
     ConvRole& r = L.roles[l1];
     memset(&r, 0, sizeof(r));
     r.x_off = L.x_off[l1];
     r.mul = x_muls[l1];
+    r.tab_off = tab_off;
     int p = 0;
     for (const PathCfg& q : L.paths) {
       if (q.l1 != l1) continue;
@@ -304,6 +309,7 @@ static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* 
       r.out_stride[p] = L.mid_K[q.l3];
       ++p;
     }
+    tab_off += knots * p * (r.mul / 2);
   }
   // gate
   GateDesc& gd = L.gate;
@@ -684,6 +690,28 @@ static int conv_forward(const LayerCfg& L, int lmax_filter, bool table, ConvArgs
   return 0;
 }
 
+// The radial table of a layer arrives as [knot][channel pair of the W columns], 16 B ("table") or 8 B ("table23")
+// per pair (engine.py pack_table_pairs).  The kernels read one image per l1 role at ConvRole::tab_off, laid out
+// [knot][path of the role][channel pair]: an edge then reaches all paths of its role from one address, at
+// offsets fixed at compile time.  Same values and total size, permuted.
+static std::vector<float> role_table_images(const LayerCfg& L, int knots, const float* host, int floats_per_pair) {
+  std::vector<float> img((size_t)knots * (L.W / 2) * floats_per_pair);
+  for (int l1 = 0; l1 < L.n_lx; ++l1) {
+    const ConvRole& r = L.roles[l1];
+    std::vector<int> cols;
+    for (const PathCfg& q : L.paths)
+      if (q.l1 == l1) cols.push_back(q.w_off);
+    const size_t run = (size_t)(r.mul / 2) * floats_per_pair;
+    float* dst = img.data() + (size_t)r.tab_off * floats_per_pair;
+    for (int k = 0; k < knots; ++k)
+      for (int c : cols) {
+        memcpy(dst, host + ((size_t)k * (L.W / 2) + c / 2) * floats_per_pair, run * sizeof(float));
+        dst += run;
+      }
+  }
+  return img;
+}
+
 }  // namespace s7b
 
 // =========================================================================================
@@ -831,7 +859,8 @@ int s7b_engine_create(const S7bModelDesc* d, S7bEngine** out) {
       delete e;
       return fail("irreps lmax out of range");
     }
-    if (build_layer_cfg(e->layers[t], d->muls[t], d->n_l[t], d->muls[t + 1], d->n_l[t + 1], d->lmax_filter)) {
+    if (build_layer_cfg(e->layers[t], d->muls[t], d->n_l[t], d->muls[t + 1], d->n_l[t + 1], d->lmax_filter,
+                        std::max(d->table_knots, 0))) {
       delete e;
       return 1;
     }
@@ -840,7 +869,7 @@ int s7b_engine_create(const S7bModelDesc* d, S7bEngine** out) {
     delete e;
     return fail("the first layer input must be scalars only");
   }
-  e->ny_stride = (d->lmax_filter == 3) ? 16 : ((d->lmax_filter == 2) ? 8 : 4);
+  e->ny_stride = y_stride((d->lmax_filter + 1) * (d->lmax_filter + 1));
   const int T = d->n_layers;
   e->x.resize(T);
   e->g.resize(T);
@@ -927,6 +956,16 @@ int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float*
   else {
     if (layer >= e->desc.n_layers) return fail("layer out of range");
     dst = &e->layers[layer].params[nm];
+  }
+  std::vector<float> img;
+  if (layer >= 0 && (nm == "table" || nm == "table23")) {
+    const int fpp = nm == "table" ? 4 : 2;
+    const LayerCfg& L = e->layers[layer];
+    if (e->desc.table_knots <= 0) return fail("parameter " + nm + ": the model was created without radial tables");
+    if (numel != (size_t)e->desc.table_knots * (L.W / 2) * fpp)
+      return fail("parameter " + nm + ": size does not match the layer configuration and knot count");
+    img = role_table_images(L, e->desc.table_knots, host, fpp);
+    host = img.data();
   }
   if (dst->ensure(numel * sizeof(float))) return fail("cudaMalloc failed for parameter " + nm);
   S7B_CUDA_CHECK(cudaMemcpy(dst->p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
@@ -1058,7 +1097,6 @@ static ConvArgs make_conv_args(const S7bEngine* e, int t, const float* x) {
   a.dim_x = L.dim_x;
   a.dim_mid = L.dim_mid;
   a.w_numel = L.W;
-  a.ny_stride = e->ny_stride;
   a.inv_h = e->radial.inv_h;
   return a;
 }
@@ -1917,12 +1955,12 @@ int s7b_conv_plan_create(int32_t n_l_x, const int32_t* x_muls, int32_t lmax_filt
     return fail("irreps out of the supported range (l <= 3)");
   S7bConvPlan* p = new S7bConvPlan();
   int out_muls[kMaxL] = {32, 32, 32, 32};   // only lmax_out matters for the path set
-  if (build_layer_cfg(p->cfg, x_muls, n_l_x, out_muls, lmax_out + 1, lmax_filter)) {
+  if (build_layer_cfg(p->cfg, x_muls, n_l_x, out_muls, lmax_out + 1, lmax_filter, 0)) {
     delete p;
     return 1;
   }
   p->lmax_filter = lmax_filter;
-  p->ny_stride = (lmax_filter == 3) ? 16 : ((lmax_filter == 2) ? 8 : 4);
+  p->ny_stride = y_stride((lmax_filter + 1) * (lmax_filter + 1));
   *out = p;
   return 0;
 }
@@ -2000,7 +2038,6 @@ int s7b_conv_forward(const S7bConvPlan* p, const float* x, const float* sh, cons
   a.dim_x = L.dim_x;
   a.dim_mid = L.dim_mid;
   a.w_numel = L.W;
-  a.ny_stride = p->ny_stride;
   a.inv_h = 1.0f;
   int rc = conv_forward(L, p->lmax_filter, false, a, out, st);
   cudaFreeAsync(rec, st);
@@ -2037,7 +2074,6 @@ int s7b_conv_backward(const S7bConvPlan* p, const float* x, const float* sh, con
   a.dim_x = L.dim_x;
   a.dim_mid = L.dim_mid;
   a.w_numel = L.W;
-  a.ny_stride = p->ny_stride;
   a.inv_h = 1.0f;
   int rc = 0;
   for (int l1 = 0; l1 < L.n_lx && !rc; ++l1)
