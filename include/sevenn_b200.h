@@ -54,7 +54,12 @@ typedef struct {
   int32_t poly_p;
   int32_t radial_hidden[2];                           /* radial MLP hidden widths (64, 64) */
   int32_t n_l[S7B_MAX_LAYERS + 1];                    /* number of l's of irreps t (t = n_layers: output) */
-  int32_t muls[S7B_MAX_LAYERS + 1][S7B_MAX_L];        /* multiplicity of l in irreps t */
+  int32_t muls[S7B_MAX_LAYERS + 1][S7B_MAX_L];        /* multiplicity of l in irreps t: positive multiples of 32
+                                                         (x of a layer: at most 1024).  The widths of SevenNet-0 /
+                                                         SevenNet-l3i5 (128, 64, 32, 32 at l = 0..3, lmax_filter 2 or 3,
+                                                         lmax_out = lmax_filter or 0) run convolution kernels
+                                                         specialised for them; every other width and lmax combination
+                                                         runs the runtime-width convolution kernels. */
   int32_t table_knots;                                /* > 0: radial weights from cubic tables */
 } S7bModelDesc;
 
@@ -260,8 +265,10 @@ S7B_API int s7b_engine_graph_stats(S7bEngine* eng, int64_t* captures, int64_t* r
 S7B_API int s7b_engine_stage_graph_stats(S7bEngine* eng, int64_t* captures, int64_t* replays);
 
 /* ---- operator-level plug-in: fused gather -> 'uvu' tensor product -> scatter ------------- */
-/* irreps of x as multiplicities per l (even parity), filter lmax, and lmax of the output; the
- * instruction set is the complete triangle-allowed one of sevenn/nn/convolution.py:61-82.      */
+/* irreps of x as multiplicities per l (even parity; positive multiples of 32, at most 1024), filter lmax 1..3,
+ * and lmax of the output 0..3; the instruction set is the complete triangle-allowed one of
+ * sevenn/nn/convolution.py:61-82.  Widths other than 128, 64, 32, 32 at l = 0..3, and (lmax_filter, lmax_out)
+ * other than (2, 2), (2, 0), (3, 3), (3, 0), run the runtime-width kernels.                                   */
 S7B_API int s7b_conv_plan_create(int32_t n_l_x, const int32_t* x_muls, int32_t lmax_filter,
                          int32_t lmax_out, S7bConvPlan** out);
 S7B_API void s7b_conv_plan_destroy(S7bConvPlan* plan);

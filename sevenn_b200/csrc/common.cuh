@@ -37,9 +37,11 @@ struct ConvRole {
 // Floats per edge of the stored harmonics Y_1 .. Y_{NY-1} (Y_0 = 1 is implicit), padded to whole float4s.
 __host__ __device__ constexpr int y_stride(int ny) { return (ny - 1 + 3) / 4 * 4; }
 
-// Return code of the per-group convolution dispatch (conv_dispatch.cuh) for a role whose multiplicity is not
-// the one its kernels were compiled for (kConvMul, conv_kernels.cuh).
+// Return code of the per-group convolution dispatch (conv_dispatch.cuh) for a role whose multiplicity no kernel
+// runs (not a positive multiple of 32; the engine refuses such models when their layers are configured).
 constexpr int kConvWrongMul = 3;
+// ... and for an l1 role whose kind has no path (for example l1 > lmax_filter with lmax_out = 0): nothing launched.
+constexpr int kConvNoPath = 4;
 
 struct ConvArgs {
   const int* rowptr;          // [n_dst + 1] CSR over destination (centre) atoms

@@ -19,15 +19,17 @@
 
 namespace s7b {
 
+// grid.y = role channels / channels per lane group; MUL = 0 takes the width from role.mul
 template <int MUL, int NV, int LPN, int CH = 2>
-static inline dim3 conv_grid(const ConvArgs& a) {
+static inline dim3 conv_grid(const ConvArgs& a, const ConvRole& role) {
   const int nodes_per_block = kConvWarpsPerBlock * (32 / LPN);
-  return dim3((a.n_dst - a.n_begin + nodes_per_block - 1) / nodes_per_block, MUL / (CH * LPN * NV));
+  const int mul = MUL > 0 ? MUL : role.mul;
+  return dim3((a.n_dst - a.n_begin + nodes_per_block - 1) / nodes_per_block, mul / (CH * LPN * NV));
 }
 
 template <class Kind, int MUL, int NV, int LPN>
 static int launch_fwd_one(bool table, const ConvArgs& a, const ConvRole& role, float* out, cudaStream_t st) {
-  const dim3 grid = conv_grid<MUL, NV, LPN>(a);
+  const dim3 grid = conv_grid<MUL, NV, LPN>(a, role);
   if (table) conv_fwd_kernel<Kind, MUL, NV, LPN, true, V2><<<grid, 32 * kConvWarpsPerBlock, 0, st>>>(a, role, out);
   else conv_fwd_kernel<Kind, MUL, NV, LPN, false, V2><<<grid, 32 * kConvWarpsPerBlock, 0, st>>>(a, role, out);
   return cudaGetLastError() == cudaSuccess ? 0 : 1;
@@ -36,7 +38,7 @@ static int launch_fwd_one(bool table, const ConvArgs& a, const ConvRole& role, f
 // one channel per lane, a full warp per node (alternative forward mapping for mul = 32, see S7B_FWD_ODD_PAIRS)
 template <class Kind, int MUL>
 static int launch_fwd_scalar(bool table, const ConvArgs& a, const ConvRole& role, float* out, cudaStream_t st) {
-  const dim3 grid = conv_grid<MUL, 1, 32, 1>(a);
+  const dim3 grid = conv_grid<MUL, 1, 32, 1>(a, role);
   if (table) conv_fwd_kernel<Kind, MUL, 1, 32, true, float><<<grid, 32 * kConvWarpsPerBlock, 0, st>>>(a, role, out);
   else conv_fwd_kernel<Kind, MUL, 1, 32, false, float><<<grid, 32 * kConvWarpsPerBlock, 0, st>>>(a, role, out);
   return cudaGetLastError() == cudaSuccess ? 0 : 1;
@@ -45,7 +47,7 @@ static int launch_fwd_scalar(bool table, const ConvArgs& a, const ConvRole& role
 template <class Kind, int MUL, int NV, int LPN, bool ALLOW_NODX>
 static int launch_bwd_one(bool table, bool need_dx, const ConvArgs& a, const ConvRole& role,
                           const float* gout, float* dx, float* dY, float* dEdr, float* dw, cudaStream_t st) {
-  const dim3 grid = conv_grid<MUL, NV, LPN>(a);
+  const dim3 grid = conv_grid<MUL, NV, LPN>(a, role);
   const int blk = 32 * kConvWarpsPerBlock;
   if (!need_dx && ALLOW_NODX) {
     if (table) conv_bwd_kernel<Kind, MUL, NV, LPN, true, !ALLOW_NODX><<<grid, blk, 0, st>>>(a, role, gout, dx, dY, dEdr, dw);
@@ -84,18 +86,84 @@ static int bwd_kind(bool table, bool need_dx, const ConvArgs& a, const ConvRole&
     return launch_bwd_one<Kind, MUL, 1, 16, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
 }
 
+// The runtime-width kernels (MUL = 0): the same lane mapping, chosen from role.mul at launch.  A width that
+// spans several CTAs (grid.y > 1, e.g. 96 or 256) makes the backward add its per-edge sums atomically.
+template <class Kind, int MAXNV>
+static int fwd_kind_rt(bool table, const ConvArgs& a, const ConvRole& role, float* out, cudaStream_t st) {
+  if (role.mul <= 0 || role.mul % 32 != 0) return kConvWrongMul;
+  if constexpr (MAXNV >= 2)
+    if (role.mul % 128 == 0) return launch_fwd_one<Kind, 0, MAXNV, 32>(table, a, role, out, st);
+  if (role.mul % 64 == 0) return launch_fwd_one<Kind, 0, 1, 32>(table, a, role, out, st);
+#if S7B_FWD_ODD_PAIRS
+  return launch_fwd_one<Kind, 0, 1, 16>(table, a, role, out, st);
+#else
+  return launch_fwd_scalar<Kind, 0>(table, a, role, out, st);
+#endif
+}
+
+template <class Kind, int MAXNV, bool ALLOW_NODX>
+static int bwd_kind_rt(bool table, bool need_dx, const ConvArgs& a, const ConvRole& role,
+                       const float* gout, float* dx, float* dY, float* dEdr, float* dw, cudaStream_t st) {
+  if (role.mul <= 0 || role.mul % 32 != 0) return kConvWrongMul;
+  if constexpr (MAXNV >= 2)
+    if (role.mul % 128 == 0)
+      return launch_bwd_one<Kind, 0, MAXNV, 32, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
+  if (role.mul % 64 == 0)
+    return launch_bwd_one<Kind, 0, 1, 32, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
+  return launch_bwd_one<Kind, 0, 1, 16, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
+}
+
+// Paths (l2, l3) of the kind (l1, lmax_filter, lmax_out): the triangle rule with l2 <= LF, l3 <= LO
+constexpr int tp_npath(int l1, int lf, int lo) {
+  int n = 0;
+  for (int l2 = 0; l2 <= lf; ++l2)
+    for (int l3 = (l1 > l2 ? l1 - l2 : l2 - l1); l3 <= l1 + l2; ++l3) n += l3 <= lo;
+  return n;
+}
+
+// One l1 role of a group.  MUL: the width its kernels are specialised for (kConvMul), 0 for none.  The
+// specialised kernel runs when role.mul == MUL, the runtime-width kernel otherwise; a role without paths
+// launches nothing.
+template <int L1, int LF, int LO, int MUL, int MAXNV>
+static int fwd_role(bool table, const ConvArgs& a, const ConvRole& role, float* out, cudaStream_t st) {
+  if constexpr (tp_npath(L1, LF, LO) == 0) {
+    return kConvNoPath;
+  } else {
+    if constexpr (MUL > 0)
+      if (role.mul == MUL) return fwd_kind<TPKind<L1, LF, LO>, MUL, MAXNV>(table, a, role, out, st);
+    return fwd_kind_rt<TPKind<L1, LF, LO>, MAXNV>(table, a, role, out, st);
+  }
+}
+
+template <int L1, int LF, int LO, int MUL, int MAXNV>
+static int bwd_role(bool table, bool need_dx, const ConvArgs& a, const ConvRole& role,
+                    const float* gout, float* dx, float* dY, float* dEdr, float* dw, cudaStream_t st) {
+  constexpr bool ALLOW_NODX = L1 == 0;
+  if constexpr (tp_npath(L1, LF, LO) == 0) {
+    return kConvNoPath;
+  } else {
+    if constexpr (MUL > 0)
+      if (role.mul == MUL)
+        return bwd_kind<TPKind<L1, LF, LO>, MUL, MAXNV, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
+    return bwd_kind_rt<TPKind<L1, LF, LO>, MAXNV, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
+  }
+}
+
 }  // namespace s7b
 
-// Defines  launch_conv_fwd_LF_LO / launch_conv_bwd_LF_LO  for l1 = 0..LF.
-#define S7B_DEFINE_CONV_GROUP(LF, LO)                                                              \
+// Defines  launch_conv_fwd_LF_LO / launch_conv_bwd_LF_LO  for l1 = 0..3.  SPEC = 1 for the groups of SevenNet-0
+// and SevenNet-l3i5, which also get the kernels specialised for the widths kConvMul (l1 = 3 only with LF = 3);
+// the other groups have only the runtime-width kernels.
+#define S7B_CONV_SPEC_MUL(SPEC, LF, L1) ((SPEC) && ((L1) < 3 || (LF) >= 3) ? s7b::kConvMul[L1] : 0)
+#define S7B_DEFINE_CONV_GROUP(LF, LO, SPEC)                                                        \
   namespace s7b {                                                                                  \
   int launch_conv_fwd_##LF##_##LO(int l1, bool table, const ConvArgs& a, const ConvRole& role,     \
                                   float* out, cudaStream_t st) {                                   \
     switch (l1) {                                                                                  \
-      case 0: return fwd_kind<TPKind<0, LF, LO>, kConvMul[0], S7B_FWD_L0_NV>(table, a, role, out, st);  \
-      case 1: return fwd_kind<TPKind<1, LF, LO>, kConvMul[1], 1>(table, a, role, out, st);              \
-      case 2: return fwd_kind<TPKind<2, LF, LO>, kConvMul[2], 1>(table, a, role, out, st);              \
-      case 3: return fwd_kind<TPKind<(LF >= 3 ? 3 : 2), LF, LO>, kConvMul[3], 1>(table, a, role, out, st); \
+      case 0: return fwd_role<0, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 0), S7B_FWD_L0_NV>(table, a, role, out, st); \
+      case 1: return fwd_role<1, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 1), 1>(table, a, role, out, st); \
+      case 2: return fwd_role<2, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 2), 1>(table, a, role, out, st); \
+      case 3: return fwd_role<3, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 3), 1>(table, a, role, out, st); \
     }                                                                                              \
     return 1;                                                                                      \
   }                                                                                                \
@@ -103,10 +171,10 @@ static int bwd_kind(bool table, bool need_dx, const ConvArgs& a, const ConvRole&
                                   const ConvRole& role, const float* gout, float* dx, float* dY,   \
                                   float* dEdr, float* dw, cudaStream_t st) {                       \
     switch (l1) {                                                                                  \
-      case 0: return bwd_kind<TPKind<0, LF, LO>, kConvMul[0], S7B_BWD_L0_NV, true>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);  \
-      case 1: return bwd_kind<TPKind<1, LF, LO>, kConvMul[1], 1, false>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
-      case 2: return bwd_kind<TPKind<2, LF, LO>, kConvMul[2], 1, false>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
-      case 3: return bwd_kind<TPKind<(LF >= 3 ? 3 : 2), LF, LO>, kConvMul[3], 1, false>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
+      case 0: return bwd_role<0, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 0), S7B_BWD_L0_NV>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
+      case 1: return bwd_role<1, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 1), 1>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
+      case 2: return bwd_role<2, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 2), 1>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
+      case 3: return bwd_role<3, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 3), 1>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
     }                                                                                              \
     return 1;                                                                                      \
   }                                                                                                \

@@ -26,10 +26,22 @@
 namespace s7b {
 
 constexpr int kConvWarpsPerBlock = 4;
-// Channels of the l1 = 0..3 blocks of x that the kernels are compiled for (those of SevenNet-0 and
-// SevenNet-l3i5).  The multiplicity is a template parameter, so that the component stride of x and the
-// table offsets are immediates; a model with other widths is refused when its layers are configured.
+// Channels of the l1 = 0..3 blocks of x that the kernels are specialised for (those of SevenNet-0 and
+// SevenNet-l3i5), in the (lmax_filter, lmax_out) groups (2, 2), (2, 0), (3, 3) and (3, 0); l1 = 3 only with
+// lmax_filter = 3.  The multiplicity is then a template parameter, so that the component stride of x and the
+// table offsets are immediates.  Every other width (any positive multiple of 32) and every other group runs the
+// runtime-width instantiation MUL = 0, which reads the width from ConvRole::mul (conv_dispatch.cuh).
 constexpr int kConvMul[kMaxL] = {128, 64, 32, 32};
+// Widest l1 block of x the engine accepts: keeps the kernels' 32-bit radial-table index (knot row * paths of the
+// role * channel pairs) far from overflow for any practical knot count.
+constexpr int kConvMaxMul = 1024;
+
+// Channels of a role: the compile-time width, or role.mul in the runtime-width instantiation (MUL = 0)
+template <int MUL>
+__device__ __forceinline__ int conv_mul(const ConvRole& role) {
+  if constexpr (MUL > 0) return MUL;
+  else return role.mul;
+}
 // Register budget, as the min-resident-CTAs argument of __launch_bounds__ (128-thread CTAs: 4 -> 128
 // registers, 3 -> 168, 1 -> 255).  Chosen by A/B timing on the previous GPU generation (7net-0, 12k atoms;
 // not re-tuned on H100):
@@ -39,6 +51,9 @@ constexpr int kConvMul[kMaxL] = {128, 64, 32, 32};
 //    l1 >= 2 at 3 (what ptxas picks by itself).  The l1 = 0 kernel without dx (first layer) at 4: it fits
 //    in 122 registers without spilling; at 3 it took 138 and 0.245 instead of 0.22 ms (H100, 700 W).  The
 //    lmax = 3 kinds need > 168 registers (they spill otherwise) and are left at 2.
+//  * runtime-width backward (MUL = 0), from -Xptxas -v: the l1 >= 1 kernels at 2 (at 3 or 4 the lmax_filter = 2
+//    kinds spill 4-156 bytes: the runtime stride and split flag cost registers, and lmax_out = 3 adds paths);
+//    l1 = 0 as above, which does not spill.
 #ifndef S7B_FWD_MINBLOCKS
 #define S7B_FWD_MINBLOCKS 1
 #endif
@@ -46,7 +61,8 @@ constexpr int kConvMul[kMaxL] = {128, 64, 32, 32};
 #ifdef S7B_BWD_MINBLOCKS
 #define S7B_BWD_BOUNDS __launch_bounds__(32 * kConvWarpsPerBlock, S7B_BWD_MINBLOCKS)
 #else
-#define S7B_BWD_BOUNDS __launch_bounds__(32 * kConvWarpsPerBlock, (Kind::NY != 9) ? 2 : ((Kind::D1 == 3 || !NEED_DX) ? 4 : 3))
+#define S7B_BWD_BOUNDS __launch_bounds__(32 * kConvWarpsPerBlock, \
+    (Kind::NY != 9 || (MUL == 0 && Kind::D1 > 1)) ? 2 : ((Kind::D1 == 3 || !NEED_DX) ? 4 : 3))
 #endif
 #ifndef S7B_COOP_REC
 #define S7B_COOP_REC 1   // lanes of a group fetch the records of LPN consecutive edges at once (see EdgeRecs)
@@ -187,13 +203,15 @@ struct LaneMap {
 // forward:  out[n, path block] = sum_{e in row n} w_e * CG(x[src_e], Y_e)
 // grid = (ceil(n_dst / (kConvWarpsPerBlock * 32/LPN)), MUL / (CH*LPN*NV)), block = 32*kConvWarpsPerBlock
 // MUL (= role.mul) is a compile-time constant: the component stride of x and the table offsets of the paths
-// become immediates, and each edge costs one x address and one table address per lane.
+// become immediates, and each edge costs one x address and one table address per lane.  MUL = 0 reads the
+// width from role.mul (runtime-width instantiation; role.mul must be a multiple of CH*LPN*NV).
 // ------------------------------------------------------------------------------------------
 template <class Kind, int MUL, int NV, int LPN, bool TABLE, class V>
 __global__ void S7B_FWD_BOUNDS
 conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) {
   constexpr int CH = VT<V>::CH;
   static_assert(MUL % (CH * LPN * NV) == 0, "channels must fill whole lane groups");
+  const int mul = conv_mul<MUL>(role);
   const LaneMap<NV, LPN, CH> m(a);
   if (m.nmax == 0 && !m.node_ok) return;      // whole warp beyond the last node (uniform)
 
@@ -219,7 +237,7 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
     float Y[Kind::NY];
     load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
     const float* __restrict__ xrow = a.x + (row_offset(rec.x, a.dim_x) + xlane);
-    const unsigned ti = tlane + rec.y * (Kind::NPATH * MUL / 2);   // knot row of the role's table image
+    const unsigned ti = tlane + rec.y * (Kind::NPATH * mul / 2);   // knot row of the role's table image
     const float4* __restrict__ k01 = a.table + ti;
     const uint2* __restrict__ k23 = a.table23 + ti;
     const float tt = __int_as_float(rec.z);
@@ -228,12 +246,12 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
       const int u = CH * LPN * c;                        // channel offset from m.uc0
       V x[Kind::D1], w[Kind::NPATH];
 #pragma unroll
-      for (int i = 0; i < Kind::D1; ++i) x[i] = VT<V>::load(xrow + i * MUL + u);
+      for (int i = 0; i < Kind::D1; ++i) x[i] = VT<V>::load(xrow + i * mul + u);
 #pragma unroll
       for (int p = 0; p < Kind::NPATH; ++p) {
         if (TABLE) {
           V a0, a1, a2, a3;
-          VT<V>::coef(k01 + (p * (MUL / 2) + u / 2), k23 + (p * (MUL / 2) + u / 2), odd, a0, a1, a2, a3);
+          VT<V>::coef(k01 + (p * (mul / 2) + u / 2), k23 + (p * (mul / 2) + u / 2), odd, a0, a1, a2, a3);
           w[p] = fma_(tt, fma_(tt, fma_(tt, a3, a2), a1), a0);
         } else {
           w[p] = VT<V>::load(a.w + (size_t)e * a.w_numel + role.w_off[p] + m.uc0 + u);
@@ -289,6 +307,7 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
 //   dx[src_e, :]        += dE/dx                                          (RED.ADD.F32x2, NEED_DX)
 // dY_acc / dEdr_acc / dw rows are owned by exactly one group of one launch: plain read-modify-write,
 // unless the role's channels are spread over several CTAs (SPLIT, gridDim.y > 1): then they are added atomically.
+// MUL = 0 (runtime width, role.mul): SPLIT is read from the launch geometry.
 // ------------------------------------------------------------------------------------------
 template <class Kind, int MUL, int NV, int LPN, bool TABLE, bool NEED_DX>
 __global__ void S7B_BWD_BOUNDS
@@ -296,7 +315,8 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
                 float* __restrict__ dx, float* __restrict__ dY_acc, float* __restrict__ dEdr_acc,
                 float* __restrict__ dw) {
   static_assert(MUL % (2 * LPN * NV) == 0, "channels must fill whole lane groups");
-  constexpr bool SPLIT = MUL > 2 * LPN * NV;
+  const int mul = conv_mul<MUL>(role);
+  const bool SPLIT = (MUL > 0) ? (MUL > 2 * LPN * NV) : (gridDim.y > 1);
   const LaneMap<NV, LPN, 2> m(a);
   if (m.nmax == 0) return;                    // uniform: no edges in any row of this warp
 
@@ -335,7 +355,7 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
     float Y[Kind::NY];
     load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
     const size_t xo = row_offset(rec.x, a.dim_x) + xlane;
-    const unsigned ti = tlane + rec.y * (Kind::NPATH * MUL / 2);   // knot row of the role's table image
+    const unsigned ti = tlane + rec.y * (Kind::NPATH * mul / 2);   // knot row of the role's table image
     const float4* __restrict__ k01 = a.table + ti;
     const uint2* __restrict__ k23 = a.table23 + ti;
     const float tt = __int_as_float(rec.z);
@@ -348,12 +368,12 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
       const int u = 2 * LPN * c;                         // channel offset from m.uc0
       V2 x[Kind::D1], w[Kind::NPATH], wd[Kind::NPATH], dwv[Kind::NPATH], dxv[Kind::D1];
 #pragma unroll
-      for (int i = 0; i < Kind::D1; ++i) x[i] = ldg2(a.x + xo + (i * MUL + u));
+      for (int i = 0; i < Kind::D1; ++i) x[i] = ldg2(a.x + xo + (i * mul + u));
 #pragma unroll
       for (int p = 0; p < Kind::NPATH; ++p) {
         if (TABLE) {
-          const float4 c01 = __ldg(k01 + (p * (MUL / 2) + u / 2));
-          const uint2 c23 = __ldg(k23 + (p * (MUL / 2) + u / 2));
+          const float4 c01 = __ldg(k01 + (p * (mul / 2) + u / 2));
+          const uint2 c23 = __ldg(k23 + (p * (mul / 2) + u / 2));
           const V2 a0 = make_float2(c01.x, c01.y), a1 = make_float2(c01.z, c01.w);
           const V2 a2 = __half22float2(*reinterpret_cast<const __half2*>(&c23.x));
           const V2 a3 = __half22float2(*reinterpret_cast<const __half2*>(&c23.y));
@@ -373,7 +393,7 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
         if (NEED_DX) {
 #pragma unroll
           for (int i = 0; i < Kind::D1; ++i)
-            atomicAdd(reinterpret_cast<float2*>(dx + xo + (i * MUL + u)), dxv[i]);
+            atomicAdd(reinterpret_cast<float2*>(dx + xo + (i * mul + u)), dxv[i]);
         }
       }
     }

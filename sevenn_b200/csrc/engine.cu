@@ -231,17 +231,20 @@ static int irreps_dim(const int* muls, int n_l) {
 }
 
 // Restates build_layer() of sevenn_b200/spec.py (reference convolution.py:61-82 path order).  knots: rows of the
-// radial table (0 without one), which places the per-role table images (ConvRole::tab_off).
+// radial table (0 without one), which places the per-role table images (ConvRole::tab_off).  layer: for messages
+// (-1: the operator-level plug-in).  The convolution runs any width of x that is a positive multiple of 32: the
+// widths kConvMul of SevenNet-0 / SevenNet-l3i5 on specialised kernels, every other on the runtime-width ones.
 static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* out_muls, int n_lo,
-                           int lmax_filter, int knots) {
+                           int lmax_filter, int knots, int layer) {
   L.n_lx = n_lx;
   L.n_lg = n_lo;
   L.lmax_out = n_lo - 1;
   int off = 0;
   for (int l = 0; l < n_lx; ++l) {
-    if (x_muls[l] != kConvMul[l])
-      return fail("the convolution kernels are compiled for " + std::to_string(kConvMul[l]) + " channels of l = " +
-                  std::to_string(l) + " in x, not " + std::to_string(x_muls[l]) + " (conv_kernels.cuh kConvMul)");
+    if (x_muls[l] <= 0 || x_muls[l] % 32 != 0 || x_muls[l] > kConvMaxMul)
+      return fail("convolution multiplicities must be positive multiples of 32, at most " +
+                  std::to_string(kConvMaxMul) + ": " + (layer >= 0 ? "layer " + std::to_string(layer) : std::string("x")) +
+                  " has " + std::to_string(x_muls[l]) + " channels of l = " + std::to_string(l));
     L.x_muls[l] = x_muls[l];
     L.x_off[l] = off;
     off += (2 * l + 1) * x_muls[l];
@@ -860,7 +863,7 @@ int s7b_engine_create(const S7bModelDesc* d, S7bEngine** out) {
       return fail("irreps lmax out of range");
     }
     if (build_layer_cfg(e->layers[t], d->muls[t], d->n_l[t], d->muls[t + 1], d->n_l[t + 1], d->lmax_filter,
-                        std::max(d->table_knots, 0))) {
+                        std::max(d->table_knots, 0), t)) {
       delete e;
       return 1;
     }
@@ -1955,7 +1958,7 @@ int s7b_conv_plan_create(int32_t n_l_x, const int32_t* x_muls, int32_t lmax_filt
     return fail("irreps out of the supported range (l <= 3)");
   S7bConvPlan* p = new S7bConvPlan();
   int out_muls[kMaxL] = {32, 32, 32, 32};   // only lmax_out matters for the path set
-  if (build_layer_cfg(p->cfg, x_muls, n_l_x, out_muls, lmax_out + 1, lmax_filter, 0)) {
+  if (build_layer_cfg(p->cfg, x_muls, n_l_x, out_muls, lmax_out + 1, lmax_filter, 0, -1)) {
     delete p;
     return 1;
   }

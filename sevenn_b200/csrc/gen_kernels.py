@@ -31,16 +31,24 @@ sys.path.insert(0, os.path.join(HERE, '..', '..'))
 from sevenn_b200.cg import tp_path_coefficients  # noqa: E402
 from sevenn_b200.sh import sh_polynomials, X, Y, Z  # noqa: E402
 
-KINDS: List[Tuple[int, int, int]] = (
-    [(l1, 2, 2) for l1 in range(3)] + [(l1, 2, 0) for l1 in range(3)]       # SevenNet-0
-    + [(l1, 3, 3) for l1 in range(4)] + [(l1, 3, 0) for l1 in range(4)]     # SevenNet-l3i5
-)
-
-
 def kind_paths(l1: int, lf: int, lo: int) -> List[Tuple[int, int]]:
     """(l2, l3) in slot order restricted to this l1: sorted by l3, then by creation (l2)."""
     ps = [(l2, l3) for l2 in range(lf + 1) for l3 in range(abs(l1 - l2), l1 + l2 + 1) if l3 <= lo]
     return sorted(ps, key=lambda p: (p[1], p[0]))
+
+
+# (lmax_filter, lmax_out) groups: each is one translation unit, conv_group_<LF><LO>.cu
+GROUPS: List[Tuple[int, int]] = [(lf, lo) for lf in (1, 2, 3) for lo in range(4)]
+# the groups of SevenNet-0 and SevenNet-l3i5, which also have kernels specialised for their widths (kConvMul)
+SPECIALISED_GROUPS: List[Tuple[int, int]] = [(2, 2), (2, 0), (3, 3), (3, 0)]
+
+KINDS: List[Tuple[int, int, int]] = (
+    [(l1, 2, 2) for l1 in range(3)] + [(l1, 2, 0) for l1 in range(3)]       # SevenNet-0
+    + [(l1, 3, 3) for l1 in range(4)] + [(l1, 3, 0) for l1 in range(4)]     # SevenNet-l3i5
+)
+# every other kind with at least one path: x of l1 <= 3, every group (a role without paths launches nothing)
+KINDS += [(l1, lf, lo) for (lf, lo) in GROUPS for l1 in range(4)
+          if (l1, lf, lo) not in KINDS and kind_paths(l1, lf, lo)]
 
 
 def _f(v: float) -> str:

@@ -9,10 +9,14 @@ bytes from `-Xptxas -v`.  One iteration handles one edge of a row, or two with 1
 half warp).  The counts are static: every instruction of the loop body once, including the edge-record refill
 that runs once per 16 or 32 edges.
 
-    python tools/conv_sass_budget.py [--groups 22 20 33 30] [--all]
+    python tools/conv_sass_budget.py [--groups 22 20 33 30 ...] [--all]
 
 By default only the kernels the engine launches in table mode are listed (table radial weights; backward
-with dx, and without dx for l1 = 0 as the first layer uses it); --all lists every instantiation.
+with dx, and without dx for l1 = 0 as the first layer uses it); --all lists every instantiation.  The groups
+default to all twelve (lmax_filter 1..3, lmax_out 0..3).  The first template argument after the kind is the
+channel width: 128 / 64 / 32 for the kernels specialised to SevenNet-0 / SevenNet-l3i5, 0 for the runtime-width
+kernels (any multiple of 32, read from ConvRole::mul), so the groups 22 / 20 / 33 / 30 list the same kind at its
+compiled and at the runtime width side by side.
 """
 import argparse
 import os
@@ -103,14 +107,12 @@ def launched_in_table_mode(kind, l1, args):
         return False
     if kind == 'bwd' and len(flags) > 1 and flags[1] != 'true' and l1 != 0:
         return False
-    if kind == 'bwd' and len(flags) > 2 and flags[2] == 'true':       # atomic split variant (unused at these widths)
-        return False
     return True
 
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
-    ap.add_argument('--groups', nargs='+', default=['22', '20', '33', '30'],
+    ap.add_argument('--groups', nargs='+', default=[f'{lf}{lo}' for lf in (1, 2, 3) for lo in range(4)],
                     help='(lmax_filter, lmax_out) groups, as in conv_group_<LFLO>.cu')
     ap.add_argument('--all', action='store_true', help='every instantiation, not only those table mode launches')
     args = ap.parse_args()
