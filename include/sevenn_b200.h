@@ -132,6 +132,15 @@ S7B_API int s7b_block_linear(const float* A, int32_t lda, int32_t n_nodes, int32
                              const int32_t* a_K, const float* W_host, float* C, int32_t ldc, const int32_t* c_off,
                              const int32_t* c_N, int32_t accumulate, int32_t use_tc, void* stream);
 
+/* Test / utility entry: one species-wise block-diagonal linear  C_l[n] (+)= A_l[n] * W_l[species[n]]  (block l has 2l+1
+ * rows per node, l < n_l) through the engine's kernels: the counting sort of the rows by species, then the
+ * species-segmented GEMM the 'nequip' self-connection runs on.  A, C and species[n_rows] are device pointers, W a host
+ * pointer laid out [num_species][l block][K_l][N_l].  Rows whose species lies outside [0, num_species) are not written.
+ * K_l, N_l, the offsets and lda / ldc must be multiples of 4. */
+S7B_API int s7b_species_linear(const float* A, int32_t lda, int32_t n_rows, const int32_t* species, int32_t num_species,
+                               int32_t n_l, const int32_t* a_off, const int32_t* a_K, const float* W_host, float* C,
+                               int32_t ldc, const int32_t* c_off, const int32_t* c_N, int32_t accumulate, void* stream);
+
 /* Debug aid: timeline (role, event, index, clock64) of CTA 0 of the following tensor-core linear launches,
  * written to a device buffer of 8 + 3 * cap int64 (words 1..5 = records of each of the five roles, then cap / 5
  * records {event, index, clock64} per role); cap = 0 switches it off. */
@@ -153,7 +162,9 @@ S7B_API int s7b_engine_set_atomic_virial(S7bEngine* eng, int enable);
 
 /* Upload one named parameter array (host pointer, fp32).  Names: "embed_x0", "embed_g0",
  * "readout" (+ optional "readout_lo", the fp32 residual of the fp64 fold), "scale", "shift", "bessel", and per layer t "si1", "si1T", "sc", "scT", "si2",
- * "si2T", "table", "mlp0".."mlp2", "mlp0T".."mlp2T" (layouts: sevenn_b200/engine.py). */
+ * "si2T", "table", "mlp0".."mlp2", "mlp0T".."mlp2T" (layouts: sevenn_b200/engine.py).  A layer with the species-wise
+ * ('nequip') self-connection takes "sc_species" / "scT_species" ([num_species][l block][K][N], the transpose per block)
+ * instead of "sc" / "scT"; setting both kinds on one layer is an error. */
 S7B_API int s7b_engine_set_param(S7bEngine* eng, const char* name, int layer, const float* host, size_t numel);
 
 /* Describe the graph of this step (device pointers, kept by reference until the next call).

@@ -26,7 +26,7 @@ from typing import Dict, Tuple
 import numpy as np
 
 from .cg import wigner_3j
-from .spec import ModelSpec, build_spec, parse_even_irreps
+from .spec import ModelSpec, build_spec, check_sc_weight, parse_even_irreps, sc_numel
 
 
 def _version_tuple(v: str) -> Tuple[int, ...]:
@@ -79,8 +79,13 @@ def convert_reference_checkpoint(path: str, name: str) -> Tuple[dict, Dict[str, 
 
     if cfg.get('is_parity', False):
         raise NotImplementedError('is_parity: True checkpoints are out of scope (SURVEY 0.9)')
-    if cfg.get('self_connection_type', 'nequip') != 'linear':
-        raise NotImplementedError("only self_connection_type 'linear' is supported")
+    sc_type = cfg.get('self_connection_type', 'nequip')     # _const.py default
+    if isinstance(sc_type, (list, tuple)):                   # one entry per layer is allowed by the reference
+        if len(set(sc_type)) != 1:
+            raise NotImplementedError(f'self_connection_type must be the same in every layer, got {list(sc_type)}')
+        sc_type = sc_type[0]
+    if sc_type not in ('linear', 'nequip'):
+        raise NotImplementedError(f"self_connection_type {sc_type!r} is not supported (only 'linear' and 'nequip')")
     if cfg.get('use_bias_in_linear', False):
         raise NotImplementedError('use_bias_in_linear is not supported')
     if cfg.get('use_modality', False):
@@ -120,6 +125,7 @@ def convert_reference_checkpoint(path: str, name: str) -> Tuple[dict, Dict[str, 
         chemical_species=list(cfg['chemical_species']),
         radial_hidden=[int(h) for h in cfg['weight_nn_hidden_neurons']],
         irreps_per_layer=irreps, readout_hidden=parse_even_irreps(irreps[-1])[0] // 2,
+        self_connection=sc_type,
     )
     spec = build_spec(meta)
 
@@ -143,7 +149,10 @@ def convert_reference_checkpoint(path: str, name: str) -> Tuple[dict, Dict[str, 
     n_mlp = len(spec.radial_hidden) + 1
     for L in spec.layers:
         t = L.t
-        arrays[f'{t}.sc'] = get(f'{t}_self_connection_intro.linear.weight')
+        # 'nequip': FullyConnectedTensorProduct(x, S x0e, gate_in) weight, blocks [mul_in, S, mul_out] per l
+        sc_key = 'fc_tensor_product.weight' if sc_type == 'nequip' else 'linear.weight'
+        arrays[f'{t}.sc'] = get(f'{t}_self_connection_intro.{sc_key}').reshape(-1)
+        check_sc_weight(L, sc_type, spec.num_species, arrays[f'{t}.sc'].size)
         arrays[f'{t}.si1'] = get(f'{t}_self_interaction_1.linear.weight')
         arrays[f'{t}.si2'] = get(f'{t}_self_interaction_2.linear.weight')
         arrays[f'{t}.den'] = get(f'{t}_convolution.denominator').reshape(1)
@@ -212,7 +221,10 @@ def random_weights(meta: dict, seed: int = 0) -> Dict[str, np.ndarray]:
     hs = [spec.n_basis] + list(spec.radial_hidden)
     for L in spec.layers:
         t = L.t
-        arrays[f'{t}.sc'] = lin(L.x_muls, L.gate_muls)
+        if spec.self_connection == 'nequip':
+            arrays[f'{t}.sc'] = rng.standard_normal(sc_numel(L, 'nequip', S)).astype(np.float32)
+        else:
+            arrays[f'{t}.sc'] = lin(L.x_muls, L.gate_muls)
         arrays[f'{t}.si1'] = lin(L.x_muls, L.x_muls)
         si2 = []
         for l3, K in enumerate(L.mid_K):

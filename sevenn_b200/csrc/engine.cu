@@ -186,6 +186,10 @@ struct S7bEngine {
   int64_t nl_n_edges = 0;
   // structures of the current graph when s7b_engine_set_positions_batch installed it (0 otherwise)
   int n_systems = 0;
+  // species segmentation of the local rows (species_segment_kernel), rebuilt by every FWD_BEGIN when a layer has
+  // the species-wise ('nequip') self-connection: seg_perm [n_local], seg [2 * num_species + 2]
+  bool species_sc = false;
+  DevBuf seg_perm, seg;
   DevBuf sys_atom_ptr;
   Profiler prof;
   // side streams: the per-l1 convolution kernels of one layer are independent (disjoint outputs) and
@@ -648,6 +652,50 @@ static int irreps_linear(const float* A, int lda, const int* a_off, const int* a
   return launch_gemm(a, st);
 }
 
+// Species-wise block-diagonal linear over the rows of a species segmentation (perm, seg of species_segment_kernel
+// over n_rows rows): C_l[n] (+)= A_l[n] * W_l[species(n)] for l < n_l, W laid out [species][l block][K_l][N_l].
+static int launch_species_linear(const float* A, int lda, const int* a_off, const int* a_K, float* C, int ldc,
+                                 const int* c_off, const int* c_N, int n_l, const float* W, int S, const int* perm,
+                                 const int* seg, int n_rows, bool accumulate, cudaStream_t st) {
+  SpLinArgs a;
+  memset(&a, 0, sizeof(a));
+  a.A = A;
+  a.C = C;
+  a.W = W;
+  a.perm = perm;
+  a.seg = seg;
+  a.S = S;
+  a.lda = lda;
+  a.ldc = ldc;
+  a.accumulate = accumulate ? 1 : 0;
+  if (lda % 4 != 0 || ldc % 4 != 0 || (reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(C)) % 16 != 0)
+    return fail("species linear: rows must be 16-byte aligned");
+  int woff = 0, zs = 0, max_n = 0;
+  for (int l = 0; l < n_l; ++l) {
+    if (a_K[l] % 4 != 0 || c_N[l] % 4 != 0 || a_off[l] % 4 != 0 || c_off[l] % 4 != 0)
+      return fail("species linear: block sizes and offsets must be multiples of 4");
+    if (a_K[l] != 0 && c_N[l] != 0) {
+      SpLinBlock& b = a.blk[a.nblocks++];
+      b = SpLinBlock{woff, 2 * l + 1, a_K[l], c_N[l], a_off[l], a_K[l], c_off[l], c_N[l]};
+      zs += 2 * l + 1;
+      max_n = std::max(max_n, c_N[l]);
+    }
+    woff += a_K[l] * c_N[l];
+  }
+  a.w_stride = woff;
+  if (n_rows <= 0 || a.nblocks == 0) return 0;
+  dim3 grid((n_rows + kSpTileRows - 1) / kSpTileRows + S, (max_n + kSpBN - 1) / kSpBN, zs);
+  species_linear_kernel<<<grid, kSpThreads, 0, st>>>(a);
+  S7B_LAUNCH_CHECK();
+  return 0;
+}
+
+static int launch_species_segment(const int* species, int n, int S, int* perm, int* seg, cudaStream_t st) {
+  species_segment_kernel<<<1, 1024, 2 * S * sizeof(int), st>>>(species, n, S, perm, seg);
+  S7B_LAUNCH_CHECK();
+  return 0;
+}
+
 // One block-diagonal node linear of layer `L`, parameter `name`: tensor cores when the shapes allow it
 // (default), else the FP32 SIMT kernel.  `re` holds the row exponents of A; `fresh_re` = compute them now
 // over the n_l_A irrep blocks of A (a later call on the same A reuses them).
@@ -836,6 +884,35 @@ int s7b_block_linear(const float* A, int32_t lda, int32_t n_nodes, int32_t n_l, 
   return rc;
 }
 
+// Test / utility entry: one species-wise block-diagonal linear  C_l[n] (+)= A_l[n] W_l[species[n]]  (l < n_l, 2l+1
+// rows per node) through the engine's segmentation and species_linear_kernel.  A, C, species device pointers; W host
+// pointer laid out [num_species][l block][K_l][N_l].
+int s7b_species_linear(const float* A, int32_t lda, int32_t n_rows, const int32_t* species, int32_t num_species, int32_t n_l,
+                       const int32_t* a_off, const int32_t* a_K, const float* W_host, float* C, int32_t ldc,
+                       const int32_t* c_off, const int32_t* c_N, int32_t accumulate, void* stream) {
+  if (!W_host || !a_off || !a_K || !c_off || !c_N) return fail("null argument");
+  if (n_l < 1 || n_l > kMaxL || n_rows < 0 || num_species < 1 || num_species > kMaxSpeciesSc) return fail("bad sizes");
+  if (n_rows > 0 && (!A || !C || !species)) return fail("null argument");
+  if (n_rows == 0) return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  size_t wn = 0;
+  for (int l = 0; l < n_l; ++l) wn += (size_t)a_K[l] * c_N[l];
+  wn *= num_species;
+  DevBuf dW, perm, seg;
+  int rc = 0;
+  if (dW.ensure(wn * sizeof(float)) || perm.ensure((size_t)n_rows * sizeof(int)) || seg.ensure((2 * (size_t)num_species + 2) * sizeof(int)))
+    rc = fail("cudaMalloc failed");
+  if (!rc && cudaMemcpyAsync(dW.p, W_host, wn * sizeof(float), cudaMemcpyHostToDevice, st) != cudaSuccess) rc = fail("cudaMemcpy failed");
+  if (!rc) rc = launch_species_segment(species, n_rows, num_species, perm.as<int>(), seg.as<int>(), st);
+  if (!rc) rc = launch_species_linear(A, lda, a_off, a_K, C, ldc, c_off, c_N, n_l, dW.as<float>(), num_species, perm.as<int>(),
+                                      seg.as<int>(), n_rows, accumulate != 0, st);
+  cudaStreamSynchronize(st);
+  dW.release();
+  perm.release();
+  seg.release();
+  return rc;
+}
+
 // Host-only: the tensor-core weight packing of tc_gemm.cuh for one [K, N] block (tests/test_tc_pack_cpu.py).
 // q: 3*K*NT*ceil(N/NT) uint16 (bf16 bits; caller allocates 3*K*(N+127) and zero-fills), laid out
 // [n tile][K/32][slice][canonical NT x 32]; fb: N floats; *NT_out = tile width.
@@ -925,6 +1002,8 @@ void s7b_engine_destroy(S7bEngine* e) {
       if (kv.second) { kv.second->q.release(); kv.second->fb.release(); delete kv.second; }
   }
   for (RowExp* r : {&e->re_mid, &e->re_h, &e->re_dg, &e->re_dx}) r->buf.release();
+  e->seg_perm.release();
+  e->seg.release();
   DevBuf* bufs[] = {&e->rec, &e->Y, &e->rlen, &e->emb, &e->dY_acc, &e->dEdr_acc, &e->demb_acc, &e->fedge,
                     &e->mid, &e->h, &e->dh, &e->dg, &e->dx, &e->dwbuf, &e->tmpA, &e->tmpB, &e->energy,
                     &e->atomic_energy, &e->forces, &e->virial, &e->atomic_virial, &e->hs_species, &e->hs_rowptr, &e->hs_src,
@@ -948,6 +1027,33 @@ int s7b_engine_set_atomic_virial(S7bEngine* e, int enable) {
 int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float* host, size_t numel) {
   if (!e || !name || !host) return fail("null argument");
   const std::string nm(name);
+  if (nm == "sc_species" || nm == "scT_species") {
+    // species-wise ('nequip') self-connection: [num_species][l block][K][N] (scT_species: each block transposed)
+    if (layer < 0 || layer >= e->desc.n_layers) return fail("parameter " + nm + " needs a layer in [0, n_layers)");
+    const LayerCfg& L = e->layers[layer];
+    if (L.params.count("sc") || L.params.count("scT"))
+      return fail("layer " + std::to_string(layer) + ": parameter " + nm + " and the linear self-connection 'sc' / 'scT' cannot both be set");
+    const int S = e->desc.num_species;
+    if (S < 1 || S > kMaxSpeciesSc) return fail("parameter " + nm + ": num_species must be 1.." + std::to_string(kMaxSpeciesSc));
+    size_t per = 0;
+    for (int l = 0; l < std::min(L.n_lx, L.n_lg); ++l) per += (size_t)L.x_muls[l] * L.g_muls[l];
+    if (numel != per * S)
+      return fail("layer " + std::to_string(layer) + ": parameter " + nm + " has " + std::to_string(numel) + " values, expected " +
+                  std::to_string(per * S) + " (num_species " + std::to_string(S) + " x " + std::to_string(per) + ")");
+    DevBuf& dst = e->layers[layer].params[nm];
+    if (dst.ensure(numel * sizeof(float))) return fail("cudaMalloc failed for parameter " + nm);
+    S7B_CUDA_CHECK(cudaMemcpy(dst.p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
+    if (!e->species_sc) {
+      e->species_sc = true;
+      if (e->seg.ensure((2 * (size_t)S + 2) * sizeof(int)) || e->seg_perm.ensure((size_t)std::max(e->n_local, 1) * sizeof(int)))
+        return fail("cudaMalloc failed for the species segmentation");
+      ++g_alloc_gen;
+    }
+    return 0;
+  }
+  if (layer >= 0 && (nm == "sc" || nm == "scT") && layer < e->desc.n_layers &&
+      (e->layers[layer].params.count("sc_species") || e->layers[layer].params.count("scT_species")))
+    return fail("layer " + std::to_string(layer) + ": parameter " + nm + " and the species-wise self-connection 'sc_species' / 'scT_species' cannot both be set");
   if (nm == "bessel") {
     if ((int)numel != e->desc.n_basis) return fail("bessel: wrong size");
     for (int b = 0; b < e->desc.n_basis; ++b) e->radial.coeffs[b] = host[b];
@@ -1065,6 +1171,7 @@ int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t
   rc |= e->dh.ensure(Nl * std::max(max_h, max_x) * sizeof(float));
   rc |= e->dg.ensure(Nl * max_g * sizeof(float));
   rc |= e->dx.ensure(Nn * max_x * sizeof(float));
+  if (e->species_sc) rc |= e->seg_perm.ensure(Nl * sizeof(int));
   // row exponents of the tensor-core GEMM inputs (at most 1+3+5+7 rows per node); sized here because the
   // step may be recorded into a CUDA graph, where cudaMalloc is not allowed
   for (RowExp* r : {&e->re_mid, &e->re_h, &e->re_dg, &e->re_dx}) rc |= r->buf.ensure(Nn * 16 * sizeof(int));
@@ -1143,6 +1250,12 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         S7B_CUDA_CHECK(cudaMemsetAsync(e->dY_acc.p, 0, (size_t)max_lx * Ecap * e->ny_stride * sizeof(float), st));
         S7B_CUDA_CHECK(cudaMemsetAsync(e->dEdr_acc.p, 0, (size_t)max_lx * Ecap * sizeof(float), st));
         if (!table) S7B_CUDA_CHECK(cudaMemsetAsync(e->demb_acc.p, 0, (size_t)E * e->desc.n_basis * sizeof(float), st));
+      }
+      if (e->species_sc && Nl > 0) {
+        // species segmentation of the local rows for the species-wise self-connection, rebuilt every step from the
+        // device species array (a replayed graph may see new species in the same buffer)
+        ProfScope ps(e->prof, st, "species_segment");
+        if (launch_species_segment(e->d_species, Nl, e->desc.num_species, e->seg_perm.as<int>(), e->seg.as<int>(), st)) return 1;
       }
       const LayerCfg& L0 = e->layers[0];
       const float* ex = gparam(e, "embed_x0");
@@ -1245,12 +1358,15 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
       if (Nl == 0 || t + 1 >= T) return 0;
       const LayerCfg& N = e->layers[t + 1];
       const float* sc = lparam(e, t + 1, "sc");
-      if (require(sc, "sc")) return 1;
+      const float* scs = lparam(e, t + 1, "sc_species");
+      if (!scs && require(sc, "sc")) return 1;
       ProfScope ps(e->prof, st, "sc_gemm", t + 1);
       // self_connection_intro of the next layer -> initial value of g[t+1]; independent of the ghost
       // exchange of x[t+1], so multi-GPU callers overlap the two
       S7B_CUDA_CHECK(cudaMemsetAsync(e->g[t + 1].p, 0, (size_t)Nl * N.dim_g * sizeof(float), st));
       const int n_sc = std::min(N.n_lx, N.n_lg);
+      if (scs) return launch_species_linear(e->h.as<float>(), N.dim_x, N.x_off, N.x_muls, e->g[t + 1].as<float>(), N.dim_g, N.g_off, N.g_muls,
+                                            n_sc, scs, e->desc.num_species, e->seg_perm.as<int>(), e->seg.as<int>(), Nl, false, st);
       if (node_linear(N, "sc", e->re_h, false, N.n_lx, e->h.as<float>(), N.dim_x, N.x_off, N.x_muls, e->g[t + 1].as<float>(), N.dim_g, N.g_off, N.g_muls, n_sc, sc, Nl, false, st)) return 1;
       return 0;
     }
@@ -1332,15 +1448,18 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
       if (t <= 0 || t >= T) return fail("BWD_LAYER_B needs 1 <= layer < n_layers");
       const LayerCfg& L = e->layers[t];
       if (Nl == 0) return 0;
-      const float *si1T = lparam(e, t, "si1T"), *scT = lparam(e, t, "scT");
-      if (require(si1T, "si1T") || require(scT, "scT")) return 1;
+      const float *si1T = lparam(e, t, "si1T"), *scT = lparam(e, t, "scT"), *scTs = lparam(e, t, "scT_species");
+      if (require(si1T, "si1T") || (!scTs && require(scT, "scT"))) return 1;
       // dE/dh(t) = dg(t) * sc^T + dx(t) * si1^T     (h(t) = gate output of layer t-1).  B1 (the self-
       // connection term) does not need the reverse ghost exchange of dx and can overlap it; B2 adds the rest.
       ProfScope ps(e->prof, st, "si1T_scT_gemm", t);
       if (stage != S7B_STAGE_BWD_LAYER_B2) {
         const int n_sc = std::min(L.n_lx, L.n_lg);
         S7B_CUDA_CHECK(cudaMemsetAsync(e->dh.p, 0, (size_t)Nl * L.dim_x * sizeof(float), st));
-        if (node_linear(L, "scT", e->re_dg, false, L.n_lg, e->dg.as<float>(), L.dim_g, L.g_off, L.g_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, n_sc, scT, Nl, false, st)) return 1;
+        if (scTs) {
+          if (launch_species_linear(e->dg.as<float>(), L.dim_g, L.g_off, L.g_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, n_sc, scTs,
+                                    e->desc.num_species, e->seg_perm.as<int>(), e->seg.as<int>(), Nl, false, st)) return 1;
+        } else if (node_linear(L, "scT", e->re_dg, false, L.n_lg, e->dg.as<float>(), L.dim_g, L.g_off, L.g_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, n_sc, scT, Nl, false, st)) return 1;
       }
       if (stage != S7B_STAGE_BWD_LAYER_B1) {
         if (node_linear(L, "si1T", e->re_dx, true, L.n_lx, e->dx.as<float>(), L.dim_x, L.x_off, L.x_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, L.n_lx, si1T, Nl, true, st)) return 1;

@@ -410,4 +410,167 @@ __global__ void readout_kernel(const float* __restrict__ h, const float* __restr
   }
 }
 
+// ---- species-wise linear: the 'nequip' self-connection (sevenn/nn/self_connection.py:11-67) -------------------
+// FullyConnectedTensorProduct(x, S x0e, gate_in) with the species one-hot as second operand is a block-diagonal
+// linear whose weight depends on the atom's species:  C_l[n] (+)= A_l[n] * W_l[species(n)].
+
+// Counting sort of rows [0, n) by species, one CTA (launched with 2 * S ints of dynamic shared memory):
+// perm[seg[s] .. seg[s+1]) lists the rows of species s, seg[S + 1 + s] is the first 64-row tile of species s and
+// seg[2S + 1] the tile count.  Rows whose species lies outside [0, S) are left out.  The order of the rows inside
+// one species is not fixed, which does not matter: every row of the linear is computed on its own.
+constexpr int kSpTileRows = 64;
+constexpr int kMaxSpeciesSc = 4096;     // 2 * S ints of shared memory in species_segment_kernel
+__global__ void __launch_bounds__(1024) species_segment_kernel(const int* __restrict__ species, int n, int S,
+                                                               int* __restrict__ perm, int* __restrict__ seg) {
+  extern __shared__ int sp_sm[];
+  int* cnt = sp_sm;
+  int* cur = sp_sm + S;
+  const int lane = threadIdx.x & 31;
+  for (int s = threadIdx.x; s < S; s += blockDim.x) cnt[s] = 0;
+  __syncthreads();
+  // lanes holding the same species add once per warp (a one-species cell would otherwise serialise on one counter)
+  for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+    const int i = i0 + threadIdx.x;
+    const int s = i < n ? __ldg(species + i) : -1;
+    const unsigned int peers = __match_any_sync(0xffffffffu, s);
+    if (s >= 0 && s < S && lane == __ffs(peers) - 1) atomicAdd(&cnt[s], __popc(peers));
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int off = 0, tile = 0;
+    for (int s = 0; s < S; ++s) {
+      cur[s] = off;
+      seg[s] = off;
+      seg[S + 1 + s] = tile;
+      off += cnt[s];
+      tile += (cnt[s] + kSpTileRows - 1) / kSpTileRows;
+    }
+    seg[S] = off;
+    seg[2 * S + 1] = tile;
+  }
+  __syncthreads();
+  for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+    const int i = i0 + threadIdx.x;
+    const int s = i < n ? __ldg(species + i) : -1;
+    const unsigned int peers = __match_any_sync(0xffffffffu, s);
+    const int leader = __ffs(peers) - 1;
+    int base = 0;
+    if (s >= 0 && s < S && lane == leader) base = atomicAdd(&cur[s], __popc(peers));
+    base = __shfl_sync(peers, base, leader);
+    if (s >= 0 && s < S) perm[base + __popc(peers & ((1u << lane) - 1u))] = i;
+  }
+}
+
+// One irrep block of the species-wise linear: W_l of species s at W + s * w_stride + w_off, [K, N] row-major.
+struct SpLinBlock {
+  int w_off;
+  int d;                // 2l+1 rows per node
+  int K, N;
+  int a_off, a_cs;
+  int c_off, c_cs;
+};
+
+struct SpLinArgs {
+  const float* A;
+  float* C;
+  const float* W;
+  long long w_stride;   // floats per species
+  const int* perm;      // species_segment_kernel output
+  const int* seg;
+  int S;
+  int lda, ldc;
+  int accumulate;       // 1: C += result
+  int nblocks;
+  SpLinBlock blk[kMaxL];
+};
+
+constexpr int kSpBN = 64, kSpBK = 16, kSpThreads = 256;
+
+// Tile: up to 64 rows of one species x 64 columns of one (block, component); 4 x 4 outputs per thread.
+// grid = (ceil(n / 64) + S, ceil(max N / 64), sum of 2l+1 over the blocks); tiles past the last one exit.  A rows
+// are read and C rows written through the permutation; every C element is written once, summed over K in a fixed
+// order, so a row's result does not depend on which other rows share its tile.  K, N, the offsets and the leading
+// dimensions are multiples of 4 (checked by the launcher).
+__global__ void __launch_bounds__(kSpThreads) species_linear_kernel(const SpLinArgs a) {
+  int z = blockIdx.z, bi = 0;
+  while (bi + 1 < a.nblocks && z >= a.blk[bi].d) { z -= a.blk[bi].d; ++bi; }
+  const SpLinBlock b = a.blk[bi];
+  const int comp = z;
+  const int col0 = blockIdx.y * kSpBN;
+  if (col0 >= b.N) return;
+  const int* tile0 = a.seg + a.S + 1;
+  const int tile = blockIdx.x;
+  if (tile >= __ldg(tile0 + a.S)) return;
+  int lo = 0, hi = a.S - 1;          // the species of this tile: the last s with tile0[s] <= tile
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(tile0 + mid) <= tile) lo = mid;
+    else hi = mid - 1;
+  }
+  const int s = lo;
+  const int r0 = __ldg(a.seg + s) + (tile - __ldg(tile0 + s)) * kSpTileRows;
+  const int nr = min(kSpTileRows, __ldg(a.seg + s + 1) - r0);
+  const float* W = a.W + (size_t)s * a.w_stride + b.w_off;
+
+  __shared__ __align__(16) float As[kSpBK][kSpTileRows + 4];
+  __shared__ __align__(16) float Bs[kSpBK][kSpBN];
+  const int tid = threadIdx.x;
+  const int tx = tid & 15, ty = tid >> 4;
+  const int a_row = tid >> 2, a_kq = tid & 3;          // A loader: row, k quad
+  const float* a_ptr = a_row < nr ? a.A + (size_t)__ldg(a.perm + r0 + a_row) * a.lda + b.a_off + comp * b.a_cs : nullptr;
+  const int b_k = tid >> 4, gc = col0 + (tid & 15) * 4;  // W loader: k, column quad
+
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+
+  float4 ra, rb;
+  auto load_tiles = [&](int k0) {
+    const int ka = k0 + a_kq * 4;
+    ra = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (a_ptr != nullptr && ka < b.K) ra = __ldg(reinterpret_cast<const float4*>(a_ptr + ka));
+    rb = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int kb = k0 + b_k;
+    if (kb < b.K && gc < b.N) rb = __ldg(reinterpret_cast<const float4*>(W + (size_t)kb * b.N + gc));
+  };
+  load_tiles(0);
+  for (int k0 = 0; k0 < b.K; k0 += kSpBK) {
+    As[a_kq * 4 + 0][a_row] = ra.x;
+    As[a_kq * 4 + 1][a_row] = ra.y;
+    As[a_kq * 4 + 2][a_row] = ra.z;
+    As[a_kq * 4 + 3][a_row] = ra.w;
+    *reinterpret_cast<float4*>(&Bs[b_k][(tid & 15) * 4]) = rb;
+    __syncthreads();
+    if (k0 + kSpBK < b.K) load_tiles(k0 + kSpBK);
+#pragma unroll
+    for (int k = 0; k < kSpBK; ++k) {
+      const float4 av = *reinterpret_cast<const float4*>(&As[k][ty * 4]);
+      const float4 bv = *reinterpret_cast<const float4*>(&Bs[k][tx * 4]);
+      const float aa[4] = {av.x, av.y, av.z, av.w}, bb[4] = {bv.x, bv.y, bv.z, bv.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(aa[i], bb[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+
+  const int c = col0 + tx * 4;
+  if (c >= b.N) return;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = ty * 4 + i;
+    if (r >= nr) continue;
+    float4* cp = reinterpret_cast<float4*>(a.C + (size_t)__ldg(a.perm + r0 + r) * a.ldc + b.c_off + comp * b.c_cs + c);
+    float4 v = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+    if (a.accumulate) {
+      const float4 o = *cp;
+      v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
+    }
+    *cp = v;
+  }
+}
+
 }  // namespace s7b

@@ -9,6 +9,8 @@ Weight preparation restates the normalisations the reference applies at run time
 modules (SURVEY Appendix A.5-A.7) and folds them into the arrays once, in float64:
   * ``o3.Linear``: 1/sqrt(fan_in) per output irrep (``sevenn/nn/linear.py:94-100``)
   * convolution ``x.div(denominator)`` (``sevenn/nn/convolution.py:135``) folded into self_interaction_2
+  * the 'nequip' self-connection (``sevenn/nn/self_connection.py:11-67``, a linear whose weight depends on the
+    atom's species): 1/sqrt(fan_in * num_species) per block; folded into ``embed_g0`` in layer 0
   * the two bias-free readout linears (``sevenn/model_build.py:102-123``) folded into one vector
   * the radial MLP ``FullyConnectedNet`` (``convolution.py:93-95,121``) either kept exact
     (``radial='mlp'``) or tabulated as cubic Hermite splines of the edge length (``radial='table'``)
@@ -22,7 +24,7 @@ from typing import Dict, Optional
 
 import numpy as np
 
-from .spec import SILU_NORM, ModelSpec, build_spec
+from .spec import SILU_NORM, ModelSpec, build_spec, check_sc_weight, sc_blocks
 
 _LIB_PATH = os.environ.get('S7B_LIB') or os.path.join(os.path.dirname(os.path.abspath(__file__)), 'lib', 'libsevenn_b200.so')
 _lib = None
@@ -60,7 +62,7 @@ EXPORTS = [
     's7b_engine_profile_count', 's7b_engine_profile_entry', 's7b_conv_plan_create',
     's7b_conv_plan_destroy', 's7b_conv_plan_dims', 's7b_conv_forward', 's7b_conv_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
-    's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results',
+    's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
 ]
 
 
@@ -89,6 +91,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_neighbor_rows_host.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp, ctypes.POINTER(i64), vp]
     lib.s7b_tc_trace_enable.argtypes = [i32, ctypes.POINTER(vp)]
     lib.s7b_block_linear.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, i32, i32, vp]
+    lib.s7b_species_linear.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp, vp, i32, vp]
     f64 = ctypes.c_double
     lib.s7b_d3_create.argtypes = [ctypes.POINTER(vp)]
     lib.s7b_d3_destroy.argtypes = [vp]
@@ -243,25 +246,46 @@ def prepare_params(spec: ModelSpec, arrays: Dict[str, np.ndarray], radial: str, 
         assert off == len(flat), (off, len(flat))
         return blocks
 
+    def sc_species_blocks(flat, L):
+        """split a 'nequip' self-connection weight (``FullyConnectedTensorProduct(x, S x0e, gate_in)``: blocks
+        [K, S, N] per l) into per-l [S, K, N] / sqrt(K * S), e3nn's 'element' path normalisation"""
+        blocks, off = [], 0
+        for k, n in sc_blocks(L):
+            blocks.append(f64(flat[off:off + k * S * n]).reshape(k, S, n).transpose(1, 0, 2) / math.sqrt(k * S))
+            off += k * S * n
+        return blocks
+
+    nequip = spec.self_connection == 'nequip'
     for L in spec.layers:
         t = L.t
         n_lx, n_lg = len(L.x_muls), len(L.gate_muls)
         si1 = lin_blocks(arrays[f'{t}.si1'], L.x_muls, L.x_muls, n_lx)
         n_sc = min(n_lx, n_lg)
-        sc = lin_blocks(arrays[f'{t}.sc'], L.x_muls, L.gate_muls, n_sc)
+        check_sc_weight(L, spec.self_connection, S, np.size(arrays[f'{t}.sc']))
+        if nequip:
+            sc = sc_species_blocks(arrays[f'{t}.sc'], L)
+        else:
+            sc = lin_blocks(arrays[f'{t}.sc'], L.x_muls, L.gate_muls, n_sc)
         den = float(arrays[f'{t}.den'][0])
         si2 = [b / den for b in lin_blocks(arrays[f'{t}.si2'], L.mid_K, L.gate_muls, n_lg)]
         if t == 0:
             x0 = h0 @ si1[0]
             g0 = np.zeros((S, L.dim_gate))
-            g0[:, :L.gate_muls[0]] = h0 @ sc[0]
+            if nequip:      # h0 depends on the species only: the whole self-connection is a per-species row
+                g0[:, :L.gate_muls[0]] = np.einsum('su,suw->sw', h0, sc[0])
+            else:
+                g0[:, :L.gate_muls[0]] = h0 @ sc[0]
             out[('embed_x0', -1)] = x0
             out[('embed_g0', -1)] = g0
         else:
             out[('si1', t)] = np.concatenate([b.ravel() for b in si1])
             out[('si1T', t)] = np.concatenate([b.T.ravel() for b in si1])
-            out[('sc', t)] = np.concatenate([b.ravel() for b in sc])
-            out[('scT', t)] = np.concatenate([b.T.ravel() for b in sc])
+            if nequip:      # [species][l block][K][N], and its per-block transpose for the backward
+                out[('sc_species', t)] = np.concatenate([b[s].ravel() for s in range(S) for b in sc])
+                out[('scT_species', t)] = np.concatenate([b[s].T.ravel() for s in range(S) for b in sc])
+            else:
+                out[('sc', t)] = np.concatenate([b.ravel() for b in sc])
+                out[('scT', t)] = np.concatenate([b.T.ravel() for b in sc])
         out[('si2', t)] = np.concatenate([b.ravel() for b in si2])
         out[('si2T', t)] = np.concatenate([b.T.ravel() for b in si2])
         if radial == 'table':

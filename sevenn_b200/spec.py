@@ -175,6 +175,7 @@ class ModelSpec:
     radial_hidden: Tuple[int, ...]
     layers: List[LayerSpec]
     readout_hidden: int
+    self_connection: str = 'linear'   # 'linear' (o3.Linear) | 'nequip' (species-wise FullyConnectedTensorProduct)
 
     @property
     def n_layers(self) -> int:
@@ -196,4 +197,36 @@ def build_spec(meta: dict) -> ModelSpec:
         num_species=int(meta['num_species']),
         type_map={int(k): int(v) for k, v in meta['type_map'].items()},
         radial_hidden=tuple(int(h) for h in meta['radial_hidden']), layers=layers,
-        readout_hidden=int(meta['readout_hidden']))
+        readout_hidden=int(meta['readout_hidden']), self_connection=self_connection_of(meta))
+
+
+SELF_CONNECTIONS = ('linear', 'nequip')
+
+
+def self_connection_of(meta: dict) -> str:
+    """The self-connection type a meta records; files written before the key existed are 'linear'."""
+    sc = str(meta.get('self_connection', 'linear'))
+    if sc not in SELF_CONNECTIONS:
+        raise NotImplementedError(f'self_connection {sc!r} is not supported (one of {SELF_CONNECTIONS})')
+    return sc
+
+
+def sc_blocks(L: LayerSpec) -> List[Tuple[int, int]]:
+    """(K, N) = (mul_in, mul_out) of the self-connection's weight blocks, l = 0 .. min(n_lx, n_lg) - 1, in weight
+    order: one block per l for both types (an e3nn o3.Linear, or the uvw instructions (l, 0e -> l) of
+    ``FullyConnectedTensorProduct(x, S x0e, gate_in)``, ``sevenn/nn/self_connection.py:11-67``)."""
+    n = min(len(L.x_muls), len(L.gate_muls))
+    return [(L.x_muls[l], L.gate_muls[l]) for l in range(n)]
+
+
+def sc_numel(L: LayerSpec, kind: str, num_species: int) -> int:
+    """Values of layer L's self-connection weight: sum K*N ('linear'), sum K*S*N ('nequip': blocks [K, S, N])."""
+    per = sum(k * n for k, n in sc_blocks(L))
+    return per * num_species if kind == 'nequip' else per
+
+
+def check_sc_weight(L: LayerSpec, kind: str, num_species: int, size: int) -> None:
+    want = sc_numel(L, kind, num_species)
+    if int(size) != want:
+        shape = ' + '.join(f'{k}x{num_species}x{n}' if kind == 'nequip' else f'{k}x{n}' for k, n in sc_blocks(L))
+        raise ValueError(f'layer {L.t}: the {kind} self-connection weight has {int(size)} values, expected {want} ({shape})')
