@@ -609,13 +609,19 @@ static int launch_tc_linear(const TcWeights& w, const RowExp& re, const float* A
 
 static int launch_gemm(const LinArgs& a, cudaStream_t st) {
   int max_rows = 0, max_n = 0;
+  // float4 loads need every A row (A + n*lda + a_off + i*a_cs) and every W row (W + k*N) on a 16-byte boundary
+  bool vec = a.lda % 4 == 0 && reinterpret_cast<uintptr_t>(a.A) % 16 == 0;
   for (int b = 0; b < a.nblocks; ++b) {
-    max_rows = std::max(max_rows, a.n_nodes * a.blk[b].d);
-    max_n = std::max(max_n, a.blk[b].N);
+    const LinBlock& k = a.blk[b];
+    max_rows = std::max(max_rows, a.n_nodes * k.d);
+    max_n = std::max(max_n, k.N);
+    vec = vec && k.a_off % 4 == 0 && (k.d == 1 || k.a_cs % 4 == 0) && k.N % 4 == 0 &&
+          reinterpret_cast<uintptr_t>(k.W) % 16 == 0;
   }
   if (max_rows == 0 || max_n == 0) return 0;
   dim3 grid((max_rows + kGemmBM - 1) / kGemmBM, (max_n + kGemmBN - 1) / kGemmBN, a.nblocks);
-  blocklin_gemm_kernel<<<grid, kGemmThreads, 0, st>>>(a);
+  if (vec) blocklin_gemm_kernel<true><<<grid, kGemmThreads, 0, st>>>(a);
+  else blocklin_gemm_kernel<false><<<grid, kGemmThreads, 0, st>>>(a);
   S7B_LAUNCH_CHECK();
   return 0;
 }

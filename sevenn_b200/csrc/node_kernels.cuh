@@ -42,6 +42,9 @@ constexpr int kGemmPadM = kGemmBM + 4;
 
 // FP32 SIMT GEMM tile: 128 x 64 per CTA, 8 x 4 per thread, inner product on float2 pairs
 // (scalar-broadcast A element x a pair of B columns).  grid = (ceil(max rows / BM), ceil(max N / BN), nblocks)
+// VEC: A rows and W rows start on 16-byte boundaries (checked by the launcher), so full quads load as float4;
+// otherwise every element loads on its own.
+template <bool VEC>
 __global__ void __launch_bounds__(kGemmThreads, 3) blocklin_gemm_kernel(const LinArgs a) {
   const LinBlock b = a.blk[blockIdx.z];
   const int rows = a.n_nodes * b.d;
@@ -80,11 +83,12 @@ __global__ void __launch_bounds__(kGemmThreads, 3) blocklin_gemm_kernel(const Li
     for (int h = 0; h < 2; ++h) {
       ra[h] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (a_ptr[h] != nullptr) {
-        if (ka + 3 < b.K) ra[h] = __ldg(reinterpret_cast<const float4*>(a_ptr[h] + ka));
+        if (VEC && ka + 3 < b.K) ra[h] = __ldg(reinterpret_cast<const float4*>(a_ptr[h] + ka));
         else {
           if (ka + 0 < b.K) ra[h].x = __ldg(a_ptr[h] + ka + 0);
           if (ka + 1 < b.K) ra[h].y = __ldg(a_ptr[h] + ka + 1);
           if (ka + 2 < b.K) ra[h].z = __ldg(a_ptr[h] + ka + 2);
+          if (!VEC && ka + 3 < b.K) ra[h].w = __ldg(a_ptr[h] + ka + 3);
         }
       }
     }
@@ -92,11 +96,12 @@ __global__ void __launch_bounds__(kGemmThreads, 3) blocklin_gemm_kernel(const Li
     const int kb = k0 + b_k;
     if (kb < b.K) {
       const float* wp = b.W + (size_t)kb * b.N + gc;
-      if (gc + 3 < b.N) rb = __ldg(reinterpret_cast<const float4*>(wp));
+      if (VEC && gc + 3 < b.N) rb = __ldg(reinterpret_cast<const float4*>(wp));
       else {
         if (gc + 0 < b.N) rb.x = __ldg(wp + 0);
         if (gc + 1 < b.N) rb.y = __ldg(wp + 1);
         if (gc + 2 < b.N) rb.z = __ldg(wp + 2);
+        if (!VEC && gc + 3 < b.N) rb.w = __ldg(wp + 3);
       }
     }
   };

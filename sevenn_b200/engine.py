@@ -224,8 +224,16 @@ def pack_table_pairs(tab: np.ndarray):
 
 
 def default_table_knots(spec: ModelSpec) -> int:
-    """A grid on which the XPLOR switching radius (a C1-only point) is a knot."""
-    return 2000 if spec.cutoff_fn == 'XPLOR' else 2048
+    """Number of table intervals over [0, cutoff].  The XPLOR envelope is only C1 at its switching radius r_on (the
+    second derivative jumps), and a cubic Hermite interval that spans r_on loses an order of magnitude in dw/dr
+    there, so for XPLOR take the smallest count in [2000, 4096] that puts r_on on a knot (to 1e-9 of an interval),
+    or failing that the one that brings r_on closest to a knot.  The polynomial cutoff is smooth: 2048."""
+    if spec.cutoff_fn != 'XPLOR':
+        return 2048
+    x = spec.cutoff_on / spec.cutoff
+    dist = lambda n: abs(x * n - round(x * n))
+    counts = range(2000, 4097)
+    return next((n for n in counts if dist(n) < 1e-9), None) or min(counts, key=dist)
 
 
 def prepare_params(spec: ModelSpec, arrays: Dict[str, np.ndarray], radial: str, knots: int):
