@@ -174,29 +174,16 @@ int s7b_d3_set_damping(S7bD3* d, int32_t damping, double s6, double s8, double a
 
 }  // extern "C"
 
-static int d3_invert3(const double* m, double* inv) {
-  const double det = m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
-  if (fabs(det) < 1e-12) return 1;
-  const double id = 1.0 / det;
-  inv[0] = (m[4] * m[8] - m[5] * m[7]) * id; inv[1] = (m[2] * m[7] - m[1] * m[8]) * id; inv[2] = (m[1] * m[5] - m[2] * m[4]) * id;
-  inv[3] = (m[5] * m[6] - m[3] * m[8]) * id; inv[4] = (m[0] * m[8] - m[2] * m[6]) * id; inv[5] = (m[2] * m[3] - m[0] * m[5]) * id;
-  inv[6] = (m[3] * m[7] - m[4] * m[6]) * id; inv[7] = (m[1] * m[6] - m[0] * m[7]) * id; inv[8] = (m[0] * m[4] - m[1] * m[3]) * id;
-  return 0;
-}
-
-// Cell-list grid of one structure (cell rows in Angstrom -> bohr): bins of ~6 A (1..128 per direction) and the search
-// radii in bins R[0..2] = R_vdw, R[3..5] = R_cn.  Non-zero when the cell is singular.
+// Cell-list grid of one structure (cell rows in Angstrom -> bohr, then nl_lattice) with D3's bin policy: bins of
+// ~6 A (1..128 per direction) and the search radii in bins R[0..2] = R_vdw, R[3..5] = R_cn.  Non-zero when the
+// cell is singular.
 static int d3_grid(const double* cell9, const int32_t* pbc3, double rthr, double cnthr, NLGrid& g, int* R) {
   memset(&g, 0, sizeof(g));
   for (int k = 0; k < 9; ++k) g.cell[k] = cell9[k] / kAuToAng;
-  if (d3_invert3(g.cell, g.inv)) return 1;
+  double height[3];
+  if (nl_lattice(g, height)) return 1;
   for (int a = 0; a < 3; ++a) { g.pbc[a] = pbc3[a] ? 1 : 0; g.fmin[a] = 0.0; g.fspan[a] = 1.0; }
   g.cutoff2 = rthr;
-  double height[3];
-  for (int a = 0; a < 3; ++a) {
-    const double nx = g.inv[0 * 3 + a], ny = g.inv[1 * 3 + a], nz = g.inv[2 * 3 + a];
-    height[a] = 1.0 / sqrt(nx * nx + ny * ny + nz * nz);
-  }
   const double w_target = 6.0 / kAuToAng;           // ~10 atoms per bin in a dense solid
   const double rc_v = sqrt(rthr), rc_c = sqrt(cnthr);
   for (int a = 0; a < 3; ++a) {
@@ -287,19 +274,10 @@ static int d3_setup(S7bD3* d, int B, const int32_t* atom_ptr, const std::vector<
   S7B_CUDA_CHECK(cudaMemcpyAsync(d->bin_off.p, bin_off.data(), (Bs + 1) * 4, cudaMemcpyHostToDevice, st));
   S7B_CUDA_CHECK(cudaMemcpyAsync(d->rtab.p, R.data(), Bs * 24, cudaMemcpyHostToDevice, st));
   if (n > 0) {
-    // the binning of the model's neighbour list: one stable sort over the bins of all structures
-    nl_bin_kernel<<<(n + 127) / 128, 128, 0, st>>>(d->grids.as<NLGrid>(), d->aptr.as<int>(), d->bin_off.as<int>(), B, d->pos.as<double>(), n,
-                                                   d->key.as<int>(), d->idx.as<int>(), d->wrapped.as<double>(), d->sys.as<int>());
-    S7B_CUDA_CHECK(cudaGetLastError());
-    int end_bit = 1;
-    while ((1LL << end_bit) < nbins) ++end_bit;
-    size_t tmp_sort = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, d->key.as<int>(), d->key_sorted.as<int>(), d->idx.as<int>(), d->idx_sorted.as<int>(), n, 0, end_bit, st);
-    if (d->tmp.ensure(tmp_sort + 256)) return d3_fail("cudaMalloc failed for cub workspace");
-    size_t tmp = d->tmp.bytes;
-    S7B_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(d->tmp.p, tmp, d->key.as<int>(), d->key_sorted.as<int>(), d->idx.as<int>(), d->idx_sorted.as<int>(), n, 0, end_bit, st));
-    nl_bin_start_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(d->key_sorted.as<int>(), n, (int)nbins, d->bin_start.as<int>());
-    S7B_CUDA_CHECK(cudaGetLastError());
+    // the binning of the model's neighbour list, uncounted (the D3 entry points do not feed the engine's launch count)
+    const NLBinArgs bins{d->grids.as<NLGrid>(), d->aptr.as<int>(), d->bin_off.as<int>(), d->pos.as<double>(), B, n, nbins, d->key.as<int>(),
+                         d->idx.as<int>(), d->key_sorted.as<int>(), d->idx_sorted.as<int>(), d->sys.as<int>(), d->bin_start.as<int>(), d->wrapped.as<double>()};
+    if (nl_bin_sort(bins, d->tmp, 0, d3_fail, nullptr, st)) return 1;
     d3_sort_gather_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, d->idx_sorted.as<int>(), d->key_sorted.as<int>(), d->wrapped.as<double>(),
                                                           d->type.as<int>(), d->sys.as<int>(), batch ? d->lrank.as<int>() : nullptr,
                                                           d->xs.as<double>(), d->ts.as<int>(), d->ss.as<int>(), d->bin_of.as<int>());

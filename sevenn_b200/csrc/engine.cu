@@ -1739,20 +1739,10 @@ int s7b_engine_compute_host(S7bEngine* e, int32_t n_nodes, int64_t n_edges, cons
 }
 
 // ---- positions in: device neighbour list + graph build (SURVEY 8(f).1) ------------------------
-static int invert3(const double* m, double* inv) {
-  const double det = m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
-  if (fabs(det) < 1e-12) return 1;
-  const double id = 1.0 / det;
-  inv[0] = (m[4] * m[8] - m[5] * m[7]) * id; inv[1] = (m[2] * m[7] - m[1] * m[8]) * id; inv[2] = (m[1] * m[5] - m[2] * m[4]) * id;
-  inv[3] = (m[5] * m[6] - m[3] * m[8]) * id; inv[4] = (m[0] * m[8] - m[2] * m[6]) * id; inv[5] = (m[2] * m[3] - m[0] * m[5]) * id;
-  inv[6] = (m[3] * m[7] - m[4] * m[6]) * id; inv[7] = (m[1] * m[6] - m[0] * m[7]) * id; inv[8] = (m[0] * m[4] - m[1] * m[3]) * id;
-  return 0;
-}
-
 // Cell-list grid of one structure (b = its index in the batch, for messages), in two steps.  nl_grid_cell:
-// lattice (missing vectors of non-periodic directions completed), inverse and plane heights -- everything
-// that does not depend on the positions.  nl_grid_bins: binned fractional range of the non-periodic
-// directions from the bounding box lo/hi (nullptr: fully periodic or no atoms), bins and search radii.
+// lattice (missing vectors of non-periodic directions completed), inverse and plane heights (nl_lattice) --
+// everything that does not depend on the positions.  nl_grid_bins, the model's bin policy: binned fractional range
+// of the non-periodic directions from the bounding box lo/hi (nullptr: fully periodic or no atoms), bins, radii.
 static int nl_grid_cell(NLGrid& g, double height[3], const double* cell9, const int32_t* pbc3, double cutoff, int b) {
   memset(&g, 0, sizeof(g));
   g.cutoff2 = cutoff * cutoff;
@@ -1765,11 +1755,7 @@ static int nl_grid_cell(NLGrid& g, double height[3], const double* cell9, const 
       g.cell[3 * a + a] = 1.0;
     }
   }
-  if (invert3(g.cell, g.inv)) return fail("singular cell (structure " + std::to_string(b) + ")");
-  for (int a = 0; a < 3; ++a) {      // |row a of inv^T| = 1 / height_a
-    const double nx = g.inv[0 * 3 + a], ny = g.inv[1 * 3 + a], nz = g.inv[2 * 3 + a];
-    height[a] = 1.0 / sqrt(nx * nx + ny * ny + nz * nz);
-  }
+  if (nl_lattice(g, height)) return fail("singular cell (structure " + std::to_string(b) + ")");
   for (int a = 0; a < 3; ++a) { g.fmin[a] = 0.0; g.fspan[a] = 1.0; }
   return 0;
 }
@@ -1874,29 +1860,19 @@ static int build_neighbor_list(S7bEngine* e, int32_t B, const int32_t* atom_ptr,
   if (n_atoms > 0) {
     if (d_species != e->hs_species.as<int>())
       S7B_CUDA_CHECK(cudaMemcpyAsync(e->hs_species.p, d_species, (size_t)n_atoms * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    const int blk = 128, grd = (n_atoms + blk - 1) / blk;
     const NLGrid* d_grids = e->nl_grids.as<NLGrid>();
     const int* d_bin_off = e->nl_bin_off.as<int>();
-    nl_bin_kernel<<<grd, blk, 0, st>>>(d_grids, e->nl_atom_ptr.as<int>(), d_bin_off, B, d_positions, n_atoms, e->nl_key.as<int>(),
-                                       e->nl_idx.as<int>(), e->nl_wrapped.as<double>(), e->nl_sys.as<int>());
-    S7B_LAUNCH_CHECK();
-    int end_bit = 1;                   // keys are < nbins <= 2^26
-    while ((1LL << end_bit) < nbins) ++end_bit;
-    size_t tmp_sort = 0, tmp_scan = 0, tmp_sum = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, e->nl_key.as<int>(), e->nl_key_sorted.as<int>(), e->nl_idx.as<int>(), e->nl_idx_sorted.as<int>(), n_atoms, 0, end_bit, st);
+    size_t tmp_scan = 0, tmp_sum = 0;  // the scan and sum below run from the binning's cub workspace
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, e->nl_count.as<int>(), e->hs_rowptr.as<int>(), n_atoms + 1, st);
     cub::DeviceReduce::Sum(nullptr, tmp_sum, e->nl_count.as<int>(), e->nl_total.as<int64_t>(), n_atoms, st);
-    if (e->nl_tmp.ensure(std::max(std::max(tmp_sort, tmp_scan), tmp_sum) + 256)) return fail("cudaMalloc failed for cub workspace");
-    size_t tmp = e->nl_tmp.bytes;
-    S7B_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(e->nl_tmp.p, tmp, e->nl_key.as<int>(), e->nl_key_sorted.as<int>(), e->nl_idx.as<int>(), e->nl_idx_sorted.as<int>(), n_atoms, 0, end_bit, st));
-    ++g_launches;
-    nl_bin_start_kernel<<<(n_atoms + 1 + 255) / 256, 256, 0, st>>>(e->nl_key_sorted.as<int>(), n_atoms, (int)nbins, e->nl_bin_start.as<int>());
-    S7B_LAUNCH_CHECK();
+    const NLBinArgs bins{d_grids, e->nl_atom_ptr.as<int>(), d_bin_off, d_positions, B, n_atoms, nbins, e->nl_key.as<int>(), e->nl_idx.as<int>(),
+                         e->nl_key_sorted.as<int>(), e->nl_idx_sorted.as<int>(), e->nl_sys.as<int>(), e->nl_bin_start.as<int>(), e->nl_wrapped.as<double>()};
+    if (nl_bin_sort(bins, e->nl_tmp, std::max(tmp_scan, tmp_sum), fail, &g_launches, st)) return 1;
     S7B_CUDA_CHECK(cudaMemsetAsync(e->nl_count.p, 0, ((size_t)n_atoms + 1) * sizeof(int), st));
-    const int grd_c = std::max(1, (n_centres + blk - 1) / blk);
+    const int blk = 128, grd_c = std::max(1, (n_centres + blk - 1) / blk);
     nl_pairs_kernel<false><<<grd_c, blk, 0, st>>>(d_grids, d_bin_off, e->nl_sys.as<int>(), e->nl_wrapped.as<double>(), e->nl_key.as<int>(), e->nl_idx_sorted.as<int>(), e->nl_bin_start.as<int>(), n_centres, e->nl_count.as<int>(), nullptr, nullptr, nullptr, d_centres);
     S7B_LAUNCH_CHECK();
-    tmp = e->nl_tmp.bytes;
+    size_t tmp = e->nl_tmp.bytes;
     S7B_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(e->nl_tmp.p, tmp, e->nl_count.as<int>(), e->hs_rowptr.as<int>(), n_centres + 1, st));
     ++g_launches;
     tmp = e->nl_tmp.bytes;             // the int32 scan wraps past 2^31 edges: the total is also summed in int64

@@ -13,8 +13,11 @@
 // the periodic image shift of every visited bin -- correct for any cell size, including cells much
 // smaller than the cutoff.  Two passes (count, exclusive scan, fill) emit the CSR directly, so the
 // engine needs no sort of the edge list.  Non-periodic directions use the bounding box and no images.
+// D3's cell list (d3.cu) shares the lattice set-up (nl_lattice) and the binning (nl_bin_sort); only the bin
+// policy, how many bins and how far to search, is each caller's own.
 #pragma once
 #include <cub/cub.cuh>
+#include <string>
 
 #include "common.cuh"
 
@@ -120,6 +123,52 @@ static __global__ void nl_bin_start_kernel(const int* __restrict__ key_sorted, i
   const int prev = (s == 0) ? -1 : key_sorted[s - 1];
   const int cur = (s == n) ? nbins : key_sorted[s];
   for (int b = prev + 1; b <= cur; ++b) bin_start[b] = s;
+}
+
+// Lattice set-up from the rows in g.cell: g.inv and height[a], the spacing of the lattice planes of direction a.
+// Non-zero when the cell is singular.
+inline int nl_lattice(NLGrid& g, double height[3]) {
+  const double* m = g.cell;
+  const double det = m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
+  if (fabs(det) < 1e-12) return 1;
+  const double id = 1.0 / det;
+  g.inv[0] = (m[4] * m[8] - m[5] * m[7]) * id; g.inv[1] = (m[2] * m[7] - m[1] * m[8]) * id; g.inv[2] = (m[1] * m[5] - m[2] * m[4]) * id;
+  g.inv[3] = (m[5] * m[6] - m[3] * m[8]) * id; g.inv[4] = (m[0] * m[8] - m[2] * m[6]) * id; g.inv[5] = (m[2] * m[3] - m[0] * m[5]) * id;
+  g.inv[6] = (m[3] * m[7] - m[4] * m[6]) * id; g.inv[7] = (m[1] * m[6] - m[0] * m[7]) * id; g.inv[8] = (m[0] * m[4] - m[1] * m[3]) * id;
+  for (int a = 0; a < 3; ++a)        // |column a of inv| = 1 / height_a
+    height[a] = 1.0 / sqrt(g.inv[a] * g.inv[a] + g.inv[3 + a] * g.inv[3 + a] + g.inv[6 + a] * g.inv[6 + a]);
+  return 0;
+}
+
+// Device arrays of the binning of a batch's n > 0 atoms (in: grids, atom_ptr, bin_off, pos; out: the rest).
+struct NLBinArgs {
+  const NLGrid* grids;
+  const int *atom_ptr, *bin_off;
+  const double* pos;
+  int B, n;
+  long long nbins;
+  int *key, *idx, *key_sorted, *idx_sorted, *sys, *bin_start;
+  double* wrapped;
+};
+
+// Bin keys, one stable radix sort over the bits the keys use, and bin_start.  Sizes the cub workspace `tmp` (the
+// caller's buffer type) to the larger of the sort's need and tmp_other, what the caller runs from it afterwards;
+// reports a failed allocation through the caller's `fail` and adds its launches to *launches (nullptr: not counted).
+template <class Buf>
+int nl_bin_sort(const NLBinArgs& a, Buf& tmp, size_t tmp_other, int (*fail)(const std::string&), int64_t* launches, cudaStream_t st) {
+  nl_bin_kernel<<<(a.n + 127) / 128, 128, 0, st>>>(a.grids, a.atom_ptr, a.bin_off, a.B, a.pos, a.n, a.key, a.idx, a.wrapped, a.sys);
+  S7B_CUDA_CHECK(cudaGetLastError());
+  int end_bit = 1;                   // keys are < nbins
+  while ((1LL << end_bit) < a.nbins) ++end_bit;
+  size_t tmp_sort = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, a.key, a.key_sorted, a.idx, a.idx_sorted, a.n, 0, end_bit, st);
+  if (tmp.ensure((tmp_sort > tmp_other ? tmp_sort : tmp_other) + 256)) return fail("cudaMalloc failed for cub workspace");
+  size_t bytes = tmp.bytes;
+  S7B_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, a.key, a.key_sorted, a.idx, a.idx_sorted, a.n, 0, end_bit, st));
+  nl_bin_start_kernel<<<(a.n + 1 + 255) / 256, 256, 0, st>>>(a.key_sorted, a.n, (int)a.nbins, a.bin_start);
+  if (launches) *launches += 3;
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
 }
 
 // One thread per centre atom (centre c = centres[tid], or tid itself when centres == nullptr; original
