@@ -60,7 +60,7 @@ typedef struct {
                                                          lmax_out = lmax_filter or 0) run convolution kernels
                                                          specialised for them; every other width and lmax combination
                                                          runs the runtime-width convolution kernels. */
-  int32_t table_knots;                                /* > 0: radial weights from cubic tables */
+  int32_t table_knots;                                /* > 0: radial weights from tables (cubic: this many intervals) */
 } S7bModelDesc;
 
 /* Stages of one energy/force evaluation (single GPU: s7b_engine_compute runs them all).
@@ -162,7 +162,9 @@ S7B_API int s7b_engine_set_atomic_virial(S7bEngine* eng, int enable);
 
 /* Upload one named parameter array (host pointer, fp32).  Names: "embed_x0", "embed_g0",
  * "readout" (+ optional "readout_lo", the fp32 residual of the fp64 fold), "scale", "shift", "bessel", and per layer t "si1", "si1T", "sc", "scT", "si2",
- * "si2T", "table", "mlp0".."mlp2", "mlp0T".."mlp2T" (layouts: sevenn_b200/engine.py).  A layer with the species-wise
+ * "si2T", "table", "table23", "table_fwd", "mlp0".."mlp2", "mlp0T".."mlp2T" (layouts: sevenn_b200/engine.py).  "table" /
+ * "table23" are the backward's cubic table on table_knots intervals; "table_fwd" ([Kf + 1][W]) holds the forward's knot
+ * values on Kf intervals of its own, read from its size (engine.py uses Kf = 3 table_knots).  A layer with the species-wise
  * ('nequip') self-connection takes "sc_species" / "scT_species" ([num_species][l block][K][N], the transpose per block)
  * instead of "sc" / "scT"; setting both kinds on one layer is an error. */
 S7B_API int s7b_engine_set_param(S7bEngine* eng, const char* name, int layer, const float* host, size_t numel);

@@ -32,6 +32,7 @@ struct ConvRole {
   int w_off[kMaxPaths];       // per path: first column in weight[E, W]
   int out_off[kMaxPaths];     // per path: offset inside a mid row of element (k = 0, u = 0)
   int out_stride[kMaxPaths];  // per path: K_l3 (component stride in the fused mid block)
+  int ftab_off;               // first channel pair of this role's value-table image (table mode, see ConvArgs::ftable)
 };
 
 // Floats per edge of the stored harmonics Y_1 .. Y_{NY-1} (Y_0 = 1 is implicit), padded to whole float4s.
@@ -45,11 +46,12 @@ constexpr int kConvNoPath = 4;
 
 struct ConvArgs {
   const int* rowptr;          // [n_dst + 1] CSR over destination (centre) atoms
-  const int4* rec;            // [E] {src, table interval, frac bits, 0}
+  const int4* rec;            // [E] {src, cubic-table interval, its frac bits, edge length r bits}
   const float* Y;             // [E, y_stride(NY)]  Y_1 .. Y_{NY-1} (Y_0 = 1 implicit), zero padded
   const float* x;             // [n_nodes, dim_x]
-  // Radial tables: one image per l1 role at ConvRole::tab_off, laid out [knot][path of the role][channel pair]
-  // (engine.cu role_table_images), so that one edge reaches all paths of its role from one address.
+  // Radial tables: one image per l1 role at ConvRole::tab_off (cubic, backward) or ConvRole::ftab_off (values,
+  // forward), laid out [knot][path of the role][channel pair] (engine.cu role_table_images), so that one edge
+  // reaches all paths of its role from one address.
   const float4* table;        // {a0e,a0o,a1e,a1o}: value and slope*h of the cubic, per channel pair
   const uint2* table23;       // {half2(a2e,a2o), half2(a3e,a3o)}: the two small cubic terms in fp16
   const float* w;             // [E, W] stored weights (operator boundary / exact-MLP mode)
@@ -58,6 +60,9 @@ struct ConvArgs {
   float inv_h;                // 1 / table interval
   unsigned int* row_max;      // optional [n_dst, rows_per_node]: running max |out| bits of every (l3, k) row of the mid
   int rows_per_node;          // features (row l3^2 + k), for the tensor-core linear that consumes them (tc_gemm.cuh)
+  const float2* ftable;       // w at knots 0..ftab_knots, per channel pair (forward: linear interpolation)
+  float ftab_inv_h;           // ftab_knots / cutoff
+  int ftab_knots;             // intervals of the value table over [0, cutoff]
 };
 
 }  // namespace s7b

@@ -13,10 +13,13 @@
 // (csrc/vec_ops.cuh), every global access of a group is one contiguous
 // 8-byte-per-lane segment of the component-major ("cm") layout, and the node accumulators of all
 // paths stay in registers over the whole CSR row -- no atomics in the forward.
-// The radial weights w_p,u(r) come either from a cubic-Hermite table indexed by the edge length
-// (TABLE: L2-resident, per (knot, channel pair) {a0e,a0o,a1e,a1o} fp32 + {a2e,a2o,a3e,a3o} fp16 = 24 B)
-// or from a stored [E, W]
-// array (!TABLE: the reference's plug-in boundary, where the radial MLP stays outside).
+// The radial weights w_p,u(r) come either from tables indexed by the edge length (TABLE, L2-resident) or from a
+// stored [E, W] array (!TABLE: the reference's plug-in boundary, where the radial MLP stays outside).  The forward
+// only needs w: it interpolates linearly in a value table on a grid three times finer (per (knot, channel pair)
+// one float2, 16 B per pair read per edge; edges shorter than kValueTableMinR are added by a second pass over the
+// row from the cubic table, in the warps that have such an edge).  The
+// backward needs w and dw/dr: it evaluates a cubic-Hermite table (per (knot, channel pair) {a0e,a0o,a1e,a1o} fp32 +
+// {a2e,a2o,a3e,a3o} fp16 = 24 B).
 #pragma once
 #include <cuda_fp16.h>
 
@@ -74,6 +77,34 @@ __device__ __forceinline__ int conv_mul(const ConvRole& role) {
 // row (one coalesced 16*LPN-byte request per LPN edges, i.e. about once per row) and every iteration
 // takes its record by shuffle.  Prefetching record + harmonics into registers was measured slower
 // (register pressure); this costs three registers.
+// Below this edge length the forward evaluates the cubic table instead of the value table.  Linear interpolation
+// errs by h^2 w'' / 12, and w'' grows steeply at distances no MD run reaches (0.2 A: 2.7e-4 eV on a SevenNet-0
+// H-H dimer, against 2.5e-6 eV with the cubic); the shortest bond, H2, is 0.74 A.
+constexpr float kValueTableMinR = 0.6f;
+
+// How the forward reads an edge record {src, cubic interval, its fraction, r} (edge_fwd_kernel):
+//  * kRecRaw: as stored (the backward, and the forward with stored weights);
+//  * kRecValue: r placed on the value grid (a.ftab_knots intervals over [0, cutoff]) with the clamps the edge kernel
+//    applies for the cubic table: an edge at or beyond the cutoff reads the end of the last interval, knot Kf, whose
+//    value is exactly 0 (s7b_engine_set_param checks it).  The fraction is one FMA from r, so it keeps the bits of
+//    the fp32 position r / h.  An edge shorter than kValueTableMinR is also sent to knot Kf, so it adds exactly 0,
+//    and raises `short_seen`: the cubic pass adds it afterwards;
+//  * kRecCubicShort: the cubic interval of a short edge, ~interval (< 0) for every other edge, which adds 0.
+enum { kRecRaw = 0, kRecValue = 1, kRecCubicShort = 2 };
+template <int MODE>
+__device__ __forceinline__ int4 fwd_rec(const ConvArgs& a, int4 r, bool valid, bool& short_seen) {
+  const float rr = __int_as_float(r.w);
+  const bool is_short = valid && rr < kValueTableMinR;
+  if (MODE == kRecValue) {
+    short_seen = short_seen || is_short;
+    const int k = is_short ? a.ftab_knots - 1 : min(max((int)(rr * a.ftab_inv_h), 0), a.ftab_knots - 1);
+    const float t = is_short ? 1.0f : fminf(fmaxf(fmaf(rr, a.ftab_inv_h, -(float)k), 0.0f), 1.0f);
+    return make_int4(r.x, k, __float_as_int(t), 0);
+  }
+  if (MODE == kRecCubicShort) return make_int4(r.x, is_short ? r.y : ~r.y, r.z, 0);
+  return r;
+}
+
 template <int LPN>
 struct EdgeRecs {
   int cx, cy, cz;
@@ -81,6 +112,14 @@ struct EdgeRecs {
     const int ei = it + sl;
     int4 r = make_int4(0, 0, 0, 0);
     if (ei < len) r = __ldg(a.rec + (unsigned)(e0 + ei));
+    cx = r.x; cy = r.y; cz = r.z;
+  }
+  template <int MODE>
+  __device__ __forceinline__ void fill(const ConvArgs& a, int e0, int len, int it, int sl, bool& short_seen) {
+    const int ei = it + sl;
+    int4 r = make_int4(0, 0, 0, 0);
+    if (ei < len) r = __ldg(a.rec + (unsigned)(e0 + ei));
+    r = fwd_rec<MODE>(a, r, ei < len, short_seen);
     cx = r.x; cy = r.y; cz = r.z;
   }
   __device__ __forceinline__ int4 get(int it) const {
@@ -146,6 +185,8 @@ template <> struct VT<V2> {
   static __device__ __forceinline__ void store(float* p, V2 v) { *reinterpret_cast<float2*>(p) = v; }
   static __device__ __forceinline__ float hsum(V2 v) { return v.x + v.y; }
   static __device__ __forceinline__ float amax(V2 v) { return fmaxf(fabsf(v.x), fabsf(v.y)); }
+  // value-table entry of the channel pair at p
+  static __device__ __forceinline__ V2 val(const float2* p, bool) { return __ldg(p); }
   // cubic coefficients of the channel pair at t01 / t23
   static __device__ __forceinline__ void coef(const float4* t01, const uint2* t23, bool, V2& a0, V2& a1, V2& a2, V2& a3) {
     const float4 c01 = __ldg(t01);
@@ -163,6 +204,8 @@ template <> struct VT<float> {
   static __device__ __forceinline__ void store(float* p, float v) { *p = v; }
   static __device__ __forceinline__ float hsum(float v) { return v; }
   static __device__ __forceinline__ float amax(float v) { return fabsf(v); }
+  // the odd or even channel of the value-table entry of the pair at p
+  static __device__ __forceinline__ float val(const float2* p, bool odd) { return __ldg(reinterpret_cast<const float*>(p) + odd); }
   // the odd or even channel of the pair at t01 / t23
   static __device__ __forceinline__ void coef(const float4* t01, const uint2* t23, bool odd, float& a0, float& a1, float& a2, float& a3) {
     const float4 c01 = __ldg(t01);
@@ -206,40 +249,37 @@ struct LaneMap {
 // become immediates, and each edge costs one x address and one table address per lane.  MUL = 0 reads the
 // width from role.mul (runtime-width instantiation; role.mul must be a multiple of CH*LPN*NV).
 // ------------------------------------------------------------------------------------------
-template <class Kind, int MUL, int NV, int LPN, bool TABLE, class V>
-__global__ void S7B_FWD_BOUNDS
-conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) {
+// The edge loop of conv_fwd_kernel over the CSR row of this lane's node: acc += w_e * CG(x[src_e], Y_e).  MODE
+// (see fwd_rec) picks the radial weights: kRecRaw the stored [E, W] array, kRecValue the value table (linear),
+// kRecCubicShort the cubic table for the edges shorter than kValueTableMinR (0 for the others).
+template <class Kind, int MUL, int NV, int LPN, bool TABLE, class V, int MODE>
+__device__ __forceinline__ void conv_fwd_edges(const ConvArgs& a, const ConvRole& role,
+                                               const LaneMap<NV, LPN, VT<V>::CH>& m,
+                                               V (&acc)[NV][Kind::NACC], bool& short_seen) {
   constexpr int CH = VT<V>::CH;
-  static_assert(MUL % (CH * LPN * NV) == 0, "channels must fill whole lane groups");
   const int mul = conv_mul<MUL>(role);
-  const LaneMap<NV, LPN, CH> m(a);
-  if (m.nmax == 0 && !m.node_ok) return;      // whole warp beyond the last node (uniform)
-
-  V acc[NV][Kind::NACC];
-#pragma unroll
-  for (int c = 0; c < NV; ++c)
-#pragma unroll
-    for (int q = 0; q < Kind::NACC; ++q) acc[c][q] = VT<V>::zero();
-
   const unsigned xlane = role.x_off + m.uc0;               // this lane's first element in a row of x
-  const unsigned tlane = role.tab_off + (m.uc0 >> 1);       // ... and its first pair in a knot row of the table
+  // ... and its first pair in a knot row of the role's image of the value table or the cubic table
+  const unsigned tlane = (MODE == kRecCubicShort ? role.tab_off : role.ftab_off) + (m.uc0 >> 1);
   const bool odd = (m.uc0 & 1) != 0;
   EdgeRecs<LPN> recs;
   for (int it = 0; it < m.nmax; ++it) {
     const bool valid = (LPN == 32) || (it < m.len);
     const int e = valid ? m.e0 + it : 0;
 #if S7B_COOP_REC
-    if (it % LPN == 0) recs.fill(a, m.e0, m.len, it, m.sl);
+    if (it % LPN == 0) recs.template fill<MODE>(a, m.e0, m.len, it, m.sl, short_seen);
     const int4 rec = recs.get(it);
 #else
-    const int4 rec = __ldg(a.rec + e);
+    const int4 rec = fwd_rec<MODE>(a, __ldg(a.rec + e), valid, short_seen);
 #endif
     float Y[Kind::NY];
     load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
     const float* __restrict__ xrow = a.x + (row_offset(rec.x, a.dim_x) + xlane);
-    const unsigned ti = tlane + rec.y * (Kind::NPATH * mul / 2);   // knot row of the role's table image
-    const float4* __restrict__ k01 = a.table + ti;
-    const uint2* __restrict__ k23 = a.table23 + ti;
+    const bool take = MODE != kRecCubicShort || rec.y >= 0;
+    const int k = take ? rec.y : ~rec.y;
+    const unsigned ti = tlane + k * (Kind::NPATH * mul / 2);     // knot row of the role's table image
+    const float2* __restrict__ v0 = a.ftable + ti;                 // value table: knot k ...
+    const float2* __restrict__ v1 = v0 + Kind::NPATH * mul / 2;    // ... and k + 1, one row further
     const float tt = __int_as_float(rec.z);
 #pragma unroll
     for (int c = 0; c < NV; ++c) {
@@ -249,10 +289,14 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
       for (int i = 0; i < Kind::D1; ++i) x[i] = VT<V>::load(xrow + i * mul + u);
 #pragma unroll
       for (int p = 0; p < Kind::NPATH; ++p) {
-        if (TABLE) {
+        if (MODE == kRecValue) {          // (1 - t) v_k + t v_k+1 (knot values: engine.py radial_value_table)
+          const V w0 = VT<V>::val(v0 + (p * (mul / 2) + u / 2), odd);
+          const V w1 = VT<V>::val(v1 + (p * (mul / 2) + u / 2), odd);
+          w[p] = fma_(tt, w1, fma_(-tt, w0, w0));
+        } else if (MODE == kRecCubicShort) {
           V a0, a1, a2, a3;
-          VT<V>::coef(k01 + (p * (mul / 2) + u / 2), k23 + (p * (mul / 2) + u / 2), odd, a0, a1, a2, a3);
-          w[p] = fma_(tt, fma_(tt, fma_(tt, a3, a2), a1), a0);
+          VT<V>::coef(a.table + ti + (p * (mul / 2) + u / 2), a.table23 + ti + (p * (mul / 2) + u / 2), odd, a0, a1, a2, a3);
+          w[p] = take ? fma_(tt, fma_(tt, fma_(tt, a3, a2), a1), a0) : VT<V>::zero();
         } else {
           w[p] = VT<V>::load(a.w + (size_t)e * a.w_numel + role.w_off[p] + m.uc0 + u);
         }
@@ -261,6 +305,29 @@ conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) 
       Kind::fwd(x, Y, w, acc[c]);
     }
   }
+}
+
+template <class Kind, int MUL, int NV, int LPN, bool TABLE, class V>
+__global__ void S7B_FWD_BOUNDS
+conv_fwd_kernel(const ConvArgs a, const ConvRole role, float* __restrict__ out) {
+  constexpr int CH = VT<V>::CH;
+  static_assert(MUL % (CH * LPN * NV) == 0, "channels must fill whole lane groups");
+  const LaneMap<NV, LPN, CH> m(a);
+  if (m.nmax == 0 && !m.node_ok) return;      // whole warp beyond the last node (uniform)
+
+  V acc[NV][Kind::NACC];
+#pragma unroll
+  for (int c = 0; c < NV; ++c)
+#pragma unroll
+    for (int q = 0; q < Kind::NACC; ++q) acc[c][q] = VT<V>::zero();
+
+  // value table (or stored weights) for every edge; then, only in a warp that met an edge shorter than
+  // kValueTableMinR, the cubic table for those edges (the first pass added 0 for them)
+  bool short_seen = false;
+  conv_fwd_edges<Kind, MUL, NV, LPN, TABLE, V, TABLE ? kRecValue : kRecRaw>(a, role, m, acc, short_seen);
+  if constexpr (TABLE)
+    if (__any_sync(0xffffffffu, short_seen))
+      conv_fwd_edges<Kind, MUL, NV, LPN, TABLE, V, kRecCubicShort>(a, role, m, acc, short_seen);
 
   // row maxima of the mid features for the tensor-core self_interaction_2 (fixed-point row scaling): one
   // group reduction and one atomicMax per (l3, k) row this role contributes to -- saves a pass over the mid tensor

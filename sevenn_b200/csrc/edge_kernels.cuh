@@ -42,7 +42,8 @@ S7B_HD void envelope(const RadialDesc& d, float r, float& env, float& denv) {
   }
 }
 
-// One thread per edge.  Writes rec = {src, interval, frac, 0}, Y[e, 0..ny_stride) = Y_1.., r, and
+// One thread per edge.  Writes rec = {src, interval, frac, r} (the cubic table's interval and fraction; the
+// forward's value table has its own grid, which conv_fwd places r on), Y[e, 0..ny_stride) = Y_1.., r, and
 // (exact-MLP mode) the radial embedding emb[e, 0..n_basis).
 // The edge count is read from device memory and the grid is sized for the engine's edge capacity, so
 // a captured CUDA graph of the step stays valid when the neighbour count changes between MD steps.
@@ -69,7 +70,7 @@ __global__ void edge_fwd_kernel(const RadialDesc rd, const float* __restrict__ e
   // edges at or beyond the cutoff sit at the end of the last interval, where the envelope has taken the
   // weights (and, for XPLOR / polynomial cutoffs, their slope) to zero: no extrapolation of the last cubic
   const float tt = fminf(fmaxf(s - (float)tk, 0.0f), 1.0f);
-  rec[e] = make_int4(__ldg(src + e), tk, __float_as_int(tt), 0);
+  rec[e] = make_int4(__ldg(src + e), tk, __float_as_int(tt), __float_as_int(r));
   rlen[e] = r;
   if (emb != nullptr) {
     float env, denv;

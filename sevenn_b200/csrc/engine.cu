@@ -136,6 +136,7 @@ struct LayerCfg {
   int dim_x = 0, dim_g = 0, dim_h = 0, dim_mid = 0, W = 0;
   int mid_K[kMaxL] = {0}, mid_off[kMaxL] = {0};
   int lmax_out = 0;
+  int ftab_knots = 0;                 // intervals of the forward value table ("table_fwd"; 0 until it is set)
   std::vector<PathCfg> paths;
   ConvRole roles[kMaxL];
   GateDesc gate;
@@ -747,20 +748,24 @@ static int conv_forward(const LayerCfg& L, int lmax_filter, bool table, ConvArgs
   return 0;
 }
 
-// The radial table of a layer arrives as [knot][channel pair of the W columns], 16 B ("table") or 8 B ("table23")
-// per pair (engine.py pack_table_pairs).  The kernels read one image per l1 role at ConvRole::tab_off, laid out
-// [knot][path of the role][channel pair]: an edge then reaches all paths of its role from one address, at
-// offsets fixed at compile time.  Same values and total size, permuted.
-static std::vector<float> role_table_images(const LayerCfg& L, int knots, const float* host, int floats_per_pair) {
-  std::vector<float> img((size_t)knots * (L.W / 2) * floats_per_pair);
+// A radial table of a layer arrives as [knot row][channel pair of the W columns], 16 B ("table") or 8 B ("table23")
+// per pair (engine.py pack_table_pairs), or 8 B ("table_fwd", engine.py radial_value_table).  The kernels read one
+// image per l1 role, laid out [knot row][path of the role][channel pair]: an edge then reaches all paths of its role
+// from one address, at offsets fixed at compile time.  Same values and total size, permuted.  The images follow
+// each other in l1 order; role_off[l1] receives the first channel pair of each (for the cubic table, rows = knots,
+// that is ConvRole::tab_off as build_layer_cfg placed it).
+static std::vector<float> role_table_images(const LayerCfg& L, int rows, const float* host, int floats_per_pair,
+                                            int* role_off) {
+  std::vector<float> img((size_t)rows * (L.W / 2) * floats_per_pair);
+  float* dst = img.data();
   for (int l1 = 0; l1 < L.n_lx; ++l1) {
     const ConvRole& r = L.roles[l1];
     std::vector<int> cols;
     for (const PathCfg& q : L.paths)
       if (q.l1 == l1) cols.push_back(q.w_off);
     const size_t run = (size_t)(r.mul / 2) * floats_per_pair;
-    float* dst = img.data() + (size_t)r.tab_off * floats_per_pair;
-    for (int k = 0; k < knots; ++k)
+    role_off[l1] = (int)((dst - img.data()) / floats_per_pair);
+    for (int k = 0; k < rows; ++k)
       for (int c : cols) {
         memcpy(dst, host + ((size_t)k * (L.W / 2) + c / 2) * floats_per_pair, run * sizeof(float));
         dst += run;
@@ -1079,8 +1084,28 @@ int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float*
     if (e->desc.table_knots <= 0) return fail("parameter " + nm + ": the model was created without radial tables");
     if (numel != (size_t)e->desc.table_knots * (L.W / 2) * fpp)
       return fail("parameter " + nm + ": size does not match the layer configuration and knot count");
-    img = role_table_images(L, e->desc.table_knots, host, fpp);
+    int off[kMaxL];
+    img = role_table_images(L, e->desc.table_knots, host, fpp, off);
     host = img.data();
+  }
+  if (layer >= 0 && nm == "table_fwd") {
+    // the forward's value table: w at knots 0..Kf over [0, cutoff], [Kf + 1][W] fp32.  Kf is the host's choice
+    // (engine.py forward_table_knots) and is read from the size; the kernels index it with 32 bits.
+    LayerCfg& L = e->layers[layer];
+    if (e->desc.table_knots <= 0) return fail("parameter " + nm + ": the model was created without radial tables");
+    const size_t rows = numel / (size_t)L.W;
+    if (numel % (size_t)L.W != 0 || rows < 2 || rows * (size_t)L.W / 2 > (size_t)INT32_MAX)
+      return fail("layer " + std::to_string(layer) + ": parameter table_fwd has " + std::to_string(numel) +
+                  " values, expected (knots + 1) x " + std::to_string(L.W) + " with at least one interval");
+    // w(cutoff) = 0 for both envelopes; conv_fwd also sends the edges it leaves to the cubic table to this knot
+    for (size_t c = 0; c < (size_t)L.W; ++c)
+      if (host[(rows - 1) * L.W + c] != 0.0f)
+        return fail("layer " + std::to_string(layer) + ": parameter table_fwd: the last knot (r = cutoff) must be 0");
+    int off[kMaxL];
+    img = role_table_images(L, (int)rows, host, 2, off);
+    host = img.data();
+    for (int l1 = 0; l1 < L.n_lx; ++l1) L.roles[l1].ftab_off = off[l1];
+    L.ftab_knots = (int)rows - 1;
   }
   if (dst->ensure(numel * sizeof(float))) return fail("cudaMalloc failed for parameter " + nm);
   S7B_CUDA_CHECK(cudaMemcpy(dst->p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
@@ -1214,6 +1239,9 @@ static ConvArgs make_conv_args(const S7bEngine* e, int t, const float* x) {
   a.dim_mid = L.dim_mid;
   a.w_numel = L.W;
   a.inv_h = e->radial.inv_h;
+  a.ftable = reinterpret_cast<const float2*>(lparam(e, t, "table_fwd"));
+  a.ftab_knots = L.ftab_knots;
+  a.ftab_inv_h = L.ftab_knots > 0 ? (float)L.ftab_knots / e->desc.cutoff : 0.0f;
   return a;
 }
 
@@ -1296,7 +1324,8 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         if (dense_gemm(e->h1[t].as<float>(), h0, e->h2[t].as<float>(), h1, w1, E, kEpiSiluStoreZ, nullptr, e->z2[t].as<float>(), false, st)) return 1;
         if (dense_gemm(e->h2[t].as<float>(), h1, e->wbuf[t].as<float>(), L.W, w2, E, kEpiNone, nullptr, nullptr, false, st)) return 1;
       } else if (head && table) {
-        if (require(lparam(e, t, "table"), "table") || require(lparam(e, t, "table23"), "table23")) return 1;
+        if (require(lparam(e, t, "table"), "table") || require(lparam(e, t, "table23"), "table23") ||
+            require(lparam(e, t, "table_fwd"), "table_fwd")) return 1;
       }
       // convolution: gather + tensor product + scatter (raw sums; 1/denominator is folded into si2)
       ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());

@@ -13,7 +13,9 @@ modules (SURVEY Appendix A.5-A.7) and folds them into the arrays once, in float6
     atom's species): 1/sqrt(fan_in * num_species) per block; folded into ``embed_g0`` in layer 0
   * the two bias-free readout linears (``sevenn/model_build.py:102-123``) folded into one vector
   * the radial MLP ``FullyConnectedNet`` (``convolution.py:93-95,121``) either kept exact
-    (``radial='mlp'``) or tabulated as cubic Hermite splines of the edge length (``radial='table'``)
+    (``radial='mlp'``) or tabulated on uniform grids of the edge length (``radial='table'``): cubic Hermite
+    splines for the backward, which needs dw/dr, and values on a three times finer grid, interpolated linearly,
+    for the forward
 """
 from __future__ import annotations
 
@@ -209,6 +211,49 @@ def radial_table(spec: ModelSpec, arrays: Dict[str, np.ndarray], t: int, knots: 
     return np.ascontiguousarray(tab, dtype=np.float32)
 
 
+def forward_table_knots(knots: int) -> int:
+    """Intervals of the forward value table for a cubic table of ``knots`` intervals.  Three times as many: every
+    cubic knot (r_on included, see ``default_table_knots``) is a value knot, and the value table ((3K + 1) rows of
+    4 B per weight) is no larger than the cubic one (K rows of 12 B per weight) but one row, so x and the table of
+    a layer still share L2 as before."""
+    return 3 * knots
+
+
+def radial_value_table(spec: ModelSpec, arrays: Dict[str, np.ndarray], t: int, fknots: int) -> np.ndarray:
+    """[fknots + 1, W] fp32 knot values at r_k = k * cutoff / fknots: the forward's table, read at knots k and k + 1
+    and interpolated linearly.  A row holds every channel pair (2c, 2c + 1) as one float2.
+
+    Linear interpolation of w errs by h^2 w'' t (1 - t) / 2 inside an interval: one sign wherever w is convex or
+    concave, so summed over a few hundred thousand edges it biases the energy (by 4.6e-3 eV on the 12 000-atom Si
+    cell, against 2.8e-4 eV with the cubic table).  The knot values are therefore w_k - h^2 w''_k / 12 (w'' from the
+    second difference of w on the grid): the error then averages to zero over each interval, and its largest value
+    drops from h^2 w'' / 8 to h^2 w'' / 12.  The last knot is w(cutoff) = 0, exactly (both envelopes vanish there;
+    the kernel also points the edges it leaves to the cubic table at it), so w stays continuous at the cutoff; the
+    first takes the second difference of its neighbour."""
+    r = np.arange(fknots + 1, dtype=np.float64) * (spec.cutoff / fknots)
+    f, _ = radial_weights(spec, arrays, t, r)
+    d2 = np.zeros_like(f)
+    d2[1:-1] = f[2:] - 2.0 * f[1:-1] + f[:-2]
+    d2[0] = d2[1]
+    v = f - d2 / 12.0
+    v[-1] = 0.0
+    return np.ascontiguousarray(v, dtype=np.float32)
+
+
+def value_table_read(tab: np.ndarray, cutoff: float, r) -> np.ndarray:
+    """w [len(r), W] float64 as ``conv_fwd`` reads a value table ``tab`` [Kf + 1, W] at fp32 radii r
+    (conv_kernels.cuh ``value_table_rec``): k = (int)(r * f32(Kf / cutoff)) clamped to [0, Kf - 1], t = fma(r,
+    f32(Kf / cutoff), -k) rounded to fp32 and clamped to [0, 1], w = (1 - t) v_k + t v_k+1.  (The kernel takes the
+    edges shorter than 0.6 A from the cubic table instead, conv_kernels.cuh ``kValueTableMinR``.)"""
+    K = tab.shape[0] - 1
+    inv_h = np.float32(np.float32(K) / np.float32(cutoff))
+    r32 = np.asarray(r, dtype=np.float32)
+    k = np.clip((r32 * inv_h).astype(np.int64), 0, K - 1)
+    # the fp32 x fp32 product is exact in float64, so this is the FMA's single rounding
+    t = np.clip((r32.astype(np.float64) * float(inv_h) - k).astype(np.float32), 0, 1).astype(np.float64)[:, None]
+    return (1.0 - t) * tab[k].astype(np.float64) + t * tab[k + 1].astype(np.float64)
+
+
 def pack_table_pairs(tab: np.ndarray):
     """[knots, W, 4] -> the two device arrays a lane reads for its channel pair:
     ``table``   [knots, W/2, 4] fp32 {a0e, a0o, a1e, a1o}  (value and slope*h: need fp32)
@@ -298,6 +343,7 @@ def prepare_params(spec: ModelSpec, arrays: Dict[str, np.ndarray], radial: str, 
         out[('si2T', t)] = np.concatenate([b.T.ravel() for b in si2])
         if radial == 'table':
             out[('table', t)], out[('table23', t)] = pack_table_pairs(radial_table(spec, arrays, t, knots))
+            out[('table_fwd', t)] = radial_value_table(spec, arrays, t, forward_table_knots(knots))
         else:
             for j in range(len(spec.radial_hidden) + 1):
                 W = f64(arrays[f'{t}.mlp{j}'])
@@ -348,8 +394,8 @@ class _DevView:
 
 
 class B200Engine:
-    """One model on one GPU.  ``radial``: 'table' (cubic-spline radial weights, default) or 'mlp'
-    (the radial MLP evaluated exactly per edge with FP32 GEMM kernels)."""
+    """One model on one GPU.  ``radial``: 'table' (tabulated radial weights, default: a value table for the forward,
+    cubic splines for the backward) or 'mlp' (the radial MLP evaluated exactly per edge with FP32 GEMM kernels)."""
 
     def __init__(self, meta: dict, arrays: Dict[str, np.ndarray], radial: str = 'table',
                  knots: Optional[int] = None, device: Optional[int] = None, atomic_virial: bool = False):
