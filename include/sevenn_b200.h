@@ -166,7 +166,10 @@ S7B_API int s7b_engine_set_atomic_virial(S7bEngine* eng, int enable);
  * "table23" are the backward's cubic table on table_knots intervals; "table_fwd" ([Kf + 1][W]) holds the forward's knot
  * values on Kf intervals of its own, read from its size (engine.py uses Kf = 3 table_knots).  A layer with the species-wise
  * ('nequip') self-connection takes "sc_species" / "scT_species" ([num_species][l block][K][N], the transpose per block)
- * instead of "sc" / "scT"; setting both kinds on one layer is an error. */
+ * instead of "sc" / "scT"; setting both kinds on one layer is an error.  Global names take layer -1, per-layer names
+ * 0 <= layer < n_layers.  Every array is checked against the element count the kernels read (from S7bModelDesc;
+ * for "table_fwd", its shape rules above); unknown names, wrong layers and wrong sizes are refused with an error that
+ * names the parameter, and a refused call leaves the engine as it was. */
 S7B_API int s7b_engine_set_param(S7bEngine* eng, const char* name, int layer, const float* host, size_t numel);
 
 /* Describe the graph of this step (device pointers, kept by reference until the next call).

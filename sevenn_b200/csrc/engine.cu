@@ -129,19 +129,21 @@ struct ProfScope {
   ~ProfScope() { if (p) cudaEventRecord(b, st); }
 };
 
+// An irreps layout of node rows of `dim` floats: block l (l < n_l) holds mul[l] channels x (2l + 1) components
+// from float off[l] on (component-major, DESIGN.md §3).
+struct Irreps {
+  int n_l = 0, dim = 0;
+  int off[kMaxL] = {0}, mul[kMaxL] = {0};
+};
+
 struct LayerCfg {
-  int n_lx = 0, n_lg = 0;             // number of l's in x / gate-out irreps
-  int x_muls[kMaxL] = {0}, out_muls[kMaxL] = {0}, g_muls[kMaxL] = {0};
-  int x_off[kMaxL] = {0}, g_off[kMaxL] = {0}, h_off[kMaxL] = {0};
-  int dim_x = 0, dim_g = 0, dim_h = 0, dim_mid = 0, W = 0;
-  int mid_K[kMaxL] = {0}, mid_off[kMaxL] = {0};
+  Irreps x, g, mid;                   // layer input, gate input (gate-out irreps + gates), convolution output (mul = K per l3)
+  int out_muls[kMaxL] = {0}, h_off[kMaxL] = {0};
+  int dim_h = 0, W = 0;
   int lmax_out = 0;
-  int ftab_knots = 0;                 // intervals of the forward value table ("table_fwd"; 0 until it is set)
   std::vector<PathCfg> paths;
   ConvRole roles[kMaxL];
   GateDesc gate;
-  std::map<std::string, DevBuf> params;
-  std::map<std::string, struct TcWeights*> tcw;   // tensor-core form of si1/si1T/sc/scT/si2/si2T (engine.cu: TcWeights)
 };
 
 // Row exponents of a GEMM input (tc_gemm.cuh): E[n, row_base[l] + i]
@@ -151,6 +153,50 @@ struct RowExp {
   bool bits = false;      // raw |a|-maximum bits (filled by the producer kernel) instead of exponents
 };
 
+// Pre-sliced weights of one block-diagonal linear (see tc_gemm.cuh): per block l the three bf16 slices of
+// W^T in the 64B-swizzled K-major layout, cut into (n tile, 32-wide K chunk) blobs that one
+// cp.async.bulk moves into a pipeline stage, plus the per-column scales 2^(Eb-7).
+struct TcWeights {
+  DevBuf q, fb;
+  int nblocks = 0;
+  bool ok = false;
+  struct Blk { int K, N, NT; size_t q_off, fb_off; } blk[kMaxL];
+};
+
+// One node linear of a layer: n_l blocks from layout `in` to layout `out` (block l: [in->mul[l]][out->mul[l]]
+// fp32, the blocks one after another in `w`), and the tensor-core form of `w`.  The layouts are those of
+// S7bEngine::layers, which is sized once at creation.  A self-connection slot holds either the linear kind or the
+// species-wise ('nequip') kind: `species`, [num_species] copies of the blocks in `w` and no tensor-core form.
+struct NodeLinear {
+  const Irreps* in = nullptr;
+  const Irreps* out = nullptr;
+  int n_l = 0;
+  bool species = false;
+  DevBuf w;
+  TcWeights tc;
+};
+
+// The per-layer parameters that s7b_engine_set_param uploads
+struct LayerParams {
+  NodeLinear si1, si1T, sc, scT, si2, si2T;
+  DevBuf table, table23, table_fwd;   // radial tables, as one image per l1 role (role_table_images)
+  int ftab_knots = 0;                 // intervals of table_fwd (0 until it is set)
+  DevBuf mlp[3], mlpT[3];             // radial MLP ('mlp' mode) and its transposes
+  void release() {
+    for (NodeLinear* s : {&si1, &si1T, &sc, &scT, &si2, &si2T})
+      for (DevBuf* b : {&s->w, &s->tc.q, &s->tc.fb}) b->release();
+    for (DevBuf* b : {&table, &table23, &table_fwd, &mlp[0], &mlp[1], &mlp[2], &mlpT[0], &mlpT[1], &mlpT[2]}) b->release();
+  }
+};
+
+// The global parameters ("bessel" lives in RadialDesc)
+struct GlobalParams {
+  DevBuf embed_x0, embed_g0, readout, readout_lo, scale, shift;
+  void release() {
+    for (DevBuf* b : {&embed_x0, &embed_g0, &readout, &readout_lo, &scale, &shift}) b->release();
+  }
+};
+
 }  // namespace s7b
 
 using namespace s7b;
@@ -158,7 +204,8 @@ using namespace s7b;
 struct S7bEngine {
   S7bModelDesc desc;
   std::vector<LayerCfg> layers;
-  std::map<std::string, DevBuf> params;   // global parameters
+  std::vector<LayerParams> layer_params;
+  GlobalParams global_params;
   RadialDesc radial;
   bool radial_ready = false;
   int ny_stride = 8;
@@ -241,8 +288,9 @@ static int irreps_dim(const int* muls, int n_l) {
 // widths kConvMul of SevenNet-0 / SevenNet-l3i5 on specialised kernels, every other on the runtime-width ones.
 static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* out_muls, int n_lo,
                            int lmax_filter, int knots, int layer) {
-  L.n_lx = n_lx;
-  L.n_lg = n_lo;
+  L.x.n_l = n_lx;
+  L.g.n_l = n_lo;
+  L.mid.n_l = n_lo;
   L.lmax_out = n_lo - 1;
   int off = 0;
   for (int l = 0; l < n_lx; ++l) {
@@ -250,25 +298,25 @@ static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* 
       return fail("convolution multiplicities must be positive multiples of 32, at most " +
                   std::to_string(kConvMaxMul) + ": " + (layer >= 0 ? "layer " + std::to_string(layer) : std::string("x")) +
                   " has " + std::to_string(x_muls[l]) + " channels of l = " + std::to_string(l));
-    L.x_muls[l] = x_muls[l];
-    L.x_off[l] = off;
+    L.x.mul[l] = x_muls[l];
+    L.x.off[l] = off;
     off += (2 * l + 1) * x_muls[l];
   }
-  L.dim_x = off;
+  L.x.dim = off;
   int n_gates = 0;
   for (int l = 1; l < n_lo; ++l) n_gates += out_muls[l];
   for (int l = 0; l < n_lo; ++l) {
     if (out_muls[l] % 32 != 0 || out_muls[l] <= 0) return fail("multiplicities must be positive multiples of 32");
     L.out_muls[l] = out_muls[l];
-    L.g_muls[l] = out_muls[l] + (l == 0 ? n_gates : 0);
+    L.g.mul[l] = out_muls[l] + (l == 0 ? n_gates : 0);
   }
-  L.dim_g = irreps_dim(L.g_muls, n_lo);
+  L.g.dim = irreps_dim(L.g.mul, n_lo);
   L.dim_h = irreps_dim(L.out_muls, n_lo);
   off = 0;
   int hoff = 0;
   for (int l = 0; l < n_lo; ++l) {
-    L.g_off[l] = off;
-    off += (2 * l + 1) * L.g_muls[l];
+    L.g.off[l] = off;
+    off += (2 * l + 1) * L.g.mul[l];
     L.h_off[l] = hoff;
     hoff += (2 * l + 1) * L.out_muls[l];
   }
@@ -295,17 +343,17 @@ static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* 
   L.W = w_off;
   off = 0;
   for (int l = 0; l <= L.lmax_out; ++l) {
-    L.mid_K[l] = k_run[l];
-    L.mid_off[l] = off;
+    L.mid.mul[l] = k_run[l];
+    L.mid.off[l] = off;
     off += (2 * l + 1) * k_run[l];
   }
-  L.dim_mid = off;
+  L.mid.dim = off;
   // conv roles: per l1 the paths in slot order; the role's table image follows those of the smaller l1
   int tab_off = 0;
   for (int l1 = 0; l1 < n_lx; ++l1) {
     ConvRole& r = L.roles[l1];
     memset(&r, 0, sizeof(r));
-    r.x_off = L.x_off[l1];
+    r.x_off = L.x.off[l1];
     r.mul = x_muls[l1];
     r.tab_off = tab_off;
     int p = 0;
@@ -313,8 +361,8 @@ static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* 
       if (q.l1 != l1) continue;
       if (p >= kMaxPaths) return fail("too many paths for one l1");
       r.w_off[p] = q.w_off;
-      r.out_off[p] = L.mid_off[q.l3] + q.k_off;
-      r.out_stride[p] = L.mid_K[q.l3];
+      r.out_off[p] = L.mid.off[q.l3] + q.k_off;
+      r.out_stride[p] = L.mid.mul[q.l3];
       ++p;
     }
     tab_off += knots * p * (r.mul / 2);
@@ -324,14 +372,14 @@ static int build_layer_cfg(LayerCfg& L, const int* x_muls, int n_lx, const int* 
   memset(&gd, 0, sizeof(gd));
   gd.n_scalars = out_muls[0];
   gd.lmax = n_lo - 1;
-  gd.dim_g = L.dim_g;
+  gd.dim_g = L.g.dim;
   gd.dim_h = L.dim_h;
   int goff = out_muls[0];
   for (int l = 0; l < kMaxL; ++l) {
     gd.mul[l] = l < n_lo ? out_muls[l] : 0;
-    gd.g_off[l] = l < n_lo ? L.g_off[l] : L.dim_g;
+    gd.g_off[l] = l < n_lo ? L.g.off[l] : L.g.dim;
     gd.h_off[l] = l < n_lo ? L.h_off[l] : L.dim_h;
-    gd.gate_off[l] = L.g_muls[0];
+    gd.gate_off[l] = L.g.mul[0];
   }
   for (int l = 1; l < n_lo; ++l) {
     gd.gate_off[l] = goff;
@@ -380,16 +428,6 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
 }
 
 // ---- tensor-core linear: host side --------------------------------------------------------------
-// Pre-sliced weights of one block-diagonal linear (see tc_gemm.cuh): per block l the three bf16 slices of
-// W^T in the 64B-swizzled K-major layout, cut into (n tile, 32-wide K chunk) blobs that one
-// cp.async.bulk moves into a pipeline stage, plus the per-column scales 2^(Eb-7).
-struct TcWeights {
-  DevBuf q, fb;
-  int nblocks = 0;
-  bool ok = false;
-  struct Blk { int K, N, NT; size_t q_off, fb_off; } blk[kMaxL];
-};
-
 // column tiling of an N-wide block: as few tiles of <= 128 columns as possible, tile width a multiple of 16;
 // the last tile may be padded (zero weights, masked in the epilogue)
 static int tc_pick_nt(int N) {
@@ -703,18 +741,24 @@ static int launch_species_segment(const int* species, int n, int S, int* perm, i
   return 0;
 }
 
-// One block-diagonal node linear of layer `L`, parameter `name`: tensor cores when the shapes allow it
-// (default), else the FP32 SIMT kernel.  `re` holds the row exponents of A; `fresh_re` = compute them now
-// over the n_l_A irrep blocks of A (a later call on the same A reuses them).
-static int node_linear(const LayerCfg& L, const char* name, RowExp& re, bool fresh_re, int n_l_A, const float* A,
-                       int lda, const int* a_off, const int* a_K, float* C, int ldc, const int* c_off,
-                       const int* c_N, int n_l, const float* W, int n_nodes, bool accumulate, cudaStream_t st) {
-  auto it = L.tcw.find(name);
-  if (g_opt_tc_gemm && it != L.tcw.end() && it->second && it->second->ok) {
-    if (fresh_re && launch_row_exponents(re, A, lda, a_off, a_K, n_l_A, n_nodes, st)) return 1;
-    return launch_tc_linear(*it->second, re, A, lda, a_off, a_K, C, ldc, c_off, c_N, n_l, n_nodes, accumulate, st);
+// A node linear runs on the tensor cores (default) when its shapes allowed a tensor-core form
+static bool on_tc(const NodeLinear& s) { return g_opt_tc_gemm && s.tc.ok; }
+
+// Node linear `s` over the local rows of engine `e`, shapes from the slot: the species-wise kernel for the species-wise
+// kind, else the tensor cores when on_tc, else the FP32 SIMT kernel.  `re` holds the row exponents of A; `fresh_re` =
+// compute them now over all irrep blocks of A (a later call on the same A reuses them).
+static int node_linear(const S7bEngine* e, const NodeLinear& s, RowExp& re, bool fresh_re, const float* A, float* C,
+                       bool accumulate, cudaStream_t st) {
+  const Irreps &a = *s.in, &c = *s.out;
+  const int n = e->n_local;
+  if (s.species)
+    return launch_species_linear(A, a.dim, a.off, a.mul, C, c.dim, c.off, c.mul, s.n_l, s.w.as<float>(), e->desc.num_species,
+                                 e->seg_perm.as<int>(), e->seg.as<int>(), n, accumulate, st);
+  if (on_tc(s)) {
+    if (fresh_re && launch_row_exponents(re, A, a.dim, a.off, a.mul, a.n_l, n, st)) return 1;
+    return launch_tc_linear(s.tc, re, A, a.dim, a.off, a.mul, C, c.dim, c.off, c.mul, s.n_l, n, accumulate, st);
   }
-  return irreps_linear(A, lda, a_off, a_K, C, ldc, c_off, c_N, n_l, W, n_nodes, accumulate, st);
+  return irreps_linear(A, a.dim, a.off, a.mul, C, c.dim, c.off, c.mul, s.n_l, s.w.as<float>(), n, accumulate, st);
 }
 
 static int dense_gemm(const float* A, int K, float* C, int N, const float* W, int64_t rows, int epilogue,
@@ -743,7 +787,7 @@ static int dense_gemm(const float* A, int K, float* C, int N, const float* W, in
 
 static int conv_forward(const LayerCfg& L, int lmax_filter, bool table, ConvArgs a, float* out,
                         cudaStream_t st) {
-  for (int l1 = 0; l1 < L.n_lx; ++l1)
+  for (int l1 = 0; l1 < L.x.n_l; ++l1)
     if (launch_conv_fwd(l1, lmax_filter, L.lmax_out, table, a, L.roles[l1], out, st)) return 1;
   return 0;
 }
@@ -758,7 +802,7 @@ static std::vector<float> role_table_images(const LayerCfg& L, int rows, const f
                                             int* role_off) {
   std::vector<float> img((size_t)rows * (L.W / 2) * floats_per_pair);
   float* dst = img.data();
-  for (int l1 = 0; l1 < L.n_lx; ++l1) {
+  for (int l1 = 0; l1 < L.x.n_l; ++l1) {
     const ConvRole& r = L.roles[l1];
     std::vector<int> cols;
     for (const PathCfg& q : L.paths)
@@ -956,12 +1000,26 @@ int s7b_engine_create(const S7bModelDesc* d, S7bEngine** out) {
       return 1;
     }
   }
-  if (e->layers[0].n_lx != 1) {
+  if (e->layers[0].x.n_l != 1) {
     delete e;
     return fail("the first layer input must be scalars only");
   }
-  e->ny_stride = y_stride((d->lmax_filter + 1) * (d->lmax_filter + 1));
   const int T = d->n_layers;
+  // the node linears of a layer (the transposes run the other way): si1 x -> x, sc x -> g on the l's both
+  // have, si2 mid -> g
+  e->layer_params.resize(T);
+  for (int t = 0; t < T; ++t) {
+    const LayerCfg& L = e->layers[t];
+    LayerParams& P = e->layer_params[t];
+    const int n_sc = std::min(L.x.n_l, L.g.n_l);
+    P.si1 = {&L.x, &L.x, L.x.n_l};
+    P.si1T = {&L.x, &L.x, L.x.n_l};
+    P.sc = {&L.x, &L.g, n_sc};
+    P.scT = {&L.g, &L.x, n_sc};
+    P.si2 = {&L.mid, &L.g, L.g.n_l};
+    P.si2T = {&L.g, &L.mid, L.g.n_l};
+  }
+  e->ny_stride = y_stride((d->lmax_filter + 1) * (d->lmax_filter + 1));
   e->x.resize(T);
   e->g.resize(T);
   e->wbuf.resize(T);
@@ -1006,12 +1064,8 @@ void s7b_engine_destroy(S7bEngine* e) {
   if (e->g_in) cudaEventDestroy(e->g_in);
   if (e->g_out) cudaEventDestroy(e->g_out);
   e->d_nE.release();
-  for (auto& kv : e->params) kv.second.release();
-  for (auto& L : e->layers) {
-    for (auto& kv : L.params) kv.second.release();
-    for (auto& kv : L.tcw)
-      if (kv.second) { kv.second->q.release(); kv.second->fb.release(); delete kv.second; }
-  }
+  e->global_params.release();
+  for (LayerParams& P : e->layer_params) P.release();
   for (RowExp* r : {&e->re_mid, &e->re_h, &e->re_dg, &e->re_dx}) r->buf.release();
   e->seg_perm.release();
   e->seg.release();
@@ -1035,107 +1089,112 @@ int s7b_engine_set_atomic_virial(S7bEngine* e, int enable) {
   return 0;
 }
 
-int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float* host, size_t numel) {
-  if (!e || !name || !host) return fail("null argument");
-  const std::string nm(name);
-  if (nm == "sc_species" || nm == "scT_species") {
-    // species-wise ('nequip') self-connection: [num_species][l block][K][N] (scT_species: each block transposed)
-    if (layer < 0 || layer >= e->desc.n_layers) return fail("parameter " + nm + " needs a layer in [0, n_layers)");
-    const LayerCfg& L = e->layers[layer];
-    if (L.params.count("sc") || L.params.count("scT"))
-      return fail("layer " + std::to_string(layer) + ": parameter " + nm + " and the linear self-connection 'sc' / 'scT' cannot both be set");
-    const int S = e->desc.num_species;
-    if (S < 1 || S > kMaxSpeciesSc) return fail("parameter " + nm + ": num_species must be 1.." + std::to_string(kMaxSpeciesSc));
-    size_t per = 0;
-    for (int l = 0; l < std::min(L.n_lx, L.n_lg); ++l) per += (size_t)L.x_muls[l] * L.g_muls[l];
-    if (numel != per * S)
-      return fail("layer " + std::to_string(layer) + ": parameter " + nm + " has " + std::to_string(numel) + " values, expected " +
-                  std::to_string(per * S) + " (num_species " + std::to_string(S) + " x " + std::to_string(per) + ")");
-    DevBuf& dst = e->layers[layer].params[nm];
-    if (dst.ensure(numel * sizeof(float))) return fail("cudaMalloc failed for parameter " + nm);
-    S7B_CUDA_CHECK(cudaMemcpy(dst.p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
-    if (!e->species_sc) {
-      e->species_sc = true;
-      if (e->seg.ensure((2 * (size_t)S + 2) * sizeof(int)) || e->seg_perm.ensure((size_t)std::max(e->n_local, 1) * sizeof(int)))
-        return fail("cudaMalloc failed for the species segmentation");
-      ++g_alloc_gen;
-    }
-    return 0;
-  }
-  if (layer >= 0 && (nm == "sc" || nm == "scT") && layer < e->desc.n_layers &&
-      (e->layers[layer].params.count("sc_species") || e->layers[layer].params.count("scT_species")))
-    return fail("layer " + std::to_string(layer) + ": parameter " + nm + " and the species-wise self-connection 'sc_species' / 'scT_species' cannot both be set");
-  if (nm == "bessel") {
-    if ((int)numel != e->desc.n_basis) return fail("bessel: wrong size");
-    for (int b = 0; b < e->desc.n_basis; ++b) e->radial.coeffs[b] = host[b];
-    e->radial_ready = true;
-    return 0;
-  }
-  DevBuf* dst;
-  if (layer < 0) dst = &e->params[nm];
-  else {
-    if (layer >= e->desc.n_layers) return fail("layer out of range");
-    dst = &e->layers[layer].params[nm];
-  }
-  std::vector<float> img;
-  if (layer >= 0 && (nm == "table" || nm == "table23")) {
-    const int fpp = nm == "table" ? 4 : 2;
-    const LayerCfg& L = e->layers[layer];
-    if (e->desc.table_knots <= 0) return fail("parameter " + nm + ": the model was created without radial tables");
-    if (numel != (size_t)e->desc.table_knots * (L.W / 2) * fpp)
-      return fail("parameter " + nm + ": size does not match the layer configuration and knot count");
-    int off[kMaxL];
-    img = role_table_images(L, e->desc.table_knots, host, fpp, off);
-    host = img.data();
-  }
-  if (layer >= 0 && nm == "table_fwd") {
-    // the forward's value table: w at knots 0..Kf over [0, cutoff], [Kf + 1][W] fp32.  Kf is the host's choice
-    // (engine.py forward_table_knots) and is read from the size; the kernels index it with 32 bits.
-    LayerCfg& L = e->layers[layer];
-    if (e->desc.table_knots <= 0) return fail("parameter " + nm + ": the model was created without radial tables");
-    const size_t rows = numel / (size_t)L.W;
-    if (numel % (size_t)L.W != 0 || rows < 2 || rows * (size_t)L.W / 2 > (size_t)INT32_MAX)
-      return fail("layer " + std::to_string(layer) + ": parameter table_fwd has " + std::to_string(numel) +
-                  " values, expected (knots + 1) x " + std::to_string(L.W) + " with at least one interval");
-    // w(cutoff) = 0 for both envelopes; conv_fwd also sends the edges it leaves to the cubic table to this knot
-    for (size_t c = 0; c < (size_t)L.W; ++c)
-      if (host[(rows - 1) * L.W + c] != 0.0f)
-        return fail("layer " + std::to_string(layer) + ": parameter table_fwd: the last knot (r = cutoff) must be 0");
-    int off[kMaxL];
-    img = role_table_images(L, (int)rows, host, 2, off);
-    host = img.data();
-    for (int l1 = 0; l1 < L.n_lx; ++l1) L.roles[l1].ftab_off = off[l1];
-    L.ftab_knots = (int)rows - 1;
-  }
-  if (dst->ensure(numel * sizeof(float))) return fail("cudaMalloc failed for parameter " + nm);
-  S7B_CUDA_CHECK(cudaMemcpy(dst->p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
-  if (layer >= 0 && (nm == "si1" || nm == "si1T" || nm == "sc" || nm == "scT" || nm == "si2" || nm == "si2T")) {
-    // tensor-core form: block shapes from the layer configuration
-    LayerCfg& L = e->layers[layer];
-    int Ks[kMaxL] = {0, 0, 0, 0}, Ns[kMaxL] = {0, 0, 0, 0}, n_l = 0;
-    const bool T = nm.back() == 'T';
-    if (nm.rfind("si1", 0) == 0) { n_l = L.n_lx; for (int l = 0; l < n_l; ++l) { Ks[l] = L.x_muls[l]; Ns[l] = L.x_muls[l]; } }
-    else if (nm.rfind("sc", 0) == 0) { n_l = std::min(L.n_lx, L.n_lg); for (int l = 0; l < n_l; ++l) { Ks[l] = L.x_muls[l]; Ns[l] = L.g_muls[l]; } }
-    else { n_l = L.n_lg; for (int l = 0; l < n_l; ++l) { Ks[l] = L.mid_K[l]; Ns[l] = L.g_muls[l]; } }
-    if (T) for (int l = 0; l < n_l; ++l) std::swap(Ks[l], Ns[l]);
-    size_t expect = 0;
-    for (int l = 0; l < n_l; ++l) expect += (size_t)Ks[l] * Ns[l];
-    if (expect != numel) return fail("parameter " + nm + ": size does not match the layer configuration");
-    TcWeights*& w = L.tcw[nm];
-    if (!w) w = new TcWeights();
-    if (tc_build_weights(*w, host, Ks, Ns, n_l)) return 1;
-    ++g_alloc_gen;
-  }
+static int upload(DevBuf& dst, const float* host, size_t numel, const std::string& what) {
+  if (dst.ensure(numel * sizeof(float))) return fail("cudaMalloc failed for " + what);
+  S7B_CUDA_CHECK(cudaMemcpy(dst.p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
   return 0;
 }
 
-static const float* lparam(const S7bEngine* e, int t, const char* name) {
-  auto it = e->layers[t].params.find(name);
-  return it == e->layers[t].params.end() ? nullptr : it->second.as<float>();
-}
-static const float* gparam(const S7bEngine* e, const char* name) {
-  auto it = e->params.find(name);
-  return it == e->params.end() ? nullptr : it->second.as<float>();
+// The name selects the slot and the element count the kernels read.  Every check comes before the first device call
+// and the first change to the engine, so a refused call leaves the engine as it was.
+int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float* host, size_t numel) {
+  if (!e || !name || !host) return fail("null argument");
+  const std::string nm(name);
+  const int T = e->desc.n_layers, S = e->desc.num_species, nb = e->desc.n_basis;
+  const std::string what = (layer >= 0 ? "layer " + std::to_string(layer) + ": " : std::string()) + "parameter " + nm;
+  auto bad_size = [&](size_t expect) {
+    return numel == expect ? 0 : fail(what + " has " + std::to_string(numel) + " values, expected " + std::to_string(expect));
+  };
+  // global parameters: layer < 0
+  GlobalParams& G = e->global_params;
+  const LayerCfg &L0 = e->layers[0], &Lz = e->layers[T - 1];
+  const struct { const char* name; DevBuf* buf; size_t numel; } globals[] = {
+      {"embed_x0", &G.embed_x0, (size_t)S * L0.x.dim}, {"embed_g0", &G.embed_g0, (size_t)S * L0.g.dim},
+      {"readout", &G.readout, (size_t)Lz.dim_h},       {"readout_lo", &G.readout_lo, (size_t)Lz.dim_h},
+      {"scale", &G.scale, (size_t)S},                  {"shift", &G.shift, (size_t)S},
+      {"bessel", nullptr, (size_t)nb}};
+  for (const auto& g : globals) {
+    if (nm != g.name) continue;
+    if (layer >= 0) return fail(what + " is global: its layer must be negative");
+    if (bad_size(g.numel)) return 1;
+    if (g.buf) return upload(*g.buf, host, numel, what);
+    for (int b = 0; b < nb; ++b) e->radial.coeffs[b] = host[b];     // bessel: a kernel argument (RadialDesc)
+    e->radial_ready = true;
+    return 0;
+  }
+  // per-layer parameters (0 <= layer < n_layers): these three lists hold every per-layer name
+  static const std::pair<const char*, NodeLinear LayerParams::*> linears[] = {
+      {"si1", &LayerParams::si1}, {"si1T", &LayerParams::si1T}, {"sc", &LayerParams::sc}, {"scT", &LayerParams::scT},
+      {"sc_species", &LayerParams::sc}, {"scT_species", &LayerParams::scT}, {"si2", &LayerParams::si2},
+      {"si2T", &LayerParams::si2T}};
+  static const std::pair<const char*, DevBuf LayerParams::*> tables[] = {
+      {"table", &LayerParams::table}, {"table23", &LayerParams::table23}, {"table_fwd", &LayerParams::table_fwd}};
+  static const char* const mlps[] = {"mlp0", "mlp1", "mlp2", "mlp0T", "mlp1T", "mlp2T"};   // mlp[j], then mlpT[j]
+  auto named = [&](const auto& q) { return nm == q.first; };
+  const auto lin = std::find_if(std::begin(linears), std::end(linears), named);
+  const auto tab = std::find_if(std::begin(tables), std::end(tables), named);
+  const int mlp = (int)(std::find(std::begin(mlps), std::end(mlps), nm) - std::begin(mlps));
+  if (lin == std::end(linears) && tab == std::end(tables) && mlp == 6) return fail("unknown parameter '" + nm + "'");
+  if (layer < 0 || layer >= T)
+    return fail("parameter " + nm + " is per layer: layer " + std::to_string(layer) + " is outside [0, " + std::to_string(T) + ")");
+  LayerCfg& L = e->layers[layer];
+  LayerParams& P = e->layer_params[layer];
+  if (lin != std::end(linears)) {
+    const bool species = nm == "sc_species" || nm == "scT_species";
+    NodeLinear& s = P.*(lin->second);
+    // one kind of self-connection per layer; checked before the size
+    if ((&s == &P.sc || &s == &P.scT) && ((P.sc.w.p && P.sc.species != species) || (P.scT.w.p && P.scT.species != species)))
+      return fail(what + " and the " + (species ? "linear self-connection 'sc' / 'scT'" : "species-wise self-connection 'sc_species' / 'scT_species'") +
+                  " cannot both be set");
+    if (species && (S < 1 || S > kMaxSpeciesSc)) return fail(what + ": num_species must be 1.." + std::to_string(kMaxSpeciesSc));
+    size_t n = 0;
+    for (int l = 0; l < s.n_l; ++l) n += (size_t)s.in->mul[l] * s.out->mul[l];
+    if (bad_size(species ? n * S : n) || upload(s.w, host, numel, what)) return 1;
+    s.species = species;
+    if (species) {
+      if (!e->species_sc) {
+        e->species_sc = true;
+        if (e->seg.ensure((2 * (size_t)S + 2) * sizeof(int)) || e->seg_perm.ensure((size_t)std::max(e->n_local, 1) * sizeof(int)))
+          return fail("cudaMalloc failed for the species segmentation");
+        ++g_alloc_gen;
+      }
+      return 0;
+    }
+    if (tc_build_weights(s.tc, host, s.in->mul, s.out->mul, s.n_l)) return 1;
+    ++g_alloc_gen;
+    return 0;
+  }
+  if (tab != std::end(tables)) {
+    DevBuf& dst = P.*(tab->second);
+    const int K = e->desc.table_knots;
+    if (K <= 0) return fail(what + ": the model was created without radial tables");
+    int off[kMaxL];
+    if (&dst != &P.table_fwd) {
+      const int fpp = &dst == &P.table ? 4 : 2;
+      if (bad_size((size_t)K * (L.W / 2) * fpp)) return 1;
+      const std::vector<float> img = role_table_images(L, K, host, fpp, off);
+      return upload(dst, img.data(), numel, what);
+    }
+    // the forward's value table: w at knots 0..Kf over [0, cutoff], [Kf + 1][W] fp32.  Kf is the host's choice
+    // (engine.py forward_table_knots) and is read from the size; the kernels index it with 32 bits.
+    const size_t rows = numel / (size_t)L.W;
+    if (numel % (size_t)L.W != 0 || rows < 2 || rows * (size_t)L.W / 2 > (size_t)INT32_MAX)
+      return fail(what + " has " + std::to_string(numel) + " values, expected (knots + 1) x " + std::to_string(L.W) +
+                  " with at least one interval");
+    // w(cutoff) = 0 for both envelopes; conv_fwd also sends the edges it leaves to the cubic table to this knot
+    for (size_t c = 0; c < (size_t)L.W; ++c)
+      if (host[(rows - 1) * L.W + c] != 0.0f) return fail(what + ": the last knot (r = cutoff) must be 0");
+    const std::vector<float> img = role_table_images(L, (int)rows, host, 2, off);
+    if (upload(dst, img.data(), numel, what)) return 1;
+    for (int l1 = 0; l1 < L.x.n_l; ++l1) L.roles[l1].ftab_off = off[l1];
+    P.ftab_knots = (int)rows - 1;
+    return 0;
+  }
+  // radial MLP (mlp < 6 here): mlp0 [n_basis][h0], mlp1 [h0][h1], mlp2 [h1][W]; mlp0T..mlp2T their transposes
+  const int j = mlp % 3;
+  const int dims[4] = {nb, e->desc.radial_hidden[0], e->desc.radial_hidden[1], L.W};
+  if (bad_size((size_t)dims[j] * dims[j + 1])) return 1;
+  return upload(mlp < 3 ? P.mlp[j] : P.mlpT[j], host, numel, what);
 }
 
 int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t n_edges,
@@ -1166,19 +1225,19 @@ int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t
   rc |= e->Y.ensure(E * e->ny_stride * sizeof(float));
   rc |= e->rlen.ensure(E * sizeof(float));
   int max_lx = 0;
-  for (auto& L : e->layers) max_lx = std::max(max_lx, L.n_lx);
+  for (auto& L : e->layers) max_lx = std::max(max_lx, L.x.n_l);
   rc |= e->dY_acc.ensure((size_t)max_lx * E * e->ny_stride * sizeof(float));
   rc |= e->dEdr_acc.ensure((size_t)max_lx * E * sizeof(float));
   rc |= e->fedge.ensure(E * 3 * sizeof(float));
   size_t max_mid = 0, max_h = 0, max_g = 0, max_x = 0, max_W = 0;
   for (int t = 0; t < T; ++t) {
     const LayerCfg& L = e->layers[t];
-    rc |= e->x[t].ensure(Nn * L.dim_x * sizeof(float));
-    rc |= e->g[t].ensure(Nl * L.dim_g * sizeof(float));
-    max_mid = std::max(max_mid, (size_t)L.dim_mid);
+    rc |= e->x[t].ensure(Nn * L.x.dim * sizeof(float));
+    rc |= e->g[t].ensure(Nl * L.g.dim * sizeof(float));
+    max_mid = std::max(max_mid, (size_t)L.mid.dim);
     max_h = std::max(max_h, (size_t)L.dim_h);
-    max_g = std::max(max_g, (size_t)L.dim_g);
-    max_x = std::max(max_x, (size_t)L.dim_x);
+    max_g = std::max(max_g, (size_t)L.g.dim);
+    max_x = std::max(max_x, (size_t)L.x.dim);
     max_W = std::max(max_W, (size_t)L.W);
     if (!table) {
       const int h0 = e->desc.radial_hidden[0], h1 = e->desc.radial_hidden[1];
@@ -1225,23 +1284,24 @@ int s7b_engine_set_interior(S7bEngine* e, int32_t n_interior) {
 
 static ConvArgs make_conv_args(const S7bEngine* e, int t, const float* x) {
   const LayerCfg& L = e->layers[t];
+  const LayerParams& P = e->layer_params[t];
   ConvArgs a;
   memset(&a, 0, sizeof(a));
   a.rowptr = e->d_rowptr;
   a.rec = e->rec.as<int4>();
   a.Y = e->Y.as<float>();
   a.x = x;
-  a.table = reinterpret_cast<const float4*>(lparam(e, t, "table"));
-  a.table23 = reinterpret_cast<const uint2*>(lparam(e, t, "table23"));
+  a.table = P.table.as<const float4>();
+  a.table23 = P.table23.as<const uint2>();
   a.w = e->desc.table_knots > 0 ? nullptr : e->wbuf[t].as<float>();
   a.n_dst = e->n_local;
-  a.dim_x = L.dim_x;
-  a.dim_mid = L.dim_mid;
+  a.dim_x = L.x.dim;
+  a.dim_mid = L.mid.dim;
   a.w_numel = L.W;
   a.inv_h = e->radial.inv_h;
-  a.ftable = reinterpret_cast<const float2*>(lparam(e, t, "table_fwd"));
-  a.ftab_knots = L.ftab_knots;
-  a.ftab_inv_h = L.ftab_knots > 0 ? (float)L.ftab_knots / e->desc.cutoff : 0.0f;
+  a.ftable = P.table_fwd.as<const float2>();
+  a.ftab_knots = P.ftab_knots;
+  a.ftab_inv_h = P.ftab_knots > 0 ? (float)P.ftab_knots / e->desc.cutoff : 0.0f;
   return a;
 }
 
@@ -1280,7 +1340,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         else edge_fwd_kernel<3><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, e->d_src, nE, e->ny_stride, e->rec.as<int4>(), e->Y.as<float>(), e->rlen.as<float>(), emb);
         S7B_LAUNCH_CHECK();
         int max_lx = 0;
-        for (auto& L : e->layers) max_lx = std::max(max_lx, L.n_lx);
+        for (auto& L : e->layers) max_lx = std::max(max_lx, L.x.n_l);
         S7B_CUDA_CHECK(cudaMemsetAsync(e->dY_acc.p, 0, (size_t)max_lx * Ecap * e->ny_stride * sizeof(float), st));
         S7B_CUDA_CHECK(cudaMemsetAsync(e->dEdr_acc.p, 0, (size_t)max_lx * Ecap * sizeof(float), st));
         if (!table) S7B_CUDA_CHECK(cudaMemsetAsync(e->demb_acc.p, 0, (size_t)E * e->desc.n_basis * sizeof(float), st));
@@ -1292,16 +1352,16 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         if (launch_species_segment(e->d_species, Nl, e->desc.num_species, e->seg_perm.as<int>(), e->seg.as<int>(), st)) return 1;
       }
       const LayerCfg& L0 = e->layers[0];
-      const float* ex = gparam(e, "embed_x0");
-      const float* eg = gparam(e, "embed_g0");
+      const float* ex = e->global_params.embed_x0.as<float>();
+      const float* eg = e->global_params.embed_g0.as<float>();
       if (require(ex, "embed_x0") || require(eg, "embed_g0")) return 1;
       ProfScope ps(e->prof, st, "embed_gather");
       if (Nn > 0) {
-        gather_rows_kernel<<<grid1d((size_t)Nn * L0.dim_x, 256), 256, 0, st>>>(ex, e->d_species, e->x[0].as<float>(), Nn, L0.dim_x, L0.dim_x);
+        gather_rows_kernel<<<grid1d((size_t)Nn * L0.x.dim, 256), 256, 0, st>>>(ex, e->d_species, e->x[0].as<float>(), Nn, L0.x.dim, L0.x.dim);
         S7B_LAUNCH_CHECK();
       }
       if (Nl > 0) {
-        gather_rows_kernel<<<grid1d((size_t)Nl * L0.dim_g, 256), 256, 0, st>>>(eg, e->d_species, e->g[0].as<float>(), Nl, L0.dim_g, L0.dim_g);
+        gather_rows_kernel<<<grid1d((size_t)Nl * L0.g.dim, 256), 256, 0, st>>>(eg, e->d_species, e->g[0].as<float>(), Nl, L0.g.dim, L0.g.dim);
         S7B_LAUNCH_CHECK();
       }
       return 0;
@@ -1312,11 +1372,12 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
     case S7B_STAGE_FWD_LAYER_A2: {
       if (t < 0 || t >= T) return fail("layer out of range");
       const LayerCfg& L = e->layers[t];
+      const LayerParams& P = e->layer_params[t];
       if (Nl == 0) return 0;
       const bool head = stage != S7B_STAGE_FWD_LAYER_A2;
       if (head && !table && E > 0) {
         // exact radial MLP (convolution.py:121): emb -> h1 -> h2 -> w
-        const float *w0 = lparam(e, t, "mlp0"), *w1 = lparam(e, t, "mlp1"), *w2 = lparam(e, t, "mlp2");
+        const float *w0 = P.mlp[0].as<float>(), *w1 = P.mlp[1].as<float>(), *w2 = P.mlp[2].as<float>();
         if (require(w0, "mlp0") || require(w1, "mlp1") || require(w2, "mlp2")) return 1;
         const int nb = e->desc.n_basis, h0 = e->desc.radial_hidden[0], h1 = e->desc.radial_hidden[1];
         ProfScope ps(e->prof, st, "radial_mlp_fwd", t);
@@ -1324,26 +1385,25 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         if (dense_gemm(e->h1[t].as<float>(), h0, e->h2[t].as<float>(), h1, w1, E, kEpiSiluStoreZ, nullptr, e->z2[t].as<float>(), false, st)) return 1;
         if (dense_gemm(e->h2[t].as<float>(), h1, e->wbuf[t].as<float>(), L.W, w2, E, kEpiNone, nullptr, nullptr, false, st)) return 1;
       } else if (head && table) {
-        if (require(lparam(e, t, "table"), "table") || require(lparam(e, t, "table23"), "table23") ||
-            require(lparam(e, t, "table_fwd"), "table_fwd")) return 1;
+        if (require(P.table.p, "table") || require(P.table23.p, "table23") || require(P.table_fwd.p, "table_fwd")) return 1;
       }
       // convolution: gather + tensor product + scatter (raw sums; 1/denominator is folded into si2)
       ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
       if (stage == S7B_STAGE_FWD_CONV_INTERIOR) ca.n_dst = e->n_interior;
       if (stage == S7B_STAGE_FWD_LAYER_A2) ca.n_begin = e->n_interior;
       // the convolution kernels also leave the row maxima of `mid` for the tensor-core self_interaction_2
-      const bool fused_rows = g_opt_tc_gemm && L.tcw.count("si2") && L.tcw.at("si2") && L.tcw.at("si2")->ok;
+      const bool fused_rows = on_tc(P.si2);
       if (fused_rows) {
-        e->re_mid.rows_per_node = L.n_lg * L.n_lg;
+        e->re_mid.rows_per_node = L.g.n_l * L.g.n_l;
         e->re_mid.bits = true;
         if (head) S7B_CUDA_CHECK(cudaMemsetAsync(e->re_mid.buf.p, 0, (size_t)Nl * e->re_mid.rows_per_node * sizeof(int), st));
         ca.row_max = e->re_mid.buf.as<unsigned int>();
         ca.rows_per_node = e->re_mid.rows_per_node;
       }
       {
-        const bool par = e->concurrent && g_opt_concurrent && !e->prof.enabled && L.n_lx > 1;
+        const bool par = e->concurrent && g_opt_concurrent && !e->prof.enabled && L.x.n_l > 1;
         if (par) S7B_CUDA_CHECK(cudaEventRecord(e->ev_fork, st));
-        for (int l1 = 0; l1 < L.n_lx; ++l1) {
+        for (int l1 = 0; l1 < L.x.n_l; ++l1) {
           cudaStream_t s1 = (par && l1 > 0) ? e->side[l1] : st;
           if (par && l1 > 0) S7B_CUDA_CHECK(cudaStreamWaitEvent(s1, e->ev_fork, 0));
           ProfScope ps(e->prof, s1, "conv_fwd", t, l1);
@@ -1356,20 +1416,18 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
       }
       if (stage == S7B_STAGE_FWD_CONV_INTERIOR) return 0;
       // self_interaction_2 accumulated onto the self-connection already stored in g[t]
-      const float* si2 = lparam(e, t, "si2");
-      if (require(si2, "si2")) return 1;
+      if (require(P.si2.w.p, "si2")) return 1;
       {
         ProfScope ps(e->prof, st, "si2_gemm", t);
-        if (node_linear(L, "si2", e->re_mid, !fused_rows, L.n_lg, e->mid.as<float>(), L.dim_mid, L.mid_off, L.mid_K, e->g[t].as<float>(), L.dim_g, L.g_off, L.g_muls, L.n_lg, si2, Nl, true, st)) return 1;
+        if (node_linear(e, P.si2, e->re_mid, !fused_rows, e->mid.as<float>(), e->g[t].as<float>(), true, st)) return 1;
       }
       // gate
       // gate; with the tensor-core linears the kernel also leaves the row exponents of h for self_interaction_1 / sc
-      const bool h_rows = g_opt_tc_gemm && t + 1 < T && e->layers[t + 1].tcw.count("si1") && e->layers[t + 1].tcw.at("si1") &&
-                          e->layers[t + 1].tcw.at("si1")->ok && L.n_lg * L.n_lg <= 16;
+      const bool h_rows = t + 1 < T && on_tc(e->layer_params[t + 1].si1) && L.g.n_l * L.g.n_l <= 16;
       {
         ProfScope ps(e->prof, st, "gate_fwd", t);
         if (h_rows) {
-          e->re_h.rows_per_node = L.n_lg * L.n_lg;
+          e->re_h.rows_per_node = L.g.n_l * L.g.n_l;
           e->re_h.bits = false;
           gate_fwd_rows_kernel<<<(Nl + 7) / 8, 256, 0, st>>>(L.gate, e->g[t].as<float>(), e->h.as<float>(), Nl, e->re_h.buf.as<int>(), e->re_h.rows_per_node, kTcZeroRow);
         } else {
@@ -1378,12 +1436,11 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         S7B_LAUNCH_CHECK();
       }
       if (t + 1 < T) {
-        const LayerCfg& N = e->layers[t + 1];
-        const float* si1 = lparam(e, t + 1, "si1");
-        if (require(si1, "si1")) return 1;
+        const NodeLinear& si1 = e->layer_params[t + 1].si1;
+        if (require(si1.w.p, "si1")) return 1;
         ProfScope ps(e->prof, st, "si1_gemm", t + 1);
         // self_interaction_1 of the next layer -> local rows of x[t+1] (ghost rows: caller's exchange)
-        if (node_linear(N, "si1", e->re_h, !h_rows, N.n_lx, e->h.as<float>(), N.dim_x, N.x_off, N.x_muls, e->x[t + 1].as<float>(), N.dim_x, N.x_off, N.x_muls, N.n_lx, si1, Nl, false, st)) return 1;
+        if (node_linear(e, si1, e->re_h, !h_rows, e->h.as<float>(), e->x[t + 1].as<float>(), false, st)) return 1;
       }
       if (stage != S7B_STAGE_FWD_LAYER) return 0;
     }
@@ -1391,29 +1448,24 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
     case S7B_STAGE_FWD_LAYER_SC: {
       if (t < 0 || t >= T) return fail("layer out of range");
       if (Nl == 0 || t + 1 >= T) return 0;
-      const LayerCfg& N = e->layers[t + 1];
-      const float* sc = lparam(e, t + 1, "sc");
-      const float* scs = lparam(e, t + 1, "sc_species");
-      if (!scs && require(sc, "sc")) return 1;
+      const NodeLinear& sc = e->layer_params[t + 1].sc;
+      if (require(sc.w.p, "sc")) return 1;
       ProfScope ps(e->prof, st, "sc_gemm", t + 1);
       // self_connection_intro of the next layer -> initial value of g[t+1]; independent of the ghost
       // exchange of x[t+1], so multi-GPU callers overlap the two
-      S7B_CUDA_CHECK(cudaMemsetAsync(e->g[t + 1].p, 0, (size_t)Nl * N.dim_g * sizeof(float), st));
-      const int n_sc = std::min(N.n_lx, N.n_lg);
-      if (scs) return launch_species_linear(e->h.as<float>(), N.dim_x, N.x_off, N.x_muls, e->g[t + 1].as<float>(), N.dim_g, N.g_off, N.g_muls,
-                                            n_sc, scs, e->desc.num_species, e->seg_perm.as<int>(), e->seg.as<int>(), Nl, false, st);
-      if (node_linear(N, "sc", e->re_h, false, N.n_lx, e->h.as<float>(), N.dim_x, N.x_off, N.x_muls, e->g[t + 1].as<float>(), N.dim_g, N.g_off, N.g_muls, n_sc, sc, Nl, false, st)) return 1;
-      return 0;
+      S7B_CUDA_CHECK(cudaMemsetAsync(e->g[t + 1].p, 0, (size_t)Nl * e->layers[t + 1].g.dim * sizeof(float), st));
+      return node_linear(e, sc, e->re_h, false, e->h.as<float>(), e->g[t + 1].as<float>(), false, st);
     }
     case S7B_STAGE_FWD_END: {
       const LayerCfg& L = e->layers[T - 1];
-      const float *wr = gparam(e, "readout"), *scale = gparam(e, "scale"), *shift = gparam(e, "shift");
+      const GlobalParams& G = e->global_params;
+      const float *wr = G.readout.as<float>(), *scale = G.scale.as<float>(), *shift = G.shift.as<float>();
       if (require(wr, "readout") || require(scale, "scale") || require(shift, "shift")) return 1;
       S7B_CUDA_CHECK(cudaMemsetAsync(e->energy.p, 0, sizeof(double), st));
       if (Nl > 0) {
         const int blk = 256;
         ProfScope ps(e->prof, st, "readout");
-        readout_kernel<<<(Nl * 32 + blk - 1) / blk, blk, 0, st>>>(e->h.as<float>(), wr, gparam(e, "readout_lo"), scale, shift, e->d_species, Nl, L.dim_h, e->atomic_energy.as<float>(), e->atomic_energy64.as<double>(), e->energy.as<double>(), e->dh.as<float>());
+        readout_kernel<<<(Nl * 32 + blk - 1) / blk, blk, 0, st>>>(e->h.as<float>(), wr, G.readout_lo.as<float>(), scale, shift, e->d_species, Nl, L.dim_h, e->atomic_energy.as<float>(), e->atomic_energy64.as<double>(), e->energy.as<double>(), e->dh.as<float>());
         S7B_LAUNCH_CHECK();
       }
       return 0;
@@ -1423,36 +1475,36 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
     case S7B_STAGE_BWD_LAYER_A2: {
       if (t < 0 || t >= T) return fail("layer out of range");
       const LayerCfg& L = e->layers[t];
+      const LayerParams& P = e->layer_params[t];
       const bool head = stage != S7B_STAGE_BWD_LAYER_A2, tail = stage != S7B_STAGE_BWD_LAYER_A1;
-      if (head && t > 0 && Nn > 0) S7B_CUDA_CHECK(cudaMemsetAsync(e->dx.p, 0, (size_t)Nn * L.dim_x * sizeof(float), st));
+      if (head && t > 0 && Nn > 0) S7B_CUDA_CHECK(cudaMemsetAsync(e->dx.p, 0, (size_t)Nn * L.x.dim * sizeof(float), st));
       if (Nl == 0) return 0;
       if (head) {
-        const bool dg_rows = g_opt_gate_bwd_rows && g_opt_tc_gemm && L.tcw.count("si2T") && L.tcw.at("si2T") && L.tcw.at("si2T")->ok && L.n_lg * L.n_lg <= 16;
+        const bool dg_rows = g_opt_gate_bwd_rows && on_tc(P.si2T) && L.g.n_l * L.g.n_l <= 16;
         {
           ProfScope ps(e->prof, st, "gate_bwd", t);
           if (dg_rows) {      // ... and the row exponents of dg for si2^T / sc^T
-            e->re_dg.rows_per_node = L.n_lg * L.n_lg;
+            e->re_dg.rows_per_node = L.g.n_l * L.g.n_l;
             e->re_dg.bits = true;
             S7B_CUDA_CHECK(cudaMemsetAsync(e->re_dg.buf.p, 0, (size_t)Nl * e->re_dg.rows_per_node * sizeof(int), st));
-            gate_bwd_rows_kernel<<<grid1d((size_t)Nl * L.dim_g, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), e->dh.as<float>(), e->dg.as<float>(), Nl, e->re_dg.buf.as<unsigned int>(), e->re_dg.rows_per_node);
+            gate_bwd_rows_kernel<<<grid1d((size_t)Nl * L.g.dim, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), e->dh.as<float>(), e->dg.as<float>(), Nl, e->re_dg.buf.as<unsigned int>(), e->re_dg.rows_per_node);
           } else {
-            gate_bwd_kernel<<<grid1d((size_t)Nl * L.dim_g, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), e->dh.as<float>(), e->dg.as<float>(), Nl);
+            gate_bwd_kernel<<<grid1d((size_t)Nl * L.g.dim, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), e->dh.as<float>(), e->dg.as<float>(), Nl);
           }
           S7B_LAUNCH_CHECK();
         }
-        const float* si2T = lparam(e, t, "si2T");
-        if (require(si2T, "si2T")) return 1;
+        if (require(P.si2T.w.p, "si2T")) return 1;
         // d(mid) = dg * si2^T
         ProfScope ps(e->prof, st, "si2T_gemm", t);
-        if (node_linear(L, "si2T", e->re_dg, !dg_rows, L.n_lg, e->dg.as<float>(), L.dim_g, L.g_off, L.g_muls, e->mid.as<float>(), L.dim_mid, L.mid_off, L.mid_K, L.n_lg, si2T, Nl, false, st)) return 1;
+        if (node_linear(e, P.si2T, e->re_dg, !dg_rows, e->dg.as<float>(), e->mid.as<float>(), false, st)) return 1;
       }
       if (E > 0) {
         ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
         if (stage == S7B_STAGE_BWD_LAYER_A1) ca.n_begin = e->n_interior;     // boundary atoms first: they own the ghost rows of dx
         if (stage == S7B_STAGE_BWD_LAYER_A2) ca.n_dst = e->n_interior;
-        const bool par = e->concurrent && g_opt_concurrent && !e->prof.enabled && L.n_lx > 1;
+        const bool par = e->concurrent && g_opt_concurrent && !e->prof.enabled && L.x.n_l > 1;
         if (par) S7B_CUDA_CHECK(cudaEventRecord(e->ev_fork, st));
-        for (int l1 = 0; l1 < L.n_lx; ++l1) {
+        for (int l1 = 0; l1 < L.x.n_l; ++l1) {
           float* dY = e->dY_acc.as<float>() + (size_t)l1 * Ecap * e->ny_stride;
           float* dEdr = e->dEdr_acc.as<float>() + (size_t)l1 * Ecap;
           cudaStream_t s1 = (par && l1 > 0) ? e->side[l1] : st;
@@ -1466,7 +1518,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         }
         if (!table && tail) {
           // radial MLP backward: dw -> demb (accumulated over layers)
-          const float *w0T = lparam(e, t, "mlp0T"), *w1T = lparam(e, t, "mlp1T"), *w2T = lparam(e, t, "mlp2T");
+          const float *w0T = P.mlpT[0].as<float>(), *w1T = P.mlpT[1].as<float>(), *w2T = P.mlpT[2].as<float>();
           if (require(w0T, "mlp0T") || require(w1T, "mlp1T") || require(w2T, "mlp2T")) return 1;
           const int nb = e->desc.n_basis, h0 = e->desc.radial_hidden[0], h1 = e->desc.radial_hidden[1];
           ProfScope ps(e->prof, st, "radial_mlp_bwd", t);
@@ -1481,23 +1533,18 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
     case S7B_STAGE_BWD_LAYER_B1:
     case S7B_STAGE_BWD_LAYER_B2: {
       if (t <= 0 || t >= T) return fail("BWD_LAYER_B needs 1 <= layer < n_layers");
-      const LayerCfg& L = e->layers[t];
+      const LayerParams& P = e->layer_params[t];
       if (Nl == 0) return 0;
-      const float *si1T = lparam(e, t, "si1T"), *scT = lparam(e, t, "scT"), *scTs = lparam(e, t, "scT_species");
-      if (require(si1T, "si1T") || (!scTs && require(scT, "scT"))) return 1;
+      if (require(P.si1T.w.p, "si1T") || require(P.scT.w.p, "scT")) return 1;
       // dE/dh(t) = dg(t) * sc^T + dx(t) * si1^T     (h(t) = gate output of layer t-1).  B1 (the self-
       // connection term) does not need the reverse ghost exchange of dx and can overlap it; B2 adds the rest.
       ProfScope ps(e->prof, st, "si1T_scT_gemm", t);
       if (stage != S7B_STAGE_BWD_LAYER_B2) {
-        const int n_sc = std::min(L.n_lx, L.n_lg);
-        S7B_CUDA_CHECK(cudaMemsetAsync(e->dh.p, 0, (size_t)Nl * L.dim_x * sizeof(float), st));
-        if (scTs) {
-          if (launch_species_linear(e->dg.as<float>(), L.dim_g, L.g_off, L.g_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, n_sc, scTs,
-                                    e->desc.num_species, e->seg_perm.as<int>(), e->seg.as<int>(), Nl, false, st)) return 1;
-        } else if (node_linear(L, "scT", e->re_dg, false, L.n_lg, e->dg.as<float>(), L.dim_g, L.g_off, L.g_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, n_sc, scT, Nl, false, st)) return 1;
+        S7B_CUDA_CHECK(cudaMemsetAsync(e->dh.p, 0, (size_t)Nl * e->layers[t].x.dim * sizeof(float), st));
+        if (node_linear(e, P.scT, e->re_dg, false, e->dg.as<float>(), e->dh.as<float>(), false, st)) return 1;
       }
       if (stage != S7B_STAGE_BWD_LAYER_B1) {
-        if (node_linear(L, "si1T", e->re_dx, true, L.n_lx, e->dx.as<float>(), L.dim_x, L.x_off, L.x_muls, e->dh.as<float>(), L.dim_x, L.x_off, L.x_muls, L.n_lx, si1T, Nl, true, st)) return 1;
+        if (node_linear(e, P.si1T, e->re_dx, true, e->dx.as<float>(), e->dh.as<float>(), true, st)) return 1;
       }
       return 0;
     }
@@ -1510,7 +1557,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         const int blk = 256;
         const int grd = (int)((Ecap + blk - 1) / blk);
         int max_lx = 0;
-        for (auto& L : e->layers) max_lx = std::max(max_lx, L.n_lx);
+        for (auto& L : e->layers) max_lx = std::max(max_lx, L.x.n_l);
         const float* dEdr = table ? e->dEdr_acc.as<float>() : nullptr;
         const float* demb = table ? nullptr : e->demb_acc.as<float>();
         ProfScope ps(e->prof, st, "edge_bwd_force_scatter");
@@ -1693,14 +1740,14 @@ void* s7b_engine_buffer(S7bEngine* e, const char* name, int layer, size_t* numel
   size_t n = 0;
   void* p = nullptr;
   auto in_range = [&](int t) { return t >= 0 && t < T; };
-  if (nm == "x" && in_range(layer)) { p = e->x[layer].p; n = (size_t)e->n_nodes * e->layers[layer].dim_x; }
-  else if (nm == "gate_in" && in_range(layer)) { p = e->g[layer].p; n = (size_t)e->n_local * e->layers[layer].dim_g; }
+  if (nm == "x" && in_range(layer)) { p = e->x[layer].p; n = (size_t)e->n_nodes * e->layers[layer].x.dim; }
+  else if (nm == "gate_in" && in_range(layer)) { p = e->g[layer].p; n = (size_t)e->n_local * e->layers[layer].g.dim; }
   else if (nm == "weight" && in_range(layer)) { p = e->wbuf[layer].p; n = (size_t)e->n_edges * e->layers[layer].W; }
-  else if (nm == "dx" && in_range(layer)) { p = e->dx.p; n = (size_t)e->n_nodes * e->layers[layer].dim_x; }
-  else if (nm == "dg" && in_range(layer)) { p = e->dg.p; n = (size_t)e->n_local * e->layers[layer].dim_g; }
-  else if (nm == "mid" && in_range(layer)) { p = e->mid.p; n = (size_t)e->n_local * e->layers[layer].dim_mid; }
+  else if (nm == "dx" && in_range(layer)) { p = e->dx.p; n = (size_t)e->n_nodes * e->layers[layer].x.dim; }
+  else if (nm == "dg" && in_range(layer)) { p = e->dg.p; n = (size_t)e->n_local * e->layers[layer].g.dim; }
+  else if (nm == "mid" && in_range(layer)) { p = e->mid.p; n = (size_t)e->n_local * e->layers[layer].mid.dim; }
   else if (nm == "h" && in_range(layer)) { p = e->h.p; n = (size_t)e->n_local * e->layers[layer].dim_h; }
-  else if (nm == "dh" && in_range(layer)) { p = e->dh.p; n = (size_t)e->n_local * e->layers[layer].dim_x; }
+  else if (nm == "dh" && in_range(layer)) { p = e->dh.p; n = (size_t)e->n_local * e->layers[layer].x.dim; }
   else if (nm == "energy") { p = e->energy.p; n = 1; }
   else if (nm == "virial") { p = e->virial.p; n = 6; }
   else if (nm == "atomic_energy") { p = e->atomic_energy.p; n = (size_t)e->n_local; }
@@ -2103,8 +2150,8 @@ void s7b_conv_plan_destroy(S7bConvPlan* p) { delete p; }
 int s7b_conv_plan_dims(const S7bConvPlan* p, int32_t* dim_x, int32_t* dim_mid, int32_t* weight_numel,
                        int32_t* n_sh) {
   if (!p) return fail("null plan");
-  if (dim_x) *dim_x = p->cfg.dim_x;
-  if (dim_mid) *dim_mid = p->cfg.dim_mid;
+  if (dim_x) *dim_x = p->cfg.x.dim;
+  if (dim_mid) *dim_mid = p->cfg.mid.dim;
   if (weight_numel) *weight_numel = p->cfg.W;
   if (n_sh) *n_sh = (p->lmax_filter + 1) * (p->lmax_filter + 1);
   return 0;
@@ -2150,7 +2197,7 @@ int s7b_conv_forward(const S7bConvPlan* p, const float* x, const float* sh, cons
   const LayerCfg& L = p->cfg;
   if (n_dst <= 0) return 0;
   if (n_edges == 0) {   // reference convolution.py:265-268: no launch, zeros out
-    S7B_CUDA_CHECK(cudaMemsetAsync(out, 0, (size_t)n_dst * L.dim_mid * sizeof(float), st));
+    S7B_CUDA_CHECK(cudaMemsetAsync(out, 0, (size_t)n_dst * L.mid.dim * sizeof(float), st));
     return 0;
   }
   const int n_sh = (p->lmax_filter + 1) * (p->lmax_filter + 1);
@@ -2168,8 +2215,8 @@ int s7b_conv_forward(const S7bConvPlan* p, const float* x, const float* sh, cons
   a.x = x;
   a.w = weight;
   a.n_dst = n_dst;
-  a.dim_x = L.dim_x;
-  a.dim_mid = L.dim_mid;
+  a.dim_x = L.x.dim;
+  a.dim_mid = L.mid.dim;
   a.w_numel = L.W;
   a.inv_h = 1.0f;
   int rc = conv_forward(L, p->lmax_filter, false, a, out, st);
@@ -2186,14 +2233,14 @@ int s7b_conv_backward(const S7bConvPlan* p, const float* x, const float* sh, con
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const LayerCfg& L = p->cfg;
   const int n_sh = (p->lmax_filter + 1) * (p->lmax_filter + 1);
-  if (n_nodes > 0) S7B_CUDA_CHECK(cudaMemsetAsync(grad_x, 0, (size_t)n_nodes * L.dim_x * sizeof(float), st));
+  if (n_nodes > 0) S7B_CUDA_CHECK(cudaMemsetAsync(grad_x, 0, (size_t)n_nodes * L.x.dim * sizeof(float), st));
   if (n_edges == 0 || n_dst <= 0) return 0;
   int4* rec = nullptr;
   float *Ypk = nullptr, *dY = nullptr;
   S7B_CUDA_CHECK(cudaMallocAsync((void**)&rec, (size_t)n_edges * sizeof(int4), st));
   S7B_CUDA_CHECK(cudaMallocAsync((void**)&Ypk, (size_t)n_edges * p->ny_stride * sizeof(float), st));
-  S7B_CUDA_CHECK(cudaMallocAsync((void**)&dY, (size_t)L.n_lx * n_edges * p->ny_stride * sizeof(float), st));
-  S7B_CUDA_CHECK(cudaMemsetAsync(dY, 0, (size_t)L.n_lx * n_edges * p->ny_stride * sizeof(float), st));
+  S7B_CUDA_CHECK(cudaMallocAsync((void**)&dY, (size_t)L.x.n_l * n_edges * p->ny_stride * sizeof(float), st));
+  S7B_CUDA_CHECK(cudaMemsetAsync(dY, 0, (size_t)L.x.n_l * n_edges * p->ny_stride * sizeof(float), st));
   conv_pack_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(src, sh, n_sh, p->ny_stride, n_edges, rec, Ypk);
   S7B_LAUNCH_CHECK();
   ConvArgs a;
@@ -2204,16 +2251,16 @@ int s7b_conv_backward(const S7bConvPlan* p, const float* x, const float* sh, con
   a.x = x;
   a.w = weight;
   a.n_dst = n_dst;
-  a.dim_x = L.dim_x;
-  a.dim_mid = L.dim_mid;
+  a.dim_x = L.x.dim;
+  a.dim_mid = L.mid.dim;
   a.w_numel = L.W;
   a.inv_h = 1.0f;
   int rc = 0;
-  for (int l1 = 0; l1 < L.n_lx && !rc; ++l1)
+  for (int l1 = 0; l1 < L.x.n_l && !rc; ++l1)
     rc = launch_conv_bwd(l1, p->lmax_filter, L.lmax_out, false, true, a, L.roles[l1], grad_out, grad_x,
                          dY + (size_t)l1 * n_edges * p->ny_stride, nullptr, grad_weight, st);
   if (!rc) {
-    conv_unpack_grad_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(dY, L.n_lx, n_sh, p->ny_stride, n_edges, grad_sh);
+    conv_unpack_grad_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(dY, L.x.n_l, n_sh, p->ny_stride, n_edges, grad_sh);
     ++g_launches;
     if (cudaGetLastError() != cudaSuccess) rc = fail("conv_unpack_grad_kernel launch failed");
   }
