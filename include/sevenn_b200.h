@@ -190,7 +190,9 @@ S7B_API int s7b_engine_compute(S7bEngine* eng, void* stream);
  * "x" (layer t input after self_interaction_1, [n_nodes, dim_x(t)]), "dx", "gate_in", "mid",
  * "h", "energy" (double[1]), "atomic_energy" [n_local], "atomic_energy_f64" (double[n_local], the same
  * per-atom energies before their rounding to float), "forces" [n_nodes,3], "edge_force" [E,3],
- * "virial" (double[6], = -sum r (x) f), "edge_Y", "edge_rec".  *numel receives the element count. */
+ * "virial" (double[6], = -sum r (x) f), "edge_Y", "edge_rec".  "dY_acc" [E, ny_stride] / "dEdr_acc" [E]: the
+ * backward's per-edge sums of the l1 role `layer` (0 <= layer < the largest n_l of x; -1 = role 0); NULL for
+ * any other layer.  *numel receives the element count (0 with NULL). */
 S7B_API void* s7b_engine_buffer(S7bEngine* eng, const char* name, int layer, size_t* numel);
 
 /* Host-buffer entry point, the analogue of PairE3GNN::compute (pair_e3gnn.cpp:74-289):

@@ -1765,8 +1765,19 @@ void* s7b_engine_buffer(S7bEngine* e, const char* name, int layer, size_t* numel
   else if (nm == "nl_vec") { p = e->hs_vec.p; n = (size_t)e->nl_n_edges * 3; }
   else if (nm == "edge_len") { p = e->rlen.p; n = (size_t)e->n_edges; }
   else if (nm == "edge_emb") { p = e->emb.p; n = (size_t)e->n_edges * e->desc.n_basis; }
-  else if (nm == "dY_acc") { p = e->dY_acc.p; n = (size_t)e->n_edges * e->ny_stride; }
-  else if (nm == "dEdr_acc") { p = e->dEdr_acc.p; n = (size_t)e->n_edges; }
+  else if (nm == "dY_acc" || nm == "dEdr_acc") {
+    // the backward's per-edge sums, one part per l1 role (E_cap rows apart); layer = the part, -1 = part 0
+    int max_lx = 0;
+    for (auto& L : e->layers) max_lx = std::max(max_lx, L.x.n_l);
+    const int part = layer < 0 ? 0 : layer;
+    const bool dY = nm == "dY_acc";
+    float* base = dY ? e->dY_acc.as<float>() : e->dEdr_acc.as<float>();
+    if (base && layer >= -1 && part < max_lx) {
+      const size_t row = dY ? (size_t)e->ny_stride : 1;
+      p = base + (size_t)part * e->E_cap * row;
+      n = (size_t)e->n_edges * row;
+    }
+  }
   if (numel) *numel = n;
   return p;
 }

@@ -268,6 +268,22 @@ def pack_table_pairs(tab: np.ndarray):
     return t01, np.ascontiguousarray(t23).view(np.float32)
 
 
+def close_table_at_cutoff(t01: np.ndarray, t23: np.ndarray) -> None:
+    """Make the packed cubic table (``pack_table_pairs``) give w = 0 and dw/dr = 0 exactly at the end of its last
+    interval, in place.  Both envelopes take w and dw/dr to 0 at the cutoff, and every edge at or beyond the cutoff
+    reads that point (interval K - 1, t = 1, edge_fwd_kernel), but a2 and a3 are rounded to fp16, so the kernels'
+    fp32 Horner sums there, a1 + (2 a2 + 3 a3) and a0 + (a1 + (a2 + a3)), leave ~1e-11 of w and ~1e-8 of dw/dr: such
+    an edge would still add to dE/dY and dE/dr.  a1 and a0 of the last interval absorb the rounding (they change by
+    that much): a1 = -fl(3 a3 + 2 a2) (the kernels' FMA), a0 = -fl(fl(a3 + a2) + a1).  The sums of two fp16 values
+    and of their small multiples are exact in float64, so each float32() below is the kernel's single rounding."""
+    a2, a3 = (t23.view(np.float16)[-1, :, c:c + 2].astype(np.float64) for c in (0, 2))
+    a1 = -(3.0 * a3 + 2.0 * a2).astype(np.float32)
+    s = (a3 + a2).astype(np.float32)
+    a0 = -(s.astype(np.float64) + a1.astype(np.float64)).astype(np.float32)
+    t01[-1, :, 2:4] = a1
+    t01[-1, :, 0:2] = a0
+
+
 def default_table_knots(spec: ModelSpec) -> int:
     """Number of table intervals over [0, cutoff].  The XPLOR envelope is only C1 at its switching radius r_on (the
     second derivative jumps), and a cubic Hermite interval that spans r_on loses an order of magnitude in dw/dr
@@ -343,6 +359,7 @@ def prepare_params(spec: ModelSpec, arrays: Dict[str, np.ndarray], radial: str, 
         out[('si2T', t)] = np.concatenate([b.T.ravel() for b in si2])
         if radial == 'table':
             out[('table', t)], out[('table23', t)] = pack_table_pairs(radial_table(spec, arrays, t, knots))
+            close_table_at_cutoff(out[('table', t)], out[('table23', t)])
             out[('table_fwd', t)] = radial_value_table(spec, arrays, t, forward_table_knots(knots))
         else:
             for j in range(len(spec.radial_hidden) + 1):

@@ -12,6 +12,8 @@ realistic, so that energies are O(eV/atom) and absolute tolerances mean what the
   B   64x0e+32x1e                        1 / 1                  4       groups (1, 1), (1, 0)
   C   128x0e+64x1e+32x2e                 3 / 2                  3       group (3, 2) at SevenNet-0 widths
   D   256x0e+96x1e+64x2e+32x3e           3 / 3                  2       split backward: 256 (NV = 2) and 96 (16 lanes)
+
+``layered`` describes any other architecture by the irreps of every layer (tests/test_conv_table_gpu.py).
 """
 from __future__ import annotations
 
@@ -28,23 +30,40 @@ ARCHS = {
 }
 
 
-def irreps_per_layer(arch: str):
-    a = ARCHS[arch]
+def layered(name: str, lmax_edge: int, lmax_node: int, irreps) -> dict:
+    """An architecture of any lmax_edge / lmax_node with the irreps of every layer given (``irreps[t]``: the input
+    of layer t, the last entry the output of the last layer), for ``reference_checkpoint`` in place of an ARCHS id"""
+    return dict(name=name, lmax_edge=lmax_edge, lmax_node=lmax_node, layers=len(irreps) - 1, irreps=list(irreps))
+
+
+def _arch(arch):
+    return ARCHS[arch] if isinstance(arch, str) else arch
+
+
+def _name(arch):
+    return arch if isinstance(arch, str) else arch['name']
+
+
+def irreps_per_layer(arch):
+    a = _arch(arch)
+    if 'irreps' in a:
+        return list(a['irreps'])
     s0 = a['mid'].split('+')[0]
     return [s0] + [a['mid']] * (a['layers'] - 1) + [s0]
 
 
-def reference_checkpoint(arch: str, seed: int = 0, parity: bool = False) -> dict:
-    """{'config', 'model_state_dict'} of a reference checkpoint (torch tensors) for architecture ``arch``"""
+def reference_checkpoint(arch, seed: int = 0, parity: bool = False) -> dict:
+    """{'config', 'model_state_dict'} of a reference checkpoint (torch tensors) for architecture ``arch``: an ARCHS
+    id or a ``layered`` description"""
     import torch
     from sevenn_b200.cg import wigner_3j
     from sevenn_b200.checkpoint import random_weights
     from sevenn_b200.spec import build_spec, parse_even_irreps
 
-    a = ARCHS[arch]
+    a = _arch(arch)
     irreps = irreps_per_layer(arch)
     cutoff = 5.0
-    meta = dict(name=f'synthetic_{arch}', cutoff=cutoff, cutoff_fn='poly_cut', cutoff_on=0.0, poly_p=6, n_basis=8,
+    meta = dict(name=f'synthetic_{_name(arch)}', cutoff=cutoff, cutoff_fn='poly_cut', cutoff_on=0.0, poly_p=6, n_basis=8,
                 lmax_filter=a['lmax_edge'], num_species=len(NUMBERS),
                 type_map={str(z): i for i, z in enumerate(NUMBERS)}, chemical_species=ELEMENTS,
                 radial_hidden=[64, 64], irreps_per_layer=irreps,
@@ -86,13 +105,13 @@ def reference_checkpoint(arch: str, seed: int = 0, parity: bool = False) -> dict
     return {'config': config, 'model_state_dict': sd}
 
 
-def write_checkpoint(path, arch: str, seed: int = 0, parity: bool = False) -> str:
+def write_checkpoint(path, arch, seed: int = 0, parity: bool = False) -> str:
     import torch
     torch.save(reference_checkpoint(arch, seed, parity), str(path))
     return str(path)
 
 
-def convert(path, arch: str):
+def convert(path, arch):
     """(meta, arrays) of a checkpoint written by write_checkpoint, through the reference-checkpoint converter"""
     from sevenn_b200.checkpoint import convert_reference_checkpoint
-    return convert_reference_checkpoint(str(path), f'synthetic_{arch}')
+    return convert_reference_checkpoint(str(path), f'synthetic_{_name(arch)}')

@@ -108,6 +108,33 @@ def test_table_matches_radial_mlp(name):
         assert ew < W_BOUND and edw < bound, (name, knots, t, ew, edw, r)
 
 
+@pytest.mark.parametrize('name', MODELS)
+def test_table_is_exactly_zero_at_the_cutoff(name):
+    """Edges at or beyond the cutoff read the end of the last interval (t = 1): the kernels' fp32 sums there,
+    w = fma(1, fma(1, fma(1, a3, a2), a1), a0) and dw/dr h = fma(1, fma(3, a3, 2 a2), a1), must be exactly 0 with the
+    fp16 a2, a3 the device holds (regression: 1e-11 of w and 1e-8 of dw/dr were left), and closing the interval
+    moves a0 and a1 by no more than that rounding"""
+    from sevenn_b200.engine import default_table_knots, pack_table_pairs, prepare_params, radial_table
+    from sevenn_b200.spec import build_spec
+    meta, arrays = _model(name)
+    spec = build_spec(meta)
+    knots = default_table_knots(spec)
+    p = prepare_params(spec, arrays, 'table', knots)
+    for t in range(spec.n_layers):
+        t01, t23 = p[('table', t)][-1], p[('table23', t)].view(np.float16)[-1].astype(np.float32)
+        a0, a1, a2, a3 = t01[:, 0:2], t01[:, 2:4], t23[:, 0:2], t23[:, 2:4]
+        f32 = lambda v: np.asarray(v, dtype=np.float64).astype(np.float32)
+        w = (((a3 + a2) + a1) + a0)                          # fp32 adds: fma(1, x, y) rounds x + y once
+        dw = f32(3.0 * a3.astype(np.float64) + 2.0 * a2.astype(np.float64)) + a1
+        assert np.all(w == 0) and np.all(dw == 0), (name, t, np.abs(w).max(), np.abs(dw).max())
+        # fp16 rounds a2 and a3 by at most 2^-11 of their size, or half the subnormal spacing 2^-25
+        raw, _ = pack_table_pairs(radial_table(spec, arrays, t, knots))
+        e16 = 2.0 ** -25 + 2.0 ** -11 * (np.abs(a2) + np.abs(a3))
+        d = np.abs(raw[-1] - p[('table', t)][-1])
+        assert np.all(d <= 8 * np.concatenate([e16, e16], 1) + 2.0 ** -22 * np.abs(raw[-1])), (name, t, d.max())
+        assert np.array_equal(raw[:-1], p[('table', t)][:-1])
+
+
 @pytest.mark.parametrize('cid', ['R1', 'R5'])
 def test_table_check_fails_with_r_on_between_knots(cid):
     """negative control: on the 2000-interval grid r_on of R1 (6.0 / 5.5) and R5 (5.3 / 4.8) is not a knot, and the
