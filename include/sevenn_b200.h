@@ -11,7 +11,7 @@
  *       sevenn/nn/convolution.py:243-247,270-276 (call contract)
  *       sevenn/nn/flash_helper.py:33-48, sevenn/nn/oeq_helper.py:30-70 (existing adapters)
  *       sevenn/pair_e3gnn/pair_e3gnn_oeq_autograd.cpp:23-27,64-133 (C++ fwd/bwd op signatures)
- *     -> s7b_conv_plan_create / s7b_conv_forward / s7b_conv_backward
+ *     -> s7b_conv_plan_create / s7b_conv_forward / s7b_conv_backward / s7b_conv_double_backward
  *   - the model forward + autograd force path executed per MD step by
  *       sevenn/calculator.py:219-233 (SevenNetCalculator.calculate)
  *       sevenn/pair_e3gnn/pair_e3gnn.cpp:74-289 (PairE3GNN::compute: edges in, E/F/virial out)
@@ -304,6 +304,20 @@ S7B_API int s7b_conv_backward(const S7bConvPlan* plan, const float* x, const flo
                       const int32_t* rowptr, const int32_t* src, int32_t n_nodes, int32_t n_dst,
                       int64_t n_edges, const float* grad_out, float* grad_x, float* grad_sh,
                       float* grad_weight, void* stream);
+/* Second order: the backward of s7b_conv_backward.  Given its inputs (x, sh, weight, grad_out = g) and the incoming
+ * gradients of its outputs, tan_x [n_nodes, dim_x], tan_sh [E, n_sh] (column 0 is ignored: Y_0 is constant) and
+ * tan_weight [E, W], any of them NULL (zero: its terms are skipped), writes (all overwritten)
+ *   grad_grad_out [n_dst, dim_mid] = forward with one operand replaced by its tangent, summed over the three
+ *   grad_x        [n_nodes, dim_x] = d_x of the tan_sh and tan_weight terms, contracted with g
+ *   grad_sh       [E, n_sh]        = d_sh of the tan_x and tan_weight terms, contracted with g (column 0 is 0)
+ *   grad_weight   [E, W]           = d_weight of the tan_x and tan_sh terms, contracted with g
+ * in two kernels per l1 role of x (conv_jvp_kernel, conv_bwd_tangent_kernel).  E == 0, or no tangent, zero-fills
+ * the outputs without a launch.                                                                               */
+S7B_API int s7b_conv_double_backward(const S7bConvPlan* plan, const float* x, const float* sh, const float* weight,
+                             const int32_t* rowptr, const int32_t* src, int32_t n_nodes, int32_t n_dst,
+                             int64_t n_edges, const float* grad_out, const float* tan_x, const float* tan_sh,
+                             const float* tan_weight, float* grad_grad_out, float* grad_x, float* grad_sh,
+                             float* grad_weight, void* stream);
 
 /* ---- D3 dispersion correction (SURVEY 8(f).2) ------------------------------------------------------
  * Cell-list DFT-D3 (zero / Becke-Johnson damping) replacing the reference's all-pairs CUDA code

@@ -14,7 +14,9 @@ class (``sevenn/nn/convolution.py:145-284``; adapters ``sevenn/nn/flash_helper.p
 
 ``B200Convolution`` keeps that interface and runs the fused gather -> tensor product -> scatter
 kernels of ``libsevenn_b200.so`` (C ABI ``s7b_conv_forward`` / ``s7b_conv_backward``), with a
-hand-written backward instead of autograd through e3nn.  Layout conversion (mul_ir <-> the
+hand-written backward instead of autograd through e3nn.  The operator is twice differentiable: under
+``create_graph=True`` (forces inside a training loss, Hessian-vector products) the backward is itself
+differentiated by ``s7b_conv_double_backward``; a third derivative raises.  Layout conversion (mul_ir <-> the
 engine's component-major layout) and the sort of edges by destination are torch index ops.
 ``edge_filter[:, 0]`` must be the constant Y_0 = 1 that ``SphericalEncoding`` produces
 (component normalisation); its gradient is returned as zero.
@@ -54,6 +56,7 @@ def is_b200_available() -> bool:
 
 def _make_module_class():
     import torch
+    from torch.autograd.function import once_differentiable
 
     class _ConvFn(torch.autograd.Function):
         @staticmethod
@@ -63,6 +66,7 @@ def _make_module_class():
             E, n_nodes = int(edge_src.shape[0]), int(x.shape[0])
             dst, src = edge_dst.long(), edge_src.long()
             perm = None
+            inputs = (x, edge_filter, weight)
             if E > 1 and bool((dst[1:] < dst[:-1]).any()):
                 perm = torch.argsort(dst, stable=True)
                 dst, src = dst[perm], src[perm]
@@ -81,15 +85,26 @@ def _make_module_class():
                 check(lib.s7b_conv_forward(mod._plan, x_cm.data_ptr(), sh.data_ptr(), w.data_ptr(),
                                            rowptr.data_ptr(), src32.data_ptr(), n_nodes, n_nodes, E,
                                            out_cm.data_ptr(), st))
-            ctx.save_for_backward(x_cm, sh, w, rowptr, src32)
+            # the inputs as well: the backward is differentiated as a function of them (second order)
+            ctx.save_for_backward(x_cm, sh, w, rowptr, src32, *inputs)
             ctx.perm, ctx.mod = perm, mod
             return out_cm.index_select(1, mod._perm_mid_inv)
 
         @staticmethod
         def backward(ctx, grad_out):
+            x_cm, sh, w, rowptr, src32, x, edge_filter, weight = ctx.saved_tensors
+            gx, gsh, gw = _ConvBwdFn.apply(grad_out, x, edge_filter, weight, x_cm, sh, w, rowptr, src32,
+                                           ctx.perm, ctx.mod)
+            return gx, gsh, gw, None, None, None
+
+    class _ConvBwdFn(torch.autograd.Function):
+        """The backward of _ConvFn as a function of (grad_out, x, edge_filter, weight), so that a graph built
+        with create_graph=True differentiates it once more (s7b_conv_double_backward).  x, edge_filter and
+        weight only tie the result to the graph; the kernels read their converted copies x_cm, sh and w."""
+
+        @staticmethod
+        def forward(ctx, grad_out, x, edge_filter, weight, x_cm, sh, w, rowptr, src32, perm, mod):
             lib = load_library()
-            x_cm, sh, w, rowptr, src32 = ctx.saved_tensors
-            mod, perm = ctx.mod, ctx.perm
             dev = x_cm.device
             n_nodes, E = int(x_cm.shape[0]), int(src32.shape[0])
             g_cm = grad_out.float().index_select(1, mod._perm_mid).contiguous()
@@ -105,7 +120,44 @@ def _make_module_class():
                 inv = torch.empty_like(perm)
                 inv[perm] = torch.arange(E, device=dev)
                 gsh, gw = gsh[inv], gw[inv]
-            return gx.index_select(1, mod._perm_x_inv), gsh, gw, None, None, None
+            ctx.save_for_backward(x_cm, sh, w, rowptr, src32, g_cm)
+            ctx.perm, ctx.mod = perm, mod
+            ctx.set_materialize_grads(False)      # an absent incoming gradient skips its terms
+            return gx.index_select(1, mod._perm_x_inv), gsh, gw
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, tan_x, tan_sh, tan_w):
+            lib = load_library()
+            x_cm, sh, w, rowptr, src32, g_cm = ctx.saved_tensors
+            mod, perm = ctx.mod, ctx.perm
+            dev = x_cm.device
+            n_nodes, E = int(x_cm.shape[0]), int(src32.shape[0])
+
+            def edges_sorted(t):      # per-edge tangent -> the kernels' dst-sorted edge order, fp32
+                if t is None:
+                    return None
+                return (t if perm is None else t[perm]).float().contiguous()
+
+            tx = None if tan_x is None else tan_x.float().index_select(1, mod._perm_x).contiguous()
+            tsh, tw = edges_sorted(tan_sh), edges_sorted(tan_w)
+            ggo = torch.empty_like(g_cm)
+            gx = torch.empty_like(x_cm)
+            gsh = torch.empty_like(sh)
+            gw = torch.empty_like(w)
+            ptr = lambda t: None if t is None else t.data_ptr()
+            st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            with torch.cuda.device(dev):
+                check(lib.s7b_conv_double_backward(
+                    mod._plan, x_cm.data_ptr(), sh.data_ptr(), w.data_ptr(), rowptr.data_ptr(), src32.data_ptr(),
+                    n_nodes, n_nodes, E, g_cm.data_ptr(), ptr(tx), ptr(tsh), ptr(tw),
+                    ggo.data_ptr(), gx.data_ptr(), gsh.data_ptr(), gw.data_ptr(), st))
+            if perm is not None:
+                inv = torch.empty_like(perm)
+                inv[perm] = torch.arange(E, device=dev)
+                gsh, gw = gsh[inv], gw[inv]
+            return (ggo.index_select(1, mod._perm_mid_inv), gx.index_select(1, mod._perm_x_inv), gsh, gw,
+                    None, None, None, None, None, None, None)
 
     class B200Convolution(torch.nn.Module):
         """``convolution_cls``-compatible fused 'uvu' tensor product (see module docstring)."""

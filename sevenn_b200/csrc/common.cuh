@@ -65,6 +65,14 @@ struct ConvArgs {
   int ftab_knots;             // intervals of the value table over [0, cutoff]
 };
 
+// Tangents of the convolution backward's inputs x, Y and w (second order, conv_jvp_kernel / conv_bwd_tangent_kernel),
+// in the layouts of ConvArgs::x, ::Y and ::w.  A null pointer is a zero tangent.
+struct ConvTangents {
+  const float* x;
+  const float* Y;
+  const float* w;
+};
+
 }  // namespace s7b
 
 #define S7B_CUDA_CHECK(expr)                                                            \

@@ -6,7 +6,10 @@ namespace s7b {
 #define S7B_DECL_GROUP(LF, LO)                                                                      \
   int launch_conv_fwd_##LF##_##LO(int, bool, const ConvArgs&, const ConvRole&, float*, cudaStream_t); \
   int launch_conv_bwd_##LF##_##LO(int, bool, bool, const ConvArgs&, const ConvRole&, const float*,  \
-                                  float*, float*, float*, float*, cudaStream_t);
+                                  float*, float*, float*, float*, cudaStream_t);             \
+  int launch_conv_jvp_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const ConvTangents&, float*, cudaStream_t); \
+  int launch_conv_bwdt_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const ConvTangents&, const float*, \
+                                   float*, float*, float*, cudaStream_t);
 S7B_DECL_GROUP(1, 0) S7B_DECL_GROUP(1, 1) S7B_DECL_GROUP(1, 2) S7B_DECL_GROUP(1, 3)
 S7B_DECL_GROUP(2, 0) S7B_DECL_GROUP(2, 1) S7B_DECL_GROUP(2, 2) S7B_DECL_GROUP(2, 3)
 S7B_DECL_GROUP(3, 0) S7B_DECL_GROUP(3, 1) S7B_DECL_GROUP(3, 2) S7B_DECL_GROUP(3, 3)
@@ -31,17 +34,22 @@ S7B_DECL_GROUP(3, 0) S7B_DECL_GROUP(3, 1) S7B_DECL_GROUP(3, 2) S7B_DECL_GROUP(3,
 extern int64_t g_conv_launches;
 int64_t g_conv_launches = 0;
 
-int launch_conv_fwd(int l1, int lf, int lo, bool table, const ConvArgs& a, const ConvRole& role,
-                    float* out, cudaStream_t st) {
-  if (a.n_dst <= a.n_begin) return 0;      // empty centre range
-  int rc = 2;
-  if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(fwd, l1, table, a, role, out, st)
+// Return code of a group launch -> 0 (launched, counted, or nothing to launch) or 1 with the error set
+static int conv_status(int rc) {
   if (rc == kConvNoPath) return 0;
   if (rc == 2) { set_error(__FILE__, __LINE__, "no tensor-product kind compiled for this (lmax_filter, lmax_out)"); return 1; }
   if (rc == kConvWrongMul) { set_error(__FILE__, __LINE__, "convolution multiplicities must be positive multiples of 32"); return 1; }
   if (rc) { set_error(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError())); return 1; }
   ++g_conv_launches;
   return 0;
+}
+
+int launch_conv_fwd(int l1, int lf, int lo, bool table, const ConvArgs& a, const ConvRole& role,
+                    float* out, cudaStream_t st) {
+  if (a.n_dst <= a.n_begin) return 0;      // empty centre range
+  int rc = 2;
+  if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(fwd, l1, table, a, role, out, st)
+  return conv_status(rc);
 }
 
 int launch_conv_bwd(int l1, int lf, int lo, bool table, bool need_dx, const ConvArgs& a,
@@ -51,12 +59,23 @@ int launch_conv_bwd(int l1, int lf, int lo, bool table, bool need_dx, const Conv
   int rc = 2;
   if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3)
     S7B_GROUP_SWITCH(bwd, l1, table, need_dx, a, role, gout, dx, dY_acc, dEdr_acc, dw, st)
-  if (rc == kConvNoPath) return 0;
-  if (rc == 2) { set_error(__FILE__, __LINE__, "no tensor-product kind compiled for this (lmax_filter, lmax_out)"); return 1; }
-  if (rc == kConvWrongMul) { set_error(__FILE__, __LINE__, "convolution multiplicities must be positive multiples of 32"); return 1; }
-  if (rc) { set_error(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError())); return 1; }
-  ++g_conv_launches;
-  return 0;
+  return conv_status(rc);
+}
+
+int launch_conv_jvp(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
+                    float* out, cudaStream_t st) {
+  if (a.n_dst <= a.n_begin) return 0;      // empty centre range
+  int rc = 2;
+  if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(jvp, l1, a, role, tan, out, st)
+  return conv_status(rc);
+}
+
+int launch_conv_bwd_tangent(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
+                            const float* gout, float* dx, float* dY_acc, float* dw, cudaStream_t st) {
+  if (a.n_dst <= a.n_begin) return 0;      // empty centre range
+  int rc = 2;
+  if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(bwdt, l1, a, role, tan, gout, dx, dY_acc, dw, st)
+  return conv_status(rc);
 }
 
 }  // namespace s7b

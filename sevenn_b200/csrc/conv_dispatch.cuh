@@ -113,6 +113,41 @@ static int bwd_kind_rt(bool table, bool need_dx, const ConvArgs& a, const ConvRo
   return launch_bwd_one<Kind, 0, 1, 16, ALLOW_NODX>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st);
 }
 
+// Second order (operator boundary only): runtime-width kernels with the lane mappings of the forward (jvp) and
+// the backward (bwd_tangent) above.
+template <class Kind, int NV, int LPN>
+static int launch_jvp_one(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan, float* out, cudaStream_t st) {
+  conv_jvp_kernel<Kind, NV, LPN><<<conv_grid<0, NV, LPN>(a, role), 32 * kConvWarpsPerBlock, 0, st>>>(a, role, tan, out);
+  return cudaGetLastError() == cudaSuccess ? 0 : 1;
+}
+
+template <class Kind, int NV, int LPN>
+static int launch_bwdt_one(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan, const float* gout,
+                           float* dx, float* dY, float* dw, cudaStream_t st) {
+  conv_bwd_tangent_kernel<Kind, NV, LPN><<<conv_grid<0, NV, LPN>(a, role), 32 * kConvWarpsPerBlock, 0, st>>>(
+      a, role, tan, gout, dx, dY, dw);
+  return cudaGetLastError() == cudaSuccess ? 0 : 1;
+}
+
+template <class Kind, int MAXNV>
+static int jvp_kind_rt(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan, float* out, cudaStream_t st) {
+  if (role.mul <= 0 || role.mul % 32 != 0) return kConvWrongMul;
+  if constexpr (MAXNV >= 2)
+    if (role.mul % 128 == 0) return launch_jvp_one<Kind, MAXNV, 32>(a, role, tan, out, st);
+  if (role.mul % 64 == 0) return launch_jvp_one<Kind, 1, 32>(a, role, tan, out, st);
+  return launch_jvp_one<Kind, 1, 16>(a, role, tan, out, st);
+}
+
+template <class Kind, int MAXNV>
+static int bwdt_kind_rt(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan, const float* gout,
+                        float* dx, float* dY, float* dw, cudaStream_t st) {
+  if (role.mul <= 0 || role.mul % 32 != 0) return kConvWrongMul;
+  if constexpr (MAXNV >= 2)
+    if (role.mul % 128 == 0) return launch_bwdt_one<Kind, MAXNV, 32>(a, role, tan, gout, dx, dY, dw, st);
+  if (role.mul % 64 == 0) return launch_bwdt_one<Kind, 1, 32>(a, role, tan, gout, dx, dY, dw, st);
+  return launch_bwdt_one<Kind, 1, 16>(a, role, tan, gout, dx, dY, dw, st);
+}
+
 // Paths (l2, l3) of the kind (l1, lmax_filter, lmax_out): the triangle rule with l2 <= LF, l3 <= LO
 constexpr int tp_npath(int l1, int lf, int lo) {
   int n = 0;
@@ -149,11 +184,25 @@ static int bwd_role(bool table, bool need_dx, const ConvArgs& a, const ConvRole&
   }
 }
 
+template <int L1, int LF, int LO, int MAXNV>
+static int jvp_role(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan, float* out, cudaStream_t st) {
+  if constexpr (tp_npath(L1, LF, LO) == 0) return kConvNoPath;
+  else return jvp_kind_rt<TPKind<L1, LF, LO>, MAXNV>(a, role, tan, out, st);
+}
+
+template <int L1, int LF, int LO, int MAXNV>
+static int bwdt_role(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan, const float* gout, float* dx,
+                     float* dY, float* dw, cudaStream_t st) {
+  if constexpr (tp_npath(L1, LF, LO) == 0) return kConvNoPath;
+  else return bwdt_kind_rt<TPKind<L1, LF, LO>, MAXNV>(a, role, tan, gout, dx, dY, dw, st);
+}
+
 }  // namespace s7b
 
 // Defines  launch_conv_fwd_LF_LO / launch_conv_bwd_LF_LO  for l1 = 0..3.  SPEC = 1 for the groups of SevenNet-0
 // and SevenNet-l3i5, which also get the kernels specialised for the widths kConvMul (l1 = 3 only with LF = 3);
-// the other groups have only the runtime-width kernels.
+// the other groups have only the runtime-width kernels.  launch_conv_jvp_LF_LO / launch_conv_bwdt_LF_LO: the
+// second-order kernels, runtime width in every group.
 #define S7B_CONV_SPEC_MUL(SPEC, LF, L1) ((SPEC) && ((L1) < 3 || (LF) >= 3) ? s7b::kConvMul[L1] : 0)
 #define S7B_DEFINE_CONV_GROUP(LF, LO, SPEC)                                                        \
   namespace s7b {                                                                                  \
@@ -175,6 +224,27 @@ static int bwd_role(bool table, bool need_dx, const ConvArgs& a, const ConvRole&
       case 1: return bwd_role<1, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 1), 1>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
       case 2: return bwd_role<2, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 2), 1>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
       case 3: return bwd_role<3, LF, LO, S7B_CONV_SPEC_MUL(SPEC, LF, 3), 1>(table, need_dx, a, role, gout, dx, dY, dEdr, dw, st); \
+    }                                                                                              \
+    return 1;                                                                                      \
+  }                                                                                                \
+  int launch_conv_jvp_##LF##_##LO(int l1, const ConvArgs& a, const ConvRole& role,                 \
+                                  const ConvTangents& tan, float* out, cudaStream_t st) {          \
+    switch (l1) {                                                                                  \
+      case 0: return jvp_role<0, LF, LO, S7B_FWD_L0_NV>(a, role, tan, out, st);                    \
+      case 1: return jvp_role<1, LF, LO, 1>(a, role, tan, out, st);                                \
+      case 2: return jvp_role<2, LF, LO, 1>(a, role, tan, out, st);                                \
+      case 3: return jvp_role<3, LF, LO, 1>(a, role, tan, out, st);                                \
+    }                                                                                              \
+    return 1;                                                                                      \
+  }                                                                                                \
+  int launch_conv_bwdt_##LF##_##LO(int l1, const ConvArgs& a, const ConvRole& role,                \
+                                   const ConvTangents& tan, const float* gout, float* dx,          \
+                                   float* dY, float* dw, cudaStream_t st) {                        \
+    switch (l1) {                                                                                  \
+      case 0: return bwdt_role<0, LF, LO, S7B_BWD_L0_NV>(a, role, tan, gout, dx, dY, dw, st);      \
+      case 1: return bwdt_role<1, LF, LO, 1>(a, role, tan, gout, dx, dY, dw, st);                  \
+      case 2: return bwdt_role<2, LF, LO, 1>(a, role, tan, gout, dx, dY, dw, st);                  \
+      case 3: return bwdt_role<3, LF, LO, 1>(a, role, tan, gout, dx, dY, dw, st);                  \
     }                                                                                              \
     return 1;                                                                                      \
   }                                                                                                \

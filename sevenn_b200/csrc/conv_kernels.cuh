@@ -25,6 +25,7 @@
 
 #include "common.cuh"
 #include "generated/tp_kinds.cuh"
+#include "tp_tangent.cuh"
 
 namespace s7b {
 
@@ -485,6 +486,185 @@ conv_bwd_kernel(const ConvArgs a, const ConvRole role, const float* __restrict__
         else dEdr_acc[e] += s;
       }
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// second order (operator boundary: stored weights, runtime width only).  Given tangents t = (tx, tY, tw) of the
+// backward's inputs, any of them absent (null pointer: zero, its terms skipped), and g = dE/d out:
+//   jvp:         out[n]      = sum_{e in row n} TP(tx[src],Y,w) + TP(x[src],tY,w) + TP(x[src],Y,tw)
+//   bwd_tangent: dx[src_e]  += (d_x TP(.,tY,w) + d_x TP(.,Y,tw))^T g[n]                (RED.ADD.F32x2, as dx)
+//                dY_acc[e]  += sum_u (d_Y TP(tx,.,w) + d_Y TP(x,.,tw))^T g[n]           (as dY_acc)
+//                dw[e, :]    = (d_w TP(tx,Y,.) + d_w TP(x,tY,.))^T g[n]
+// The per-lane arithmetic is TPTangent (tp_tangent.cuh); lane mapping, edge walk and reductions are those of
+// conv_fwd_kernel / conv_bwd_kernel, the tangents are read at the same offsets as their primals.  The backward's
+// per-edge sums go atomic when the role spans several CTAs (gridDim.y > 1), as in conv_bwd_kernel.
+// ------------------------------------------------------------------------------------------
+template <class Kind, int NV, int LPN>
+__global__ void S7B_FWD_BOUNDS
+conv_jvp_kernel(const ConvArgs a, const ConvRole role, const ConvTangents tan, float* __restrict__ out) {
+  const LaneMap<NV, LPN, 2> m(a);
+  if (m.nmax == 0 && !m.node_ok) return;      // whole warp beyond the last node (uniform)
+  const int mul = role.mul;
+  const bool hx = tan.x != nullptr, hY = tan.Y != nullptr, hw = tan.w != nullptr;
+
+  V2 acc[NV][Kind::NACC];
+#pragma unroll
+  for (int c = 0; c < NV; ++c)
+#pragma unroll
+    for (int q = 0; q < Kind::NACC; ++q) acc[c][q] = splat2(0.0f);
+
+  const unsigned xlane = role.x_off + m.uc0;
+  EdgeRecs<LPN> recs;
+  for (int it = 0; it < m.nmax; ++it) {
+    const bool valid = (LPN == 32) || (it < m.len);
+    const int e = valid ? m.e0 + it : 0;
+    if (it % LPN == 0) recs.fill(a, m.e0, m.len, it, m.sl);
+    const int4 rec = recs.get(it);
+    float Y[Kind::NY], tY[Kind::NY];
+    load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
+    if (hY) load_Y<Kind>(tan.Y + row_offset(e, y_stride(Kind::NY)), tY);
+    const size_t xo = row_offset(rec.x, a.dim_x) + xlane;
+    const size_t wo = (size_t)e * a.w_numel + m.uc0;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+      const int u = 2 * LPN * c;                         // channel offset from m.uc0
+      V2 x[Kind::D1], tx[Kind::D1], w[Kind::NPATH], tw[Kind::NPATH];
+#pragma unroll
+      for (int i = 0; i < Kind::D1; ++i) {
+        x[i] = ldg2(a.x + xo + (i * mul + u));
+        if (hx) tx[i] = ldg2(tan.x + xo + (i * mul + u));
+      }
+#pragma unroll
+      for (int p = 0; p < Kind::NPATH; ++p) {
+        w[p] = ldg2(a.w + wo + (role.w_off[p] + u));
+        if (hw) tw[p] = ldg2(tan.w + wo + (role.w_off[p] + u));
+        if (LPN != 32 && !valid) w[p] = tw[p] = splat2(0.0f);   // every term has w or tw as a factor
+      }
+      TPTangent<Kind>::jvp(x, Y, w, tx, tY, tw, hx, hY, hw, acc[c]);
+    }
+  }
+  if (!m.node_ok) return;
+  float* __restrict__ orow = out + (size_t)m.n * a.dim_mid;
+#pragma unroll
+  for (int c = 0; c < NV; ++c) {
+    const int u = m.uc0 + 2 * LPN * c;
+#pragma unroll
+    for (int p = 0; p < Kind::NPATH; ++p) {
+#pragma unroll
+      for (int k = 0; k < 2 * Kind::path_l3(p) + 1; ++k)
+        VT<V2>::store(orow + role.out_off[p] + k * role.out_stride[p] + u, acc[c][Kind::acc_off(p) + k]);
+    }
+  }
+}
+
+// One walk of conv_bwd_tangent_kernel over the CSR row of this lane's node, computing the outputs in OUT
+// (kTanDw | kTanDx | kTanDY)
+enum { kTanDw = 1, kTanDx = 2, kTanDY = 4 };
+template <class Kind, int NV, int LPN, int OUT>
+__device__ __forceinline__ void conv_bwd_tangent_edges(const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
+                                                       const LaneMap<NV, LPN, 2>& m, const V2 (&ga)[NV][Kind::NACC],
+                                                       float* __restrict__ dx, float* __restrict__ dY_acc,
+                                                       float* __restrict__ dw) {
+  constexpr bool DW = (OUT & kTanDw) != 0, DX = (OUT & kTanDx) != 0, DY = (OUT & kTanDY) != 0;
+  const int mul = role.mul;
+  const bool SPLIT = gridDim.y > 1;
+  const bool hx = tan.x != nullptr, hY = tan.Y != nullptr, hw = tan.w != nullptr;
+  const bool need_dx = DX && (hY || hw);
+  constexpr int NR = (Kind::NY <= 9) ? 8 : 16;   // values reduced with the transposing butterfly
+  constexpr int PER = LPN / NR;
+  const int idx = (m.sl / PER) % NR;                      // which reduced value ends up in this lane
+  const bool writer = (m.sl % PER) == 0 && idx + 1 < Kind::NY;
+  const unsigned xlane = role.x_off + m.uc0;
+  EdgeRecs<LPN> recs;
+  for (int it = 0; it < m.nmax; ++it) {
+    const bool valid = (LPN == 32) || (it < m.len);
+    const int e = valid ? m.e0 + it : 0;
+    if (it % LPN == 0) recs.fill(a, m.e0, m.len, it, m.sl);
+    const int4 rec = recs.get(it);
+    float Y[Kind::NY], tY[Kind::NY];
+    load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
+    if (hY && (DW || DX)) load_Y<Kind>(tan.Y + row_offset(e, y_stride(Kind::NY)), tY);
+    const size_t xo = row_offset(rec.x, a.dim_x) + xlane;
+    const size_t wo = (size_t)e * a.w_numel + m.uc0;
+    V2 dY[Kind::NY];
+#pragma unroll
+    for (int j = 0; j < Kind::NY; ++j) dY[j] = splat2(0.0f);
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+      const int u = 2 * LPN * c;                         // channel offset from m.uc0
+      V2 x[Kind::D1], tx[Kind::D1], w[Kind::NPATH], tw[Kind::NPATH], dwv[Kind::NPATH], dxv[Kind::D1];
+#pragma unroll
+      for (int i = 0; i < Kind::D1; ++i) {
+        x[i] = ldg2(a.x + xo + (i * mul + u));
+        if (hx && (DW || DY)) tx[i] = ldg2(tan.x + xo + (i * mul + u));
+      }
+#pragma unroll
+      for (int p = 0; p < Kind::NPATH; ++p) {
+        w[p] = ldg2(a.w + wo + (role.w_off[p] + u));
+        if (hw && (DX || DY)) tw[p] = ldg2(tan.w + wo + (role.w_off[p] + u));
+      }
+      TPTangent<Kind>::template bwd<DW, DX, DY>(x, Y, w, ga[c], tx, tY, tw, hx, hY, hw, dwv, dxv, dY);
+      if (valid) {
+        if (DW) {
+#pragma unroll
+          for (int p = 0; p < Kind::NPATH; ++p)
+            *reinterpret_cast<float2*>(dw + wo + (role.w_off[p] + u)) = dwv[p];
+        }
+        if (need_dx) {
+#pragma unroll
+          for (int i = 0; i < Kind::D1; ++i)
+            atomicAdd(reinterpret_cast<float2*>(dx + xo + (i * mul + u)), dxv[i]);
+        }
+      }
+    }
+    if (DY) {
+      float red[NR];
+#pragma unroll
+      for (int j = 0; j < NR; ++j) red[j] = (j + 1 < Kind::NY) ? dY[j + 1].x + dY[j + 1].y : 0.0f;
+      group_reduce_multi<NR, LPN>(red, m.sl);
+      if (valid && writer) {
+        float* dst = dY_acc + row_offset(e, y_stride(Kind::NY)) + idx;
+        if (SPLIT) atomicAdd(dst, red[0]);
+        else *dst += red[0];
+      }
+    }
+  }
+}
+
+// Kinds whose one-walk form needs more than 255 registers (from -Xptxas -v: it spilled 70-1300 bytes for every kind
+// above this bound and for none below) walk the row once per output instead: each walk runs only the terms of its
+// output, at about the register need of conv_bwd_kernel, for a second read of the row's operands.
+template <class Kind>
+constexpr bool tangent_walk_per_output() { return Kind::NACC * (Kind::D1 + Kind::NY) > 400; }
+
+template <class Kind, int NV, int LPN>
+__global__ void S7B_FWD_BOUNDS
+conv_bwd_tangent_kernel(const ConvArgs a, const ConvRole role, const ConvTangents tan, const float* __restrict__ gout,
+                        float* __restrict__ dx, float* __restrict__ dY_acc, float* __restrict__ dw) {
+  const LaneMap<NV, LPN, 2> m(a);
+  if (m.nmax == 0) return;                    // uniform: no edges in any row of this warp
+
+  V2 ga[NV][Kind::NACC];
+  {
+    const float* __restrict__ grow = gout + (size_t)(m.node_ok ? m.n : 0) * a.dim_mid;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+      const int u = m.uc0 + 2 * LPN * c;
+#pragma unroll
+      for (int p = 0; p < Kind::NPATH; ++p)
+#pragma unroll
+        for (int k = 0; k < 2 * Kind::path_l3(p) + 1; ++k)
+          ga[c][Kind::acc_off(p) + k] = ldg2(grow + role.out_off[p] + k * role.out_stride[p] + u);
+    }
+  }
+  if constexpr (!tangent_walk_per_output<Kind>()) {
+    conv_bwd_tangent_edges<Kind, NV, LPN, kTanDw | kTanDx | kTanDY>(a, role, tan, m, ga, dx, dY_acc, dw);
+  } else {
+    // dw is always written (zero without tx and tY); dx and dY_acc arrive zeroed
+    conv_bwd_tangent_edges<Kind, NV, LPN, kTanDw>(a, role, tan, m, ga, dx, dY_acc, dw);
+    if (tan.Y != nullptr || tan.w != nullptr) conv_bwd_tangent_edges<Kind, NV, LPN, kTanDx>(a, role, tan, m, ga, dx, dY_acc, dw);
+    if (tan.x != nullptr || tan.w != nullptr) conv_bwd_tangent_edges<Kind, NV, LPN, kTanDY>(a, role, tan, m, ga, dx, dY_acc, dw);
   }
 }
 

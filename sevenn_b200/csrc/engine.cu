@@ -51,6 +51,10 @@ int launch_conv_fwd(int l1, int lf, int lo, bool table, const ConvArgs& a, const
 int launch_conv_bwd(int l1, int lf, int lo, bool table, bool need_dx, const ConvArgs& a,
                     const ConvRole& role, const float* gout, float* dx, float* dY_acc,
                     float* dEdr_acc, float* dw, cudaStream_t st);
+int launch_conv_jvp(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
+                    float* out, cudaStream_t st);
+int launch_conv_bwd_tangent(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
+                            const float* gout, float* dx, float* dY_acc, float* dw, cudaStream_t st);
 
 static int64_t g_alloc_gen = 0;   // bumped by every (re)allocation: captured CUDA graphs hold raw pointers
 
@@ -2277,6 +2281,69 @@ int s7b_conv_backward(const S7bConvPlan* p, const float* x, const float* sh, con
   }
   cudaFreeAsync(rec, st);
   cudaFreeAsync(Ypk, st);
+  cudaFreeAsync(dY, st);
+  return rc;
+}
+
+int s7b_conv_double_backward(const S7bConvPlan* p, const float* x, const float* sh, const float* weight,
+                             const int32_t* rowptr, const int32_t* src, int32_t n_nodes, int32_t n_dst,
+                             int64_t n_edges, const float* grad_out, const float* tan_x, const float* tan_sh,
+                             const float* tan_weight, float* grad_grad_out, float* grad_x, float* grad_sh,
+                             float* grad_weight, void* stream) {
+  if (!p) return fail("null plan");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const LayerCfg& L = p->cfg;
+  const int n_sh = (p->lmax_filter + 1) * (p->lmax_filter + 1);
+  if (n_nodes > 0) S7B_CUDA_CHECK(cudaMemsetAsync(grad_x, 0, (size_t)n_nodes * L.x.dim * sizeof(float), st));
+  if (n_edges == 0 || n_dst <= 0 || (!tan_x && !tan_sh && !tan_weight)) {   // every term is zero: no launch
+    if (n_dst > 0) S7B_CUDA_CHECK(cudaMemsetAsync(grad_grad_out, 0, (size_t)n_dst * L.mid.dim * sizeof(float), st));
+    if (n_edges > 0) {
+      S7B_CUDA_CHECK(cudaMemsetAsync(grad_sh, 0, (size_t)n_edges * n_sh * sizeof(float), st));
+      S7B_CUDA_CHECK(cudaMemsetAsync(grad_weight, 0, (size_t)n_edges * L.W * sizeof(float), st));
+    }
+    return 0;
+  }
+  int4* rec = nullptr;
+  float *Ypk = nullptr, *tYpk = nullptr, *dY = nullptr;
+  const size_t ny_bytes = (size_t)n_edges * p->ny_stride * sizeof(float);
+  S7B_CUDA_CHECK(cudaMallocAsync((void**)&rec, (size_t)n_edges * sizeof(int4), st));
+  S7B_CUDA_CHECK(cudaMallocAsync((void**)&Ypk, ny_bytes, st));
+  if (tan_sh) S7B_CUDA_CHECK(cudaMallocAsync((void**)&tYpk, ny_bytes, st));
+  S7B_CUDA_CHECK(cudaMallocAsync((void**)&dY, (size_t)L.x.n_l * ny_bytes, st));
+  S7B_CUDA_CHECK(cudaMemsetAsync(dY, 0, (size_t)L.x.n_l * ny_bytes, st));
+  conv_pack_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(src, sh, n_sh, p->ny_stride, n_edges, rec, Ypk);
+  S7B_LAUNCH_CHECK();
+  if (tan_sh) {   // the tangent's harmonics in the same packed layout (rec is rewritten with the same values)
+    conv_pack_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(src, tan_sh, n_sh, p->ny_stride, n_edges, rec, tYpk);
+    S7B_LAUNCH_CHECK();
+  }
+  ConvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.rowptr = rowptr;
+  a.rec = rec;
+  a.Y = Ypk;
+  a.x = x;
+  a.w = weight;
+  a.n_dst = n_dst;
+  a.dim_x = L.x.dim;
+  a.dim_mid = L.mid.dim;
+  a.w_numel = L.W;
+  a.inv_h = 1.0f;
+  const ConvTangents tan{tan_x, tYpk, tan_weight};
+  int rc = 0;
+  for (int l1 = 0; l1 < L.x.n_l && !rc; ++l1)
+    rc = launch_conv_jvp(l1, p->lmax_filter, L.lmax_out, a, L.roles[l1], tan, grad_grad_out, st);
+  for (int l1 = 0; l1 < L.x.n_l && !rc; ++l1)
+    rc = launch_conv_bwd_tangent(l1, p->lmax_filter, L.lmax_out, a, L.roles[l1], tan, grad_out, grad_x,
+                                 dY + (size_t)l1 * n_edges * p->ny_stride, grad_weight, st);
+  if (!rc) {
+    conv_unpack_grad_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(dY, L.x.n_l, n_sh, p->ny_stride, n_edges, grad_sh);
+    ++g_launches;
+    if (cudaGetLastError() != cudaSuccess) rc = fail("conv_unpack_grad_kernel launch failed");
+  }
+  cudaFreeAsync(rec, st);
+  cudaFreeAsync(Ypk, st);
+  if (tYpk) cudaFreeAsync(tYpk, st);
   cudaFreeAsync(dY, st);
   return rc;
 }

@@ -63,6 +63,7 @@ EXPORTS = [
     's7b_engine_read_rows_host', 's7b_engine_write_rows_host', 's7b_engine_read_scalars_host', 's7b_engine_set_profiling',
     's7b_engine_profile_count', 's7b_engine_profile_entry', 's7b_conv_plan_create',
     's7b_conv_plan_destroy', 's7b_conv_plan_dims', 's7b_conv_forward', 's7b_conv_backward',
+    's7b_conv_double_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
 ]
@@ -138,6 +139,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_conv_plan_dims.argtypes = [vp] + [ctypes.POINTER(i32)] * 4
     lib.s7b_conv_forward.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i64, vp, vp]
     lib.s7b_conv_backward.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i64, vp, vp, vp, vp, vp]
+    lib.s7b_conv_double_backward.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = lib
     return lib
 
