@@ -186,6 +186,20 @@ S7B_API int s7b_engine_set_interior(S7bEngine* eng, int32_t n_interior);
 S7B_API int s7b_engine_run_stage(S7bEngine* eng, int stage, int layer, void* stream);
 S7B_API int s7b_engine_compute(S7bEngine* eng, void* stream);
 
+/* Second derivatives: the Hessian-vector product H v = (d2E/dr dr) v = -dF/de along positions r + e v, with the
+ * edge list held fixed (periodic images: the Gamma-point supercell Hessian).  Forward over reverse through every
+ * layer: the tangent of the forward, then the primal and tangent backward together, on the intermediates the last
+ * compute left (DESIGN.md §8).  The radial weights come from the radial MLP in forward mode (w, w', w'') in both
+ * radial modes, so a table-mode engine needs 'mlp0'..'mlp2' set too (a compute never reads them).  The first call
+ * allocates its buffers (about 7 x E x W floats at the widest layer); a compute that never meets an HVP allocates
+ * and launches exactly what it did before.  Single GPU, one tangent per call, not captured into a CUDA graph.
+ *
+ * Hv (eV/A^2, [n_nodes,3], overwritten) for the tangent v [n_nodes,3] (device pointers), on the graph and
+ * forward of the last s7b_engine_compute.  Fails (message set, nothing launched) without such a compute since
+ * the last set_graph / set_param (setting 'mlp0'..'mlp2' of a table-mode engine keeps it), on a graph with ghosts
+ * (n_local < n_nodes), or when an 'mlp' parameter is missing.  E == 0 zero-fills. */
+S7B_API int s7b_engine_hvp(S7bEngine* eng, const float* d_v, float* d_out, void* stream);
+
 /* Device pointer to an engine-owned buffer (valid until the next set_graph that grows it):
  * "x" (layer t input after self_interaction_1, [n_nodes, dim_x(t)]), "dx", "gate_in", "mid",
  * "h", "energy" (double[1]), "atomic_energy" [n_local], "atomic_energy_f64" (double[n_local], the same

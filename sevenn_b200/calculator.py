@@ -96,10 +96,8 @@ class SevenNetCalculator(_Base):
         self.compute_atomic_virial = compute_atomic_virial
         self.sevennet_config = sevennet_config or dict(self.meta)
 
-    def calculate(self, atoms=None, properties=None, system_changes=_all_changes):
-        super().calculate(atoms, properties, system_changes)
-        if atoms is None:
-            raise ValueError('No atoms to evaluate')
+    def _inputs(self, atoms):
+        """(species, positions, cell, pbc, atomic numbers) of ``atoms`` for the engine"""
         pos = np.asarray(atoms.get_positions(), dtype=np.float64)
         cell = np.asarray(atoms.get_cell(), dtype=np.float64).reshape(3, 3)
         pbc = np.asarray(atoms.get_pbc(), dtype=bool)
@@ -108,6 +106,13 @@ class SevenNetCalculator(_Base):
             species = np.array([self.type_map[int(z)] for z in numbers], dtype=np.int32)
         except KeyError as e:  # same failure mode as sequential.py:131-137 for unknown elements
             raise ValueError(f'atomic number {e} is not known to this model') from None
+        return species, pos, cell, pbc, numbers
+
+    def calculate(self, atoms=None, properties=None, system_changes=_all_changes):
+        super().calculate(atoms, properties, system_changes)
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        species, pos, cell, pbc, numbers = self._inputs(atoms)
         # neighbour list, graph build, model and force path all run on the GPU (one C-ABI call);
         # the reference builds the graph on the CPU every step (calculator.py:224-226)
         energy, energies, forces, virial, n_edges = self.engine.compute_positions(species, pos, cell, pbc)
@@ -126,3 +131,24 @@ class SevenNetCalculator(_Base):
         if self.compute_atomic_virial:   # calculator.py:211-216: 'stresses' = the per-atom virial as the model gives it
             self.results['stresses'] = self.engine.buffer('atomic_virial', shape=(len(numbers), 6)).cpu().numpy().astype(np.float64)
         return self.results
+
+    def get_hessian(self, atoms=None) -> np.ndarray:
+        """Hessian d2E/dr dr of ``atoms`` (default: the calculator's atoms), [3N, 3N] float64 in eV/A^2, row 3i + a
+        = H e_(i,a).  Built from 3N Hessian-vector products (``B200Engine.hvp``) on the calculator's own graph of the
+        atoms, with that edge list held fixed, so a periodic cell gives the Gamma-point (supercell) Hessian that
+        phonon codes take force constants from.  Not symmetrised (the two triangles agree to the fp32 error of the
+        products); ``.reshape(N, 3, N, 3)`` gives the force constants Phi[i, a, j, b].  ``results`` and the other
+        ``get_*`` methods are not touched.  D3 dispersion has no second order here."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        torch = self.engine.torch
+        species, pos, cell, pbc, _ = self._inputs(atoms)
+        n = len(species)
+        self.engine.set_positions(species, pos, cell, pbc)
+        self.engine.compute()
+        eye = torch.eye(3 * n, dtype=torch.float32, device=self.engine.device)
+        rows = [self.engine.hvp(eye[k].reshape(n, 3)).reshape(-1) for k in range(3 * n)]
+        if not rows:
+            return np.zeros((0, 0))
+        return torch.stack(rows).double().cpu().numpy()

@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "conv_kernels.cuh"
 #include "edge_kernels.cuh"
+#include "hvp_kernels.cuh"
 #include "neighbor.cuh"
 #include "node_kernels.cuh"
 #include "tc_gemm.cuh"
@@ -193,6 +194,23 @@ struct LayerParams {
   }
 };
 
+// Buffers of the Hessian-vector product (s7b_engine_hvp), allocated on its first call: a step that never meets
+// one allocates and launches nothing more.  Edge buffers hold E rows, node buffers n_nodes rows.
+struct HvpBufs {
+  DevBuf dvec, dr, dY, gY, dgY, ar, dar, fneg, virial;     // edge tangents, dE/dY and dE/dr with their tangents
+  DevBuf emb3, hA, hB, w3, dw, aw, daw1, daw2;             // radial jets [3][E][.] of one layer; [E, W] weights
+  DevBuf ah, dah, ag, dag, amid, damid, dmid, ax, dax, th;  // node adjoints and tangents of one layer
+  std::vector<DevBuf> tx, tg;                             // per layer: tangents of x[t] and g[t]
+  RowExp re;
+  void release() {
+    for (DevBuf* b : {&dvec, &dr, &dY, &gY, &dgY, &ar, &dar, &fneg, &virial, &emb3, &hA, &hB, &w3, &dw, &aw, &daw1, &daw2,
+                      &ah, &dah, &ag, &dag, &amid, &damid, &dmid, &ax, &dax, &th, &re.buf})
+      b->release();
+    for (auto* v : {&tx, &tg})
+      for (DevBuf& b : *v) b.release();
+  }
+};
+
 // The global parameters ("bessel" lives in RadialDesc)
 struct GlobalParams {
   DevBuf embed_x0, embed_g0, readout, readout_lo, scale, shift;
@@ -270,6 +288,9 @@ struct S7bEngine {
   std::map<int, StageGraph> stage_graphs;
   bool capturing = false;
   int64_t sg_captures = 0, sg_replays = 0;
+  // second order: hvp_ready = an s7b_engine_compute ran since the last set_graph / set_param
+  bool hvp_ready = false;
+  HvpBufs hv;
 };
 
 struct S7bConvPlan {
@@ -1083,6 +1104,7 @@ void s7b_engine_destroy(S7bEngine* e) {
   for (DevBuf* b : bufs) b->release();
   for (auto* v : {&e->x, &e->g, &e->wbuf, &e->z1, &e->z2, &e->h1, &e->h2})
     for (auto& b : *v) b.release();
+  e->hv.release();
   delete e;
 }
 
@@ -1104,6 +1126,9 @@ static int upload(DevBuf& dst, const float* host, size_t numel, const std::strin
 int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float* host, size_t numel) {
   if (!e || !name || !host) return fail("null argument");
   const std::string nm(name);
+  // a parameter the step reads leaves the last compute's intermediates stale for s7b_engine_hvp; the radial MLP of a
+  // table-mode engine is read by the HVP alone
+  if (!(e->desc.table_knots > 0 && nm.compare(0, 3, "mlp") == 0)) e->hvp_ready = false;
   const int T = e->desc.n_layers, S = e->desc.num_species, nb = e->desc.n_basis;
   const std::string what = (layer >= 0 ? "layer " + std::to_string(layer) + ": " : std::string()) + "parameter " + nm;
   auto bad_size = [&](size_t expect) {
@@ -1207,6 +1232,7 @@ int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t
   if (!e) return fail("null engine");
   if (n_local < 0 || n_nodes < n_local || n_edges < 0) return fail("bad graph sizes");
   if (n_edges >= ((int64_t)1 << 31)) return fail("more than 2^31-1 edges per GPU are not supported");
+  e->hvp_ready = false;
   e->n_nodes = n_nodes;
   e->n_local = n_local;
   e->n_interior = n_local;
@@ -1675,8 +1701,13 @@ static int run_all_stages(S7bEngine* e, void* stream) {
 // neighbour count replay the same graph.
 int s7b_engine_compute(S7bEngine* e, void* stream) {
   if (!e) return fail("null engine");
+  e->hvp_ready = false;
   const bool table = e->desc.table_knots > 0;
-  if (!g_opt_cuda_graph || !table || e->prof.enabled) return run_all_stages(e, stream);
+  if (!g_opt_cuda_graph || !table || e->prof.enabled) {
+    const int rc = run_all_stages(e, stream);
+    e->hvp_ready = rc == 0;
+    return rc;
+  }
   if (!e->radial_ready) return fail("parameter 'bessel' was not set");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (ensure_graph_stream(e)) return 1;
@@ -1694,7 +1725,178 @@ int s7b_engine_compute(S7bEngine* e, void* stream) {
   S7B_CUDA_CHECK(cudaStreamWaitEvent(st, e->g_out, 0));
   g_launches += e->g_launches_per_replay;
   ++e->g_replays;
+  e->hvp_ready = true;
   return 0;
+}
+
+// ---- second order: Hessian-vector product -----------------------------------------------------------------------
+// Hv = d(dE/dr)/de along r + e v, forward over reverse on the graph and forward of the last compute (DESIGN.md §8).
+// The radial weights come from the radial MLP in forward mode in both radial modes (w'' of the cubic table is not
+// accurate enough: fp16 a2/a3, and XPLOR is only C1 at r_on), one layer at a time, and the convolution runs its raw
+// (stored-weight) kernels on them.
+
+// w, w', w'' of layer t as hv.w3 [3][E][W] from the radial basis jet hv.emb3 [3][E][n_basis]
+static int hvp_radial_jet(S7bEngine* e, int t, cudaStream_t st) {
+  const LayerParams& P = e->layer_params[t];
+  const int64_t E3 = 3 * e->n_edges;
+  const int nb = e->desc.n_basis, h0 = e->desc.radial_hidden[0], h1 = e->desc.radial_hidden[1], W = e->layers[t].W;
+  HvpBufs& hv = e->hv;
+  if (dense_gemm(hv.emb3.as<float>(), nb, hv.hA.as<float>(), h0, P.mlp[0].as<float>(), E3, kEpiNone, nullptr, nullptr, false, st)) return 1;
+  hvp_silu_jet_kernel<<<grid1d((size_t)e->n_edges * h0, 256), 256, 0, st>>>(hv.hA.as<float>(), e->n_edges * h0);
+  S7B_LAUNCH_CHECK();
+  if (dense_gemm(hv.hA.as<float>(), h0, hv.hB.as<float>(), h1, P.mlp[1].as<float>(), E3, kEpiNone, nullptr, nullptr, false, st)) return 1;
+  hvp_silu_jet_kernel<<<grid1d((size_t)e->n_edges * h1, 256), 256, 0, st>>>(hv.hB.as<float>(), e->n_edges * h1);
+  S7B_LAUNCH_CHECK();
+  if (dense_gemm(hv.hB.as<float>(), h1, hv.w3.as<float>(), W, P.mlp[2].as<float>(), E3, kEpiNone, nullptr, nullptr, false, st)) return 1;
+  hvp_scale_rows_kernel<<<grid1d((size_t)e->n_edges * W, 256), 256, 0, st>>>(hv.w3.as<float>() + (size_t)e->n_edges * W, hv.dr.as<float>(), e->n_edges, W, hv.dw.as<float>());
+  S7B_LAUNCH_CHECK();
+  return 0;
+}
+
+static int hvp_alloc(S7bEngine* e) {
+  HvpBufs& hv = e->hv;
+  const size_t E = (size_t)e->n_edges, N = (size_t)std::max(e->n_nodes, 1), ny = (size_t)e->ny_stride;
+  const int T = e->desc.n_layers;
+  size_t mx = 0, mg = 0, mm = 0, mh = 0, mW = 0;
+  hv.tx.resize(T);
+  hv.tg.resize(T);
+  int rc = 0;
+  for (int t = 0; t < T; ++t) {
+    const LayerCfg& L = e->layers[t];
+    mx = std::max(mx, (size_t)L.x.dim);
+    mg = std::max(mg, (size_t)L.g.dim);
+    mm = std::max(mm, (size_t)L.mid.dim);
+    mh = std::max(mh, (size_t)L.dim_h);
+    mW = std::max(mW, (size_t)L.W);
+    rc |= hv.tx[t].ensure(N * L.x.dim * sizeof(float));
+    rc |= hv.tg[t].ensure(N * L.g.dim * sizeof(float));
+  }
+  mh = std::max(mh, mx);
+  for (DevBuf* b : {&hv.ah, &hv.dah, &hv.th}) rc |= b->ensure(N * mh * sizeof(float));
+  for (DevBuf* b : {&hv.ag, &hv.dag}) rc |= b->ensure(N * mg * sizeof(float));
+  for (DevBuf* b : {&hv.amid, &hv.damid, &hv.dmid}) rc |= b->ensure(N * mm * sizeof(float));
+  for (DevBuf* b : {&hv.ax, &hv.dax}) rc |= b->ensure(N * mx * sizeof(float));
+  rc |= hv.re.buf.ensure(N * 16 * sizeof(int));
+  rc |= hv.virial.ensure(6 * sizeof(double));
+  for (DevBuf* b : {&hv.dvec, &hv.fneg}) rc |= b->ensure(E * 3 * sizeof(float));
+  for (DevBuf* b : {&hv.dr, &hv.ar, &hv.dar}) rc |= b->ensure(E * sizeof(float));
+  for (DevBuf* b : {&hv.dY, &hv.gY, &hv.dgY}) rc |= b->ensure(E * ny * sizeof(float));
+  rc |= hv.emb3.ensure(3 * E * e->desc.n_basis * sizeof(float));
+  rc |= hv.hA.ensure(3 * E * e->desc.radial_hidden[0] * sizeof(float));
+  rc |= hv.hB.ensure(3 * E * e->desc.radial_hidden[1] * sizeof(float));
+  rc |= hv.w3.ensure(3 * E * mW * sizeof(float));
+  for (DevBuf* b : {&hv.dw, &hv.aw, &hv.daw1, &hv.daw2}) rc |= b->ensure(E * mW * sizeof(float));
+  return rc ? fail("cudaMalloc failed for the Hessian-vector product's buffers") : 0;
+}
+
+static int hvp_pass(S7bEngine* e, const float* v, float* out, cudaStream_t st) {
+  const int T = e->desc.n_layers, LF = e->desc.lmax_filter, N = e->n_nodes;
+  const int64_t E = e->n_edges;
+  HvpBufs& hv = e->hv;
+  const int ny = e->ny_stride;
+  // ---- edge tangents and the radial basis jet (layer independent)
+  {
+    const int grd = (N * 32 + 255) / 256;
+    if (LF == 1) hvp_edge_fwd_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    else if (LF == 2) hvp_edge_fwd_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    else hvp_edge_fwd_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    S7B_LAUNCH_CHECK();
+    hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, hv.emb3.as<float>());
+    S7B_LAUNCH_CHECK();
+  }
+  auto conv_args = [&](int t) {
+    ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
+    ca.w = hv.w3.as<float>();          // raw kernels on the MLP's weights, in both radial modes
+    return ca;
+  };
+  // ---- tangent forward: dx(0) = 0 (the embedding depends on the species only), dx(t) = si1(dh(t-1)),
+  // dmid = conv JVP, dg = si2(dmid) + sc(dh(t-1)), dh = gate'(g) dg
+  for (int t = 0; t < T; ++t) {
+    const LayerCfg& L = e->layers[t];
+    const LayerParams& P = e->layer_params[t];
+    if (hvp_radial_jet(e, t, st)) return 1;
+    if (t > 0 && node_linear(e, P.si1, hv.re, true, hv.th.as<float>(), hv.tx[t].as<float>(), false, st)) return 1;
+    const ConvArgs ca = conv_args(t);
+    const ConvTangents tan{t > 0 ? hv.tx[t].as<float>() : nullptr, hv.dY.as<float>(), hv.dw.as<float>()};
+    for (int l1 = 0; l1 < L.x.n_l; ++l1)
+      if (launch_conv_jvp(l1, LF, L.lmax_out, ca, L.roles[l1], tan, hv.dmid.as<float>(), st)) return 1;
+    S7B_CUDA_CHECK(cudaMemsetAsync(hv.tg[t].p, 0, (size_t)N * L.g.dim * sizeof(float), st));
+    if (t > 0 && node_linear(e, P.sc, hv.re, true, hv.th.as<float>(), hv.tg[t].as<float>(), false, st)) return 1;
+    if (node_linear(e, P.si2, hv.re, true, hv.dmid.as<float>(), hv.tg[t].as<float>(), true, st)) return 1;
+    gate_jvp_kernel<<<grid1d((size_t)N * L.dim_h, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), hv.tg[t].as<float>(), hv.th.as<float>(), N);
+    S7B_LAUNCH_CHECK();
+  }
+  // ---- primal and tangent backward together, in reverse layer order.  The readout is linear: dah(T) = 0.
+  const LayerCfg& Lz = e->layers[T - 1];
+  const GlobalParams& G = e->global_params;
+  hvp_readout_seed_kernel<<<grid1d((size_t)N * Lz.dim_h, 256), 256, 0, st>>>(G.readout.as<float>(), G.scale.as<float>(), e->d_species, N, Lz.dim_h, hv.ah.as<float>());
+  S7B_LAUNCH_CHECK();
+  S7B_CUDA_CHECK(cudaMemsetAsync(hv.dah.p, 0, (size_t)N * Lz.dim_h * sizeof(float), st));
+  for (DevBuf* b : {&hv.gY, &hv.dgY}) S7B_CUDA_CHECK(cudaMemsetAsync(b->p, 0, (size_t)E * ny * sizeof(float), st));
+  for (DevBuf* b : {&hv.ar, &hv.dar}) S7B_CUDA_CHECK(cudaMemsetAsync(b->p, 0, (size_t)E * sizeof(float), st));
+  for (int t = T - 1; t >= 0; --t) {
+    const LayerCfg& L = e->layers[t];
+    const LayerParams& P = e->layer_params[t];
+    if (hvp_radial_jet(e, t, st)) return 1;
+    const int gg = grid1d((size_t)N * L.g.dim, 256);
+    gate_bwd_kernel<<<gg, 256, 0, st>>>(L.gate, e->g[t].as<float>(), hv.ah.as<float>(), hv.ag.as<float>(), N);
+    S7B_LAUNCH_CHECK();
+    gate_bwd_tangent_kernel<<<gg, 256, 0, st>>>(L.gate, e->g[t].as<float>(), hv.tg[t].as<float>(), hv.ah.as<float>(), hv.dah.as<float>(), hv.dag.as<float>(), N);
+    S7B_LAUNCH_CHECK();
+    if (node_linear(e, P.si2T, hv.re, true, hv.ag.as<float>(), hv.amid.as<float>(), false, st)) return 1;
+    if (node_linear(e, P.si2T, hv.re, true, hv.dag.as<float>(), hv.damid.as<float>(), false, st)) return 1;
+    for (DevBuf* b : {&hv.ax, &hv.dax}) S7B_CUDA_CHECK(cudaMemsetAsync(b->p, 0, (size_t)N * L.x.dim * sizeof(float), st));
+    const ConvArgs ca = conv_args(t);
+    const ConvTangents tan{t > 0 ? hv.tx[t].as<float>() : nullptr, hv.dY.as<float>(), hv.dw.as<float>()};
+    for (int l1 = 0; l1 < L.x.n_l; ++l1) {
+      const ConvRole& role = L.roles[l1];
+      // primal adjoints (dE/dx, dE/dY, dE/dw) and their tangent: the backward of the tangent adjoint dmid plus
+      // the second-order terms of the operand tangents contracted with the primal adjoint
+      if (launch_conv_bwd(l1, LF, L.lmax_out, false, t > 0, ca, role, hv.amid.as<float>(), hv.ax.as<float>(), hv.gY.as<float>(), nullptr, hv.aw.as<float>(), st) ||
+          launch_conv_bwd(l1, LF, L.lmax_out, false, t > 0, ca, role, hv.damid.as<float>(), hv.dax.as<float>(), hv.dgY.as<float>(), nullptr, hv.daw1.as<float>(), st) ||
+          launch_conv_bwd_tangent(l1, LF, L.lmax_out, ca, role, tan, hv.amid.as<float>(), hv.dax.as<float>(), hv.dgY.as<float>(), hv.daw2.as<float>(), st))
+        return 1;
+    }
+    const float* w3 = hv.w3.as<float>();
+    hvp_radial_reduce_kernel<<<(int)((E * 32 + 255) / 256), 256, 0, st>>>(hv.aw.as<float>(), hv.daw1.as<float>(), hv.daw2.as<float>(), w3 + (size_t)E * L.W,
+                                                                         w3 + 2 * (size_t)E * L.W, hv.dr.as<float>(), E, L.W, hv.ar.as<float>(), hv.dar.as<float>());
+    S7B_LAUNCH_CHECK();
+    if (t > 0) {   // dE/dh(t-1) = sc^T dg + si1^T dx, and its tangent
+      for (DevBuf* b : {&hv.ah, &hv.dah}) S7B_CUDA_CHECK(cudaMemsetAsync(b->p, 0, (size_t)N * L.x.dim * sizeof(float), st));
+      if (node_linear(e, P.scT, hv.re, true, hv.ag.as<float>(), hv.ah.as<float>(), false, st) ||
+          node_linear(e, P.si1T, hv.re, true, hv.ax.as<float>(), hv.ah.as<float>(), true, st) ||
+          node_linear(e, P.scT, hv.re, true, hv.dag.as<float>(), hv.dah.as<float>(), false, st) ||
+          node_linear(e, P.si1T, hv.re, true, hv.dax.as<float>(), hv.dah.as<float>(), true, st))
+        return 1;
+    }
+  }
+  // ---- edge backward tangent and the force scatter of its negative: H v
+  const int grd = (int)((E + 255) / 256);
+  if (LF == 1) hvp_edge_bwd_kernel<1><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>());
+  else if (LF == 2) hvp_edge_bwd_kernel<2><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>());
+  else hvp_edge_bwd_kernel<3><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>());
+  S7B_LAUNCH_CHECK();
+  S7B_CUDA_CHECK(cudaMemsetAsync(hv.virial.p, 0, 6 * sizeof(double), st));
+  force_scatter_kernel<<<(N * 32 + 255) / 256, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, hv.fneg.as<float>(), N, out, hv.virial.as<double>(), nullptr);
+  S7B_LAUNCH_CHECK();
+  return 0;
+}
+
+int s7b_engine_hvp(S7bEngine* e, const float* d_v, float* d_out, void* stream) {
+  if (!e) return fail("null engine");
+  if (!e->hvp_ready) return fail("s7b_engine_hvp needs an s7b_engine_compute on the current graph and parameters");
+  if (e->n_local < e->n_nodes) return fail("s7b_engine_hvp does not run on graphs with ghost atoms (n_local < n_nodes)");
+  for (int t = 0; t < e->desc.n_layers; ++t)
+    for (int j = 0; j < 3; ++j)
+      if (!e->layer_params[t].mlp[j].p)
+        return fail("s7b_engine_hvp evaluates the radial MLP: parameter mlp" + std::to_string(j) + " of layer " + std::to_string(t) + " is missing");
+  if (e->n_nodes > 0 && (!d_v || !d_out)) return fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (e->n_nodes == 0) return 0;
+  S7B_CUDA_CHECK(cudaMemsetAsync(d_out, 0, (size_t)e->n_nodes * 3 * sizeof(float), st));
+  if (e->n_edges == 0) return 0;      // the energy does not depend on the positions
+  if (hvp_alloc(e)) return 1;
+  return hvp_pass(e, d_v, d_out, st);
 }
 
 int s7b_engine_graph_stats(S7bEngine* e, int64_t* captures, int64_t* replays) {

@@ -215,6 +215,41 @@ def gen_sh(lmax: int) -> str:
     return '\n'.join(lines)
 
 
+def gen_sh2(lmax: int) -> str:
+    """SH2<L>::jvp: dY[j] = sum_c dY_j/du_c t_c (j = 1..);  SH2<L>::hvp: h_c = sum_d d2(gY . Y)/du_c du_d t_d,
+    both w.r.t. the unconstrained unit-vector components like SH<L>::vjp (the Hessian-vector product's edge terms)."""
+    import sympy as sp
+    polys = sh_polynomials(lmax)
+    n = len(polys)
+    tsym = sp.symbols('tx ty tz', real=True)
+    lines = [f'template <> struct SH2<{lmax}> {{',
+             '  // Jacobian-vector product: writes dY[1..NY-1] (dY[0] = 0)',
+             '  S7B_HD static void jvp(float x, float y, float z, float tx, float ty, float tz, float* __restrict__ dY) {',
+             '    dY[0] = 0.0f;']
+    jv = [sp.N(sp.expand(sum(sp.diff(p, v) * t for v, t in zip((X, Y, Z), tsym))), 12) for p in polys[1:]]
+    repl, red = sp.cse(jv, optimizations='basic')
+    for s, e in repl:
+        lines.append(f'    const float {s} = {_cc(e)};')
+    for j, e in enumerate(red):
+        lines.append(f'    dY[{j + 1}] = {_cc(e)};')
+    lines.append('  }')
+    lines.append('  // Hessian of gY . Y(u) times t')
+    lines.append('  S7B_HD static void hvp(float x, float y, float z, const float* __restrict__ gY, float tx, float ty,')
+    lines.append('                         float tz, float& hx, float& hy, float& hz) {')
+    gsym = sp.symbols(f'g1:{n}', real=True)
+    tot = sum(g * p for g, p in zip(gsym, polys[1:]))
+    hv = [sp.N(sp.expand(sum(sp.diff(tot, a, b) * t for b, t in zip((X, Y, Z), tsym))), 12) for a in (X, Y, Z)]
+    repl, red = sp.cse(hv, optimizations='basic')
+    sub = {str(g): f'gY[{j + 1}]' for j, g in enumerate(gsym)}
+    for s, e in repl:
+        lines.append(f'    const float {s} = {_cc(e, sub)};')
+    for nme, e in zip(('hx', 'hy', 'hz'), red):
+        lines.append(f'    {nme} = {_cc(e, sub)};')
+    lines.append('  }')
+    lines.append('};')
+    return '\n'.join(lines)
+
+
 def _cc(expr, sub=None) -> str:
     import sympy as sp
     from sympy.printing.c import C99CodePrinter
@@ -256,6 +291,9 @@ def main():
     tp += ''.join(gen_kind(*k) + '\n\n' for k in KINDS) + '}  // namespace s7b\n'
     sh = HEADER + 'namespace s7b {\ntemplate <int LMAX> struct SH;\n\n'
     sh += ''.join(gen_sh(lmax) + '\n\n' for lmax in (1, 2, 3)) + '}  // namespace s7b\n'
+    # second order (Hessian-vector products), appended so that the first-order text above stays as it is
+    sh += '\n// second order: SH2<L>::jvp / SH2<L>::hvp\nnamespace s7b {\ntemplate <int LMAX> struct SH2;\n\n'
+    sh += ''.join(gen_sh2(lmax) + '\n\n' for lmax in (1, 2, 3)) + '}  // namespace s7b\n'
     for fname, text in (('tp_kinds.cuh', tp), ('sh.cuh', sh)):
         path = os.path.join(gen_dir, fname)
         if not os.path.exists(path) or open(path).read() != text:   # keep mtimes for make

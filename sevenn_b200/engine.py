@@ -66,6 +66,7 @@ EXPORTS = [
     's7b_conv_double_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
+    's7b_engine_hvp',
 ]
 
 
@@ -114,6 +115,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_set_graph.argtypes = [vp, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.s7b_engine_run_stage.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]
     lib.s7b_engine_compute.argtypes = [vp, vp]
+    lib.s7b_engine_hvp.argtypes = [vp, vp, vp, vp]
     lib.s7b_engine_buffer.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(sz)]
     lib.s7b_engine_buffer.restype = vp
     lib.s7b_engine_compute_host.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -200,6 +202,48 @@ def radial_weights(spec: ModelSpec, arrays: Dict[str, np.ndarray], t: int, r: np
         else:
             h, dh = z, dz
     return h, dh
+
+
+def radial_weights_jet(spec: ModelSpec, arrays: Dict[str, np.ndarray], t: int, r: np.ndarray):
+    """w(r), dw/dr and d2w/dr2 [len(r), W] of layer t's radial MLP in forward mode, float64, zero from the cutoff
+    on: what the Hessian-vector product evaluates per edge (csrc/hvp_math.cuh, csrc/hvp_kernels.cuh)."""
+    r = np.asarray(r, dtype=np.float64)
+    rr = r[:, None]
+    c = np.asarray(arrays['bessel_coeffs'], dtype=np.float64)[None, :]
+    pre = 2.0 / spec.cutoff
+    with np.errstate(divide='ignore', invalid='ignore'):
+        sn, cs = np.sin(c * rr), np.cos(c * rr)
+        b = [pre * sn / rr, pre * (c * cs - sn / rr) / rr, pre * (-c * c * sn - 2 * c * cs / rr + 2 * sn / rr ** 2) / rr]
+    if spec.cutoff_fn == 'XPLOR':
+        on2, c2, r2 = spec.cutoff_on ** 2, spec.cutoff ** 2, r * r
+        den = (c2 - on2) ** 3
+        a, bb = c2 - r2, c2 + 2 * r2 - 3 * on2
+        inner = r >= spec.cutoff_on
+        f = [np.where(inner, a * a * bb / den, 1.0), np.where(inner, (-4 * r * a * bb + 4 * r * a * a) / den, 0.0),
+             np.where(inner, (-4 * a * bb + 8 * r2 * bb - 32 * r2 * a + 4 * a * a) / den, 0.0)]
+    else:
+        p = float(spec.poly_p)
+        x = r / spec.cutoff
+        c0, c1, c2 = (p + 1) * (p + 2) / 2, p * (p + 2), p * (p + 1) / 2
+        f = [1 - c0 * x ** p + c1 * x ** (p + 1) - c2 * x ** (p + 2),
+             (-c0 * p * x ** (p - 1) + c1 * (p + 1) * x ** p - c2 * (p + 2) * x ** (p + 1)) / spec.cutoff,
+             (-c0 * p * (p - 1) * x ** (p - 2) + c1 * (p + 1) * p * x ** (p - 1) - c2 * (p + 2) * (p + 1) * x ** p)
+             / spec.cutoff ** 2]
+    inside = (r < spec.cutoff)[:, None]
+    f = [np.where(inside, fk[:, None], 0.0) for fk in f]
+    h = [b[0] * f[0], b[1] * f[0] + b[0] * f[1], b[2] * f[0] + 2 * b[1] * f[1] + b[0] * f[2]]
+    n_mlp = len(spec.radial_hidden) + 1
+    for j in range(n_mlp):
+        W = arrays[f'{t}.mlp{j}'].astype(np.float64) / math.sqrt(arrays[f'{t}.mlp{j}'].shape[0])
+        z = [hk @ W for hk in h]
+        if j < n_mlp - 1:
+            s = 1.0 / (1.0 + np.exp(-z[0]))
+            d1 = SILU_NORM * _dsilu(z[0])
+            d2 = SILU_NORM * s * (1 - s) * (2 + z[0] * (1 - 2 * s))
+            h = [SILU_NORM * _silu(z[0]), d1 * z[1], d2 * z[1] ** 2 + d1 * z[2]]
+        else:
+            h = z
+    return h[0], h[1], h[2]
 
 
 def radial_table(spec: ModelSpec, arrays: Dict[str, np.ndarray], t: int, knots: int) -> np.ndarray:
@@ -441,6 +485,8 @@ class B200Engine:
                 check(self.lib.s7b_engine_set_param(self._h, name.encode(), t, arr.ctypes.data, arr.size))
         self._graph = None
         self.n_nodes = self.n_local = self.n_edges = 0
+        self._arrays = arrays
+        self._hvp_mlp = radial == 'mlp'        # the radial MLP is on the device (hvp reads it in both radial modes)
 
     def __del__(self):
         try:
@@ -554,6 +600,23 @@ class B200Engine:
         with self.torch.cuda.device(self.device):
             check(self.lib.s7b_engine_compute(self._h, self._stream()))
         return self
+
+    def hvp(self, v):
+        """Hessian-vector product H v = (d2E/dr dr) v, [n_nodes, 3] float32 device tensor in eV/A^2, on the graph and
+        forward of the last ``compute``, with its edge list held fixed (C ABI ``s7b_engine_hvp``).  v [n_nodes, 3],
+        numpy or torch (any device).  A table-mode engine uploads its radial MLP on the first call: the second order
+        evaluates w, w' and w'' from it rather than from the tables."""
+        torch = self.torch
+        v = torch.as_tensor(v).to(self.device, torch.float32).contiguous().reshape(self.n_nodes, 3)
+        out = torch.empty(self.n_nodes, 3, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            if not self._hvp_mlp:
+                for (name, t), arr in prepare_params(self.spec, self._arrays, 'mlp', 0).items():
+                    if name in ('mlp0', 'mlp1', 'mlp2'):
+                        check(self.lib.s7b_engine_set_param(self._h, name.encode(), t, arr.ctypes.data, arr.size))
+                self._hvp_mlp = True
+            check(self.lib.s7b_engine_hvp(self._h, v.data_ptr(), out.data_ptr(), self._stream()))
+        return out
 
     def buffer(self, name: str, layer: int = 0, dtype: str = 'f4', shape=None):
         """Zero-copy torch view of an engine buffer (valid until the next set_graph)."""
