@@ -200,6 +200,20 @@ S7B_API int s7b_engine_compute(S7bEngine* eng, void* stream);
  * (n_local < n_nodes), or when an 'mlp' parameter is missing.  E == 0 zero-fills. */
 S7B_API int s7b_engine_hvp(S7bEngine* eng, const float* d_v, float* d_out, void* stream);
 
+/* The same product with a homogeneous strain in the tangent as well (elastic constants, DESIGN.md §8): along
+ * r -> (I + s eps_b) r + s v for the atoms and cell of every structure b, edge list fixed, each edge vector moves by
+ * eps_b . vec + v[neighbour] - v[centre].  Device pointers:
+ *   d_v       [n_nodes,3] f32, or NULL (no position tangent);
+ *   d_strain  [B,9] f64 (row-major general 3x3 per structure), or NULL (no strain);
+ *   d_out     [n_nodes,3] f32, overwritten with H v + Lambda eps, Lambda = d2E/dr de (eV/A);
+ *   d_dvirial [B,6] f64 or NULL, overwritten with the tangent of the virial W = -sum_e vec_e (x) dE/dvec_e per
+ *             structure, order (xx,yy,zz,xy,yz,zx) as s7b_engine_system_results, in fp64 and a fixed order.
+ * B = the structure count of a graph from s7b_engine_set_positions_batch, else 1.  Preconditions and refusals are
+ * those of s7b_engine_hvp; with d_strain NULL, d_out is what s7b_engine_hvp gives.  E == 0 (or no tangent)
+ * zero-fills. */
+S7B_API int s7b_engine_hvp_strain(S7bEngine* eng, const float* d_v, const double* d_strain, float* d_out,
+                                  double* d_dvirial, void* stream);
+
 /* Device pointer to an engine-owned buffer (valid until the next set_graph that grows it):
  * "x" (layer t input after self_interaction_1, [n_nodes, dim_x(t)]), "dx", "gate_in", "mid",
  * "h", "energy" (double[1]), "atomic_energy" [n_local], "atomic_energy_f64" (double[n_local], the same

@@ -19,7 +19,7 @@ from typing import List, Optional, Sequence
 
 import numpy as np
 
-from .engine import B200Engine
+from .engine import B200Engine, _host
 
 
 class BatchedEvaluator:
@@ -154,6 +154,49 @@ class DeviceBatch:
         ae = eng.buffer('atomic_energy', shape=(eng.n_local,)).clone()
         forces = eng.buffer('forces', shape=(eng.n_nodes, 3)).clone()
         return dict(energy=energy, atomic_energy=ae, forces=forces, virial=virial, n_edges=eng.n_edges)
+
+    def elastic_tensors(self, numbers, positions, cells, pbc, system_idx, relaxed: bool = True) -> np.ndarray:
+        """Elastic tensors of every structure, [B, 6, 6] float64 in eV/A^3 (``SevenNetCalculator.get_elastic_tensor``'s
+        definition, units and Voigt order, per structure; inputs as ``compute``).  Every structure must be periodic in
+        all three directions with a volume > 0.  C0 and Lambda of all structures come from six batched strain
+        products (``B200Engine.hvp_strain``).  The union graph has no edge between structures, so with ``relaxed``
+        every structure's Hessian comes from 3 max_b(n_b) more products: product k puts a unit tangent on direction
+        k % 3 of local atom k // 3 of every structure at once."""
+        from . import elastic
+        torch = self.engine.torch
+        c = torch.as_tensor(cells).detach().to('cpu', torch.float64).reshape(-1, 3, 3).numpy()
+        B = c.shape[0]
+        vol = np.abs(np.linalg.det(c))
+        pb = np.broadcast_to(np.asarray(_host(pbc), dtype=bool), (B, 3))
+        if not pb.all() or not (vol > 0).all():
+            raise ValueError('elastic tensors need every cell periodic in all three directions with a volume > 0')
+        self.set_batch(numbers, positions, c, pbc, system_idx)
+        eng = self.engine
+        eng.compute()
+        ap = np.asarray(self.atom_ptr, dtype=np.int64)
+        counts = np.diff(ap)
+        outs, dvir = [], []
+        for eps in elastic.voigt_strains():
+            o, d = eng.hvp_strain(None, np.repeat(eps[None], B, axis=0))
+            outs.append(o)
+            dvir.append(d)
+        outs = torch.stack(outs).double().cpu().numpy()            # [6, n, 3]
+        dvir = torch.stack(dvir).cpu().numpy()                     # [6, B, 6]
+        hess = [np.zeros((3 * int(m), 3 * int(m))) for m in counts] if relaxed else None
+        if relaxed and eng.n_nodes:
+            base = torch.as_tensor(ap[:-1], device=eng.device)
+            cnt = torch.as_tensor(counts, device=eng.device)
+            rows = []
+            for k in range(3 * int(counts.max())):
+                v = torch.zeros(eng.n_nodes, 3, dtype=torch.float32, device=eng.device)
+                v[base[cnt > k // 3] + k // 3, k % 3] = 1.0
+                rows.append(eng.hvp_strain(v, None)[0])
+            rows = torch.stack(rows).double().cpu().numpy()         # [3 max n_b, n, 3]
+            for b in range(B):
+                m = int(counts[b])
+                hess[b][:] = rows[:3 * m, ap[b]:ap[b + 1]].reshape(3 * m, 3 * m)
+        return np.stack([elastic.elastic_tensor(dvir[:, b], outs[:, ap[b]:ap[b + 1]], vol[b],
+                                                hess[b] if relaxed else None) for b in range(B)])
 
 
 class SevenNetModel:

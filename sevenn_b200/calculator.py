@@ -152,3 +152,36 @@ class SevenNetCalculator(_Base):
         if not rows:
             return np.zeros((0, 0))
         return torch.stack(rows).double().cpu().numpy()
+
+    def get_elastic_tensor(self, atoms=None, relaxed: bool = True) -> np.ndarray:
+        """Elastic tensor d2E/de de / V of ``atoms`` (default: the calculator's atoms), [6, 6] float64 in eV/A^3 (the
+        unit of ASE stress; ``/ ase.units.GPa`` gives GPa), ASE Voigt order (xx, yy, zz, yz, xz, xy), engineering
+        strains, V the volume of the unstrained cell.  From six strain products (``B200Engine.hvp_strain``) on the
+        calculator's own graph of the atoms, with that edge list held fixed.  ``relaxed=True`` gives the relaxed-ion
+        tensor C0 - Lambda^T H+ Lambda / V, which also takes the Hessian (``get_hessian``, 3N more products);
+        ``relaxed=False`` the clamped-ion tensor C0 (``sevenn_b200.elastic`` defines both).  This is the second
+        derivative of the energy: at a stress-free, force-free structure it is the elastic tensor; no pre-stress
+        correction is made and none is checked for.  All three directions must be periodic.  ``results`` and the other
+        ``get_*`` methods are not touched.  D3 dispersion has no second order here."""
+        from . import elastic
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        species, pos, cell, pbc, _ = self._inputs(atoms)
+        vol = abs(np.linalg.det(cell))
+        if not pbc.all() or not vol > 0:
+            raise ValueError('the elastic tensor needs a cell periodic in all three directions with a volume > 0')
+        if relaxed:
+            hessian = self.get_hessian(atoms)      # leaves the engine on the atoms' graph and forward
+        else:
+            hessian = None
+            self.engine.set_positions(species, pos, cell, pbc)
+            self.engine.compute()
+        outs, dvir = [], []
+        for eps in elastic.voigt_strains():
+            o, d = self.engine.hvp_strain(None, eps[None])
+            outs.append(o)
+            dvir.append(d[0])
+        torch = self.engine.torch
+        return elastic.elastic_tensor(torch.stack(dvir).cpu().numpy(), torch.stack(outs).double().cpu().numpy(), vol,
+                                      hessian)

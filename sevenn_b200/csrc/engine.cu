@@ -200,11 +200,12 @@ struct HvpBufs {
   DevBuf dvec, dr, dY, gY, dgY, ar, dar, fneg, virial;     // edge tangents, dE/dY and dE/dr with their tangents
   DevBuf emb3, hA, hB, w3, dw, aw, daw1, daw2;             // radial jets [3][E][.] of one layer; [E, W] weights
   DevBuf ah, dah, ag, dag, amid, damid, dmid, ax, dax, th;  // node adjoints and tangents of one layer
+  DevBuf atom_ptr1, sys_energy, dvir2;                    // virial tangent: {0, n} of a one-structure graph; scratch
   std::vector<DevBuf> tx, tg;                             // per layer: tangents of x[t] and g[t]
   RowExp re;
   void release() {
     for (DevBuf* b : {&dvec, &dr, &dY, &gY, &dgY, &ar, &dar, &fneg, &virial, &emb3, &hA, &hB, &w3, &dw, &aw, &daw1, &daw2,
-                      &ah, &dah, &ag, &dag, &amid, &damid, &dmid, &ax, &dax, &th, &re.buf})
+                      &ah, &dah, &ag, &dag, &amid, &damid, &dmid, &ax, &dax, &th, &atom_ptr1, &sys_energy, &dvir2, &re.buf})
       b->release();
     for (auto* v : {&tx, &tg})
       for (DevBuf& b : *v) b.release();
@@ -1789,7 +1790,8 @@ static int hvp_alloc(S7bEngine* e) {
   return rc ? fail("cudaMalloc failed for the Hessian-vector product's buffers") : 0;
 }
 
-static int hvp_pass(S7bEngine* e, const float* v, float* out, cudaStream_t st) {
+static int hvp_pass(S7bEngine* e, const float* v, const double* strain, const int* atom_ptr, int n_sys, float* out,
+                    cudaStream_t st) {
   const int T = e->desc.n_layers, LF = e->desc.lmax_filter, N = e->n_nodes;
   const int64_t E = e->n_edges;
   HvpBufs& hv = e->hv;
@@ -1797,9 +1799,9 @@ static int hvp_pass(S7bEngine* e, const float* v, float* out, cudaStream_t st) {
   // ---- edge tangents and the radial basis jet (layer independent)
   {
     const int grd = (N * 32 + 255) / 256;
-    if (LF == 1) hvp_edge_fwd_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
-    else if (LF == 2) hvp_edge_fwd_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
-    else hvp_edge_fwd_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    if (LF == 1) hvp_edge_fwd_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    else if (LF == 2) hvp_edge_fwd_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    else hvp_edge_fwd_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
     S7B_LAUNCH_CHECK();
     hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, hv.emb3.as<float>());
     S7B_LAUNCH_CHECK();
@@ -1882,21 +1884,64 @@ static int hvp_pass(S7bEngine* e, const float* v, float* out, cudaStream_t st) {
   return 0;
 }
 
-int s7b_engine_hvp(S7bEngine* e, const float* d_v, float* d_out, void* stream) {
+// The preconditions both entry points share; `who` names the caller in the messages.
+static int hvp_check(S7bEngine* e, const char* who) {
   if (!e) return fail("null engine");
-  if (!e->hvp_ready) return fail("s7b_engine_hvp needs an s7b_engine_compute on the current graph and parameters");
-  if (e->n_local < e->n_nodes) return fail("s7b_engine_hvp does not run on graphs with ghost atoms (n_local < n_nodes)");
+  if (!e->hvp_ready) return fail(std::string(who) + " needs an s7b_engine_compute on the current graph and parameters");
+  if (e->n_local < e->n_nodes) return fail(std::string(who) + " does not run on graphs with ghost atoms (n_local < n_nodes)");
   for (int t = 0; t < e->desc.n_layers; ++t)
     for (int j = 0; j < 3; ++j)
       if (!e->layer_params[t].mlp[j].p)
-        return fail("s7b_engine_hvp evaluates the radial MLP: parameter mlp" + std::to_string(j) + " of layer " + std::to_string(t) + " is missing");
+        return fail(std::string(who) + " evaluates the radial MLP: parameter mlp" + std::to_string(j) + " of layer " + std::to_string(t) + " is missing");
+  return 0;
+}
+
+int s7b_engine_hvp(S7bEngine* e, const float* d_v, float* d_out, void* stream) {
+  if (hvp_check(e, "s7b_engine_hvp")) return 1;
   if (e->n_nodes > 0 && (!d_v || !d_out)) return fail("null argument");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (e->n_nodes == 0) return 0;
   S7B_CUDA_CHECK(cudaMemsetAsync(d_out, 0, (size_t)e->n_nodes * 3 * sizeof(float), st));
   if (e->n_edges == 0) return 0;      // the energy does not depend on the positions
   if (hvp_alloc(e)) return 1;
-  return hvp_pass(e, d_v, d_out, st);
+  return hvp_pass(e, d_v, nullptr, nullptr, 1, d_out, st);
+}
+
+// The same pass with the strain tangent added to every edge's, and the virial's tangent per structure:
+// dW_b = -sum_e (dvec_e (x) f_e + vec_e (x) df_e) over structure b's edges = sums(dvec, f) - sums(vec, -df), both by
+// the batch's fixed-order per-structure reduction (deterministic).
+int s7b_engine_hvp_strain(S7bEngine* e, const float* d_v, const double* d_strain, float* d_out, double* d_dvirial,
+                          void* stream) {
+  if (hvp_check(e, "s7b_engine_hvp_strain")) return 1;
+  if (e->n_nodes > 0 && !d_out) return fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int B = std::max(e->n_systems, 1);
+  if (d_dvirial) S7B_CUDA_CHECK(cudaMemsetAsync(d_dvirial, 0, (size_t)B * 6 * sizeof(double), st));
+  if (e->n_nodes == 0) return 0;
+  S7B_CUDA_CHECK(cudaMemsetAsync(d_out, 0, (size_t)e->n_nodes * 3 * sizeof(float), st));
+  if (e->n_edges == 0 || (!d_v && !d_strain)) return 0;
+  if (hvp_alloc(e)) return 1;
+  HvpBufs& hv = e->hv;
+  const int* atom_ptr = e->sys_atom_ptr.as<int>();
+  if (e->n_systems < 1) {
+    const int one[2] = {0, e->n_nodes};
+    if (hv.atom_ptr1.ensure(2 * sizeof(int))) return fail("cudaMalloc failed for the Hessian-vector product's buffers");
+    S7B_CUDA_CHECK(cudaMemcpyAsync(hv.atom_ptr1.p, one, sizeof(one), cudaMemcpyHostToDevice, st));
+    atom_ptr = hv.atom_ptr1.as<int>();
+  }
+  if (hvp_pass(e, d_v, d_strain, atom_ptr, B, d_out, st)) return 1;
+  if (!d_dvirial) return 0;
+  if (hv.sys_energy.ensure((size_t)B * sizeof(double)) || hv.dvir2.ensure((size_t)B * 6 * sizeof(double)))
+    return fail("cudaMalloc failed for the Hessian-vector product's buffers");
+  system_sums_kernel<<<B, kSysBlock, 0, st>>>(atom_ptr, e->d_rowptr, e->atomic_energy64.as<double>(), hv.dvec.as<float>(),
+                                              e->fedge.as<float>(), hv.sys_energy.as<double>(), d_dvirial);
+  S7B_LAUNCH_CHECK();
+  system_sums_kernel<<<B, kSysBlock, 0, st>>>(atom_ptr, e->d_rowptr, e->atomic_energy64.as<double>(), e->d_edge_vec,
+                                              hv.fneg.as<float>(), hv.sys_energy.as<double>(), hv.dvir2.as<double>());
+  S7B_LAUNCH_CHECK();
+  hvp_sub_kernel<<<(6 * B + 255) / 256, 256, 0, st>>>(d_dvirial, hv.dvir2.as<double>(), 6 * B);
+  S7B_LAUNCH_CHECK();
+  return 0;
 }
 
 int s7b_engine_graph_stats(S7bEngine* e, int64_t* captures, int64_t* replays) {

@@ -9,21 +9,28 @@
 
 namespace s7b {
 
-// One warp per centre atom, lanes over its CSR row: dvec[e] = v[src] - v[centre], dr[e] = u . dvec and the tangent
-// of the harmonics dY[e, 0..ny_stride) (Y_1.., the layout of the step's Y).
+// One warp per centre atom, lanes over its CSR row: dvec[e] = v[src] - v[centre] + strain[b] . edge_vec[e], dr[e] =
+// u . dvec and the tangent of the harmonics dY[e, 0..ny_stride) (Y_1.., the layout of the step's Y).  v null: no
+// position tangent.  strain null: no strain tangent; else [n_sys][3][3] fp64, b the centre's structure in atom_ptr
+// [n_sys + 1] (edges never join two structures).
 template <int LMAX>
 __global__ void hvp_edge_fwd_kernel(const int* __restrict__ rowptr, const int* __restrict__ src,
-                                    const float* __restrict__ edge_vec, const float* __restrict__ v, int n_dst,
-                                    int ny_stride, float* __restrict__ dvec, float* __restrict__ dr,
+                                    const float* __restrict__ edge_vec, const float* __restrict__ v,
+                                    const double* __restrict__ strain, const int* __restrict__ atom_ptr, int n_sys,
+                                    int n_dst, int ny_stride, float* __restrict__ dvec, float* __restrict__ dr,
                                     float* __restrict__ dY) {
   const int n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (n >= n_dst) return;
-  const float vc[3] = {v[3 * (size_t)n], v[3 * (size_t)n + 1], v[3 * (size_t)n + 2]};
+  const double* eps = strain ? strain + 9 * (size_t)structure_of(atom_ptr, n_sys, n) : nullptr;
+  float vc[3] = {0.0f, 0.0f, 0.0f};
+  if (v) for (int c = 0; c < 3; ++c) vc[c] = v[3 * (size_t)n + c];
   for (int e = rowptr[n] + lane; e < rowptr[n + 1]; e += 32) {
     const int s = src[e];
     const float ev[3] = {edge_vec[3 * (size_t)e], edge_vec[3 * (size_t)e + 1], edge_vec[3 * (size_t)e + 2]};
-    const float dv[3] = {v[3 * (size_t)s] - vc[0], v[3 * (size_t)s + 1] - vc[1], v[3 * (size_t)s + 2] - vc[2]};
+    float dv[3] = {0.0f, 0.0f, 0.0f};
+    if (v) for (int c = 0; c < 3; ++c) dv[c] = v[3 * (size_t)s + c] - vc[c];
+    if (eps) add_strain_tangent(eps, ev, dv);
     float t[SH<LMAX>::NY], d;
     edge_tangent<LMAX>(ev, dv, d, t);
     for (int c = 0; c < 3; ++c) dvec[3 * (size_t)e + c] = dv[c];
@@ -197,6 +204,12 @@ __global__ void hvp_edge_bwd_kernel(const float* __restrict__ edge_vec, const fl
   float df[3];
   edge_bwd_tangent<LMAX>(v, dv, gY, dgY, ar[e], dar[e], df);
   for (int c = 0; c < 3; ++c) out[3 * e + c] = -df[c];
+}
+
+// a[i] -= b[i]
+__global__ void hvp_sub_kernel(double* __restrict__ a, const double* __restrict__ b, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) a[i] -= b[i];
 }
 
 }  // namespace s7b

@@ -79,6 +79,25 @@ S7B_HD void edge_tangent(const float v[3], const float dv[3], float& dr, float* 
   SH2<LMAX>::jvp(u[0], u[1], u[2], du[0], du[1], du[2], dY);
 }
 
+// Structure of atom n in a batch whose structure b owns atoms [atom_ptr[b], atom_ptr[b+1]) (n < atom_ptr[n_sys]):
+// the largest b with atom_ptr[b] <= n, so empty structures are skipped.
+S7B_HD int structure_of(const int* atom_ptr, int n_sys, int n) {
+  int lo = 0, hi = n_sys;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (atom_ptr[mid] <= n) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// dv += eps . v: the tangent of the edge vector under the homogeneous deformation r -> (I + s eps) r of atoms and
+// cell (eps row-major 3x3, applied in fp64).
+S7B_HD void add_strain_tangent(const double* eps, const float v[3], float dv[3]) {
+  for (int a = 0; a < 3; ++a)
+    dv[a] += (float)(eps[3 * a] * v[0] + eps[3 * a + 1] * v[1] + eps[3 * a + 2] * v[2]);
+}
+
 // Tangent of edge_bwd_kernel's f = ar u + (I - u u^T) J_Y^T gY / r along dv, given the tangents dgY of gY and dar
 // of ar (gY[0], dgY[0] unused).  Writes df.
 template <int LMAX>

@@ -66,7 +66,7 @@ EXPORTS = [
     's7b_conv_double_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
-    's7b_engine_hvp',
+    's7b_engine_hvp', 's7b_engine_hvp_strain',
 ]
 
 
@@ -116,6 +116,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_run_stage.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]
     lib.s7b_engine_compute.argtypes = [vp, vp]
     lib.s7b_engine_hvp.argtypes = [vp, vp, vp, vp]
+    lib.s7b_engine_hvp_strain.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.s7b_engine_buffer.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(sz)]
     lib.s7b_engine_buffer.restype = vp
     lib.s7b_engine_compute_host.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -610,13 +611,45 @@ class B200Engine:
         v = torch.as_tensor(v).to(self.device, torch.float32).contiguous().reshape(self.n_nodes, 3)
         out = torch.empty(self.n_nodes, 3, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            if not self._hvp_mlp:
-                for (name, t), arr in prepare_params(self.spec, self._arrays, 'mlp', 0).items():
-                    if name in ('mlp0', 'mlp1', 'mlp2'):
-                        check(self.lib.s7b_engine_set_param(self._h, name.encode(), t, arr.ctypes.data, arr.size))
-                self._hvp_mlp = True
+            self._upload_hvp_mlp()
             check(self.lib.s7b_engine_hvp(self._h, v.data_ptr(), out.data_ptr(), self._stream()))
         return out
+
+    def _upload_hvp_mlp(self):
+        if not self._hvp_mlp:
+            for (name, t), arr in prepare_params(self.spec, self._arrays, 'mlp', 0).items():
+                if name in ('mlp0', 'mlp1', 'mlp2'):
+                    check(self.lib.s7b_engine_set_param(self._h, name.encode(), t, arr.ctypes.data, arr.size))
+            self._hvp_mlp = True
+
+    def hvp_strain(self, v=None, strain=None):
+        """Second derivatives along positions and a homogeneous strain together (C ABI ``s7b_engine_hvp_strain``):
+        along r -> (I + s eps_b) r + s v for the atoms and cell of every structure b, on the graph and forward of the
+        last ``compute`` with its edge list held fixed.  v [n_nodes, 3] or None (zero); strain [B, 3, 3] (general
+        3x3, applied as eps . r) or None (zero), B = the structure count of a ``set_positions_batch`` graph, else 1.
+        numpy or torch (any device).  Returns (H v + Lambda eps [n_nodes, 3] float32 in eV/A^2 resp. eV/A, Lambda =
+        d2E/dr de; dW [B, 6] float64, the tangent of the virial W = -sum_e vec_e (x) dE/dvec_e per structure, order
+        xx,yy,zz,xy,yz,zx, in eV), device tensors.  ``hvp(v)`` equals ``hvp_strain(v)[0]``.  Uploads the radial MLP
+        of a table-mode engine on first use, as ``hvp``."""
+        torch = self.torch
+        n = self.n_nodes
+        B = max((self._graph or {}).get('n_systems', 0), 1)
+        if v is not None:
+            v = torch.as_tensor(v).to(self.device, torch.float32).contiguous()
+            if v.numel() != 3 * n:
+                raise ValueError(f'v has {tuple(v.shape)}, expected [{n}, 3] (n_nodes)')
+        if strain is not None:
+            strain = torch.as_tensor(strain).to(self.device, torch.float64).contiguous()
+            if strain.numel() != 9 * B:
+                raise ValueError(f'strain has {tuple(strain.shape)}, expected [{B}, 3, 3] (one per structure)')
+        out = torch.empty(n, 3, dtype=torch.float32, device=self.device)
+        dvir = torch.empty(B, 6, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._upload_hvp_mlp()
+            check(self.lib.s7b_engine_hvp_strain(self._h, None if v is None else v.data_ptr(),
+                                                 None if strain is None else strain.data_ptr(), out.data_ptr(),
+                                                 dvir.data_ptr(), self._stream()))
+        return out, dvir
 
     def buffer(self, name: str, layer: int = 0, dtype: str = 'f4', shape=None):
         """Zero-copy torch view of an engine buffer (valid until the next set_graph)."""
