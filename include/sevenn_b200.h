@@ -396,6 +396,18 @@ S7B_API int s7b_d3_set_system_batch(S7bD3* d3, int32_t n_systems, const int32_t*
  * device pointers, no synchronisation.  Per-structure sums in a fixed order: deterministic, and independent of the
  * other structures of the batch. */
 S7B_API int s7b_d3_system_results(S7bD3* d3, double* d_energy, double* d_forces, double* d_virial, void* stream);
+/* Second derivatives of the D3 energy of the current system (one structure or a batch) along
+ * r -> (I + s eps_b) r + s v for the atoms and cell of every structure b, with the forward of the last three stages
+ * held.  d_v: device double [n,3] (Angstrom, caller's atom order) or NULL (zero); d_strain: device double [B,3,3]
+ * (general 3x3, applied as eps . r) or NULL (zero).  d_out: device double [n,3], H v + Lambda eps in eV/A^2 x A resp.
+ * eV/A (Lambda = d2E/dr de), caller's atom order; d_dvirial: device double [B,6] or NULL, the tangent of the virial in
+ * eV (xx,yy,zz,xy,yz,zx: the order and sign of s7b_engine_hvp_strain's, so the two add).  Refused unless stages 1, 2
+ * and 3 ran, in that order, over all atoms [0, n) since the last set_system[_batch], set_params, set_element_tables
+ * or set_damping.  With no atoms or no tangent the outputs are zero-filled.  Scratch buffers are allocated on the
+ * first call and kept; no forward buffer is written, so the results of the stages read afterwards are unchanged.
+ * Per-structure sums in a fixed order: deterministic, and independent of the other structures of the batch. */
+S7B_API int s7b_d3_hvp_strain(S7bD3* d3, const double* d_v, const double* d_strain, double* d_out, double* d_dvirial,
+                              void* stream);
 
 /* The reference's own D3 entry points (pair_d3_for_ase.cu:2034-2082; ctypes signatures sevenn/calculator.py:430-483),
  * same names / arguments / call order, so its D3Calculator can load this library in place of pair_d3.so.

@@ -155,13 +155,15 @@ class DeviceBatch:
         forces = eng.buffer('forces', shape=(eng.n_nodes, 3)).clone()
         return dict(energy=energy, atomic_energy=ae, forces=forces, virial=virial, n_edges=eng.n_edges)
 
-    def elastic_tensors(self, numbers, positions, cells, pbc, system_idx, relaxed: bool = True) -> np.ndarray:
+    def elastic_tensors(self, numbers, positions, cells, pbc, system_idx, relaxed: bool = True, d3=None) -> np.ndarray:
         """Elastic tensors of every structure, [B, 6, 6] float64 in eV/A^3 (``SevenNetCalculator.get_elastic_tensor``'s
         definition, units and Voigt order, per structure; inputs as ``compute``).  Every structure must be periodic in
         all three directions with a volume > 0.  C0 and Lambda of all structures come from six batched strain
         products (``B200Engine.hvp_strain``).  The union graph has no edge between structures, so with ``relaxed``
         every structure's Hessian comes from 3 max_b(n_b) more products: product k puts a unit tangent on direction
-        k % 3 of local atom k // 3 of every structure at once."""
+        k % 3 of local atom k // 3 of every structure at once.  ``d3`` (a ``d3.D3Batch``) adds D3 dispersion: its
+        strain products and Hessian blocks, from the same tangents (D3 has no pair between structures either), are
+        added to the network's before each structure's tensor is assembled."""
         from . import elastic
         torch = self.engine.torch
         c = torch.as_tensor(cells).detach().to('cpu', torch.float64).reshape(-1, 3, 3).numpy()
@@ -175,9 +177,14 @@ class DeviceBatch:
         eng.compute()
         ap = np.asarray(self.atom_ptr, dtype=np.int64)
         counts = np.diff(ap)
+        if d3 is not None:
+            d3.compute(numbers, positions, c, pbc, atom_ptr=ap)
         outs, dvir = [], []
         for eps in elastic.voigt_strains():
             o, d = eng.hvp_strain(None, np.repeat(eps[None], B, axis=0))
+            if d3 is not None:
+                o3, d3v = d3.hvp_strain(None, np.repeat(eps[None], B, axis=0))
+                o, d = o.double() + o3, d + d3v
             outs.append(o)
             dvir.append(d)
         outs = torch.stack(outs).double().cpu().numpy()            # [6, n, 3]
@@ -190,7 +197,8 @@ class DeviceBatch:
             for k in range(3 * int(counts.max())):
                 v = torch.zeros(eng.n_nodes, 3, dtype=torch.float32, device=eng.device)
                 v[base[cnt > k // 3] + k // 3, k % 3] = 1.0
-                rows.append(eng.hvp_strain(v, None)[0])
+                row = eng.hvp_strain(v, None)[0]
+                rows.append(row if d3 is None else row.double() + d3.hvp_strain(v, None)[0])
             rows = torch.stack(rows).double().cpu().numpy()         # [3 max n_b, n, 3]
             for b in range(B):
                 m = int(counts[b])
@@ -289,3 +297,9 @@ class SevenNetD3Model(SevenNetModel):
                 'forces': (out['forces'].double() + d3['forces']).to(self._dtype), 'stress': stress.to(self._dtype)}
 
     __call__ = forward
+
+    def elastic_tensors(self, state, relaxed: bool = True) -> np.ndarray:
+        """Elastic tensors of the network plus D3 energy of every structure of the state, [B, 6, 6] float64 in eV/A^3
+        (``DeviceBatch.elastic_tensors`` with this model's ``D3Batch``)."""
+        return self._batch.elastic_tensors(state.atomic_numbers, state.positions, self._cells(state), state.pbc,
+                                           state.system_idx, relaxed, d3=self.d3)

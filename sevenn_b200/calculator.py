@@ -138,7 +138,7 @@ class SevenNetCalculator(_Base):
         atoms, with that edge list held fixed, so a periodic cell gives the Gamma-point (supercell) Hessian that
         phonon codes take force constants from.  Not symmetrised (the two triangles agree to the fp32 error of the
         products); ``.reshape(N, 3, N, 3)`` gives the force constants Phi[i, a, j, b].  ``results`` and the other
-        ``get_*`` methods are not touched.  D3 dispersion has no second order here."""
+        ``get_*`` methods are not touched.  ``SevenNetD3Calculator.get_hessian`` adds D3 dispersion's."""
         atoms = atoms if atoms is not None else self.atoms
         if atoms is None:
             raise ValueError('No atoms to evaluate')
@@ -162,11 +162,17 @@ class SevenNetCalculator(_Base):
         ``relaxed=False`` the clamped-ion tensor C0 (``sevenn_b200.elastic`` defines both).  This is the second
         derivative of the energy: at a stress-free, force-free structure it is the elastic tensor; no pre-stress
         correction is made and none is checked for.  All three directions must be periodic.  ``results`` and the other
-        ``get_*`` methods are not touched.  D3 dispersion has no second order here."""
+        ``get_*`` methods are not touched.  ``SevenNetD3Calculator.get_elastic_tensor`` adds D3 dispersion's."""
         from . import elastic
         atoms = atoms if atoms is not None else self.atoms
         if atoms is None:
             raise ValueError('No atoms to evaluate')
+        return elastic.elastic_tensor(*self._strain_pieces(atoms, relaxed))
+
+    def _strain_pieces(self, atoms, relaxed: bool):
+        """The raw second derivatives ``elastic.elastic_tensor`` assembles: (dvirial [6, 6], outs [6, N, 3], volume,
+        Hessian [3N, 3N] or None), from the six Voigt strain products and, when ``relaxed``, the Hessian."""
+        from . import elastic
         species, pos, cell, pbc, _ = self._inputs(atoms)
         vol = abs(np.linalg.det(cell))
         if not pbc.all() or not vol > 0:
@@ -183,5 +189,4 @@ class SevenNetCalculator(_Base):
             outs.append(o)
             dvir.append(d[0])
         torch = self.engine.torch
-        return elastic.elastic_tensor(torch.stack(dvir).cpu().numpy(), torch.stack(outs).double().cpu().numpy(), vol,
-                                      hessian)
+        return torch.stack(dvir).cpu().numpy(), torch.stack(outs).double().cpu().numpy(), vol, hessian

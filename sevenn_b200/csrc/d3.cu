@@ -1,7 +1,7 @@
 // Host side of the D3 dispersion C ABI (include/sevenn_b200.h, "D3" section): parameters, cell list, the set-up of
 // one structure (host arrays) or of a batch (device arrays, s7b_d3_set_system_batch), stage launches, per-structure
-// results and the reference-named entry points (pair_init ... pair_fin) that sevenn/calculator.py:430-483 binds with
-// ctypes.  Kernels: d3_kernels.cuh.
+// results, the Hessian-vector product (s7b_d3_hvp_strain) and the reference-named entry points (pair_init ... pair_fin)
+// that sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh, d3_hvp_kernels.cuh.
 #include <dlfcn.h>
 
 #include <algorithm>
@@ -15,6 +15,7 @@
 
 #include "../../include/sevenn_b200.h"
 #include "common.cuh"
+#include "d3_hvp_kernels.cuh"
 #include "d3_kernels.cuh"
 
 namespace s7b {
@@ -56,6 +57,11 @@ struct S7bD3 {
   // the current system; grids / aptr / lrows / nloc are swapped in from their st_ scratch once the checks have passed
   D3Buf grids, aptr, lrows, nloc, bin_off, rtab, idx_sorted, bin_start;
   D3Buf xs, ts, ss, bin_of, W, dW, logD, near_, cn, dc6i, force, eatom, spair, schain, energy, sigma, out_force;
+  // stages run in sequence over all atoms [0, n) since the current system and tables were set (0..3): the
+  // Hessian-vector product reads cn, W, dW and dc6i of all atoms and needs 3
+  int stages_done = 0;
+  // Hessian-vector product scratch, allocated on its first call
+  D3Buf hv_v, hv_dcn, hv_dWt, hv_dW1t, hv_ddc, hv_force, hv_spair, hv_schain, hv_sigma, hv_energy, hv_oute, hv_dvir;
   std::vector<double> host_force;      // reference ABI: pair_get_force returns a pointer
   double host_energy = 0.0, host_sigma[6] = {0, 0, 0, 0, 0, 0};
   // reference-ABI staging (pair_set_atom / pair_set_domain / pair_run_settings / pair_run_coeff)
@@ -133,7 +139,9 @@ void s7b_d3_destroy(S7bD3* d) {
                    &d->present, &d->lrank, &d->err, &d->st_grids, &d->st_aptr, &d->st_lrows, &d->st_nloc,
                    &d->grids, &d->aptr, &d->lrows, &d->nloc, &d->bin_off, &d->rtab, &d->idx_sorted, &d->bin_start,
                    &d->xs, &d->ts, &d->ss, &d->bin_of, &d->W, &d->dW, &d->logD, &d->near_, &d->cn, &d->dc6i,
-                   &d->force, &d->eatom, &d->spair, &d->schain, &d->energy, &d->sigma, &d->out_force};
+                   &d->force, &d->eatom, &d->spair, &d->schain, &d->energy, &d->sigma, &d->out_force,
+                   &d->hv_v, &d->hv_dcn, &d->hv_dWt, &d->hv_dW1t, &d->hv_ddc, &d->hv_force, &d->hv_spair,
+                   &d->hv_schain, &d->hv_sigma, &d->hv_energy, &d->hv_oute, &d->hv_dvir};
   for (D3Buf* b : bufs) b->release();
   delete d;
 }
@@ -144,6 +152,7 @@ int s7b_d3_set_params(S7bD3* d, int32_t ntypes, const double* rcov, const double
   if (ntypes < 1 || ntypes > kD3MaxTypes) return d3_fail("D3: 1.." + std::to_string(kD3MaxTypes) + " atom types are supported");
   if (d3_upload_tables(d->P, ntypes, rcov, r2r4, r0ab, c6ref, cnref, mxc, d->r0ab, d->c6ref, d->cnref, d->mxc)) return 1;
   d->have_params = true;
+  d->stages_done = 0;
   return 0;
 }
 
@@ -153,6 +162,7 @@ int s7b_d3_set_element_tables(S7bD3* d, const double* rcov, const double* r2r4, 
   if (d3_upload_tables(d->Pe, kD3Elements, rcov, r2r4, r0ab, c6ref, cnref, mxc, d->el_r0ab, d->el_c6ref, d->el_cnref, d->el_mxc))
     return 1;
   d->have_elements = true;
+  d->stages_done = 0;
   return 0;
 }
 
@@ -169,6 +179,7 @@ int s7b_d3_set_damping(S7bD3* d, int32_t damping, double s6, double s8, double a
     P->cnthr = (double)(float)cn_cutoff_au2;
   }
   d->have_damping = true;
+  d->stages_done = 0;
   return 0;
 }
 
@@ -262,6 +273,7 @@ static int d3_setup(S7bD3* d, int B, const int32_t* atom_ptr, const std::vector<
   std::swap(d->lrows, d->st_lrows);
   std::swap(d->nloc, d->st_nloc);
   d->have_system = false;
+  d->stages_done = 0;
   rc = 0;
   rc |= d->bin_off.ensure((Bs + 1) * 4); rc |= d->rtab.ensure(Bs * 24); rc |= d->idx_sorted.ensure(N * 4);
   rc |= d->bin_start.ensure(((size_t)nbins + 1) * 4);
@@ -378,6 +390,7 @@ int s7b_d3_run_stage(S7bD3* d, int32_t stage, int32_t i_begin, int32_t i_end, vo
     return d3_fail("D3: unknown stage");
   }
   S7B_CUDA_CHECK(cudaGetLastError());
+  d->stages_done = (i_begin == 0 && i_end == n && stage <= d->stages_done + 1) ? stage : 0;
   return 0;
 }
 
@@ -434,6 +447,69 @@ int s7b_d3_system_results(S7bD3* d, double* d_energy, double* d_forces, double* 
   const int threads = std::max(3 * d->n, d->B);
   d3_system_results_kernel<<<(threads + 255) / 256, 256, 0, st>>>(d->n, d->B, d->idx_sorted.as<int>(), d->force.as<double>(),
                                                                   d->energy.as<double>(), d->sigma.as<double>(), d_energy, d_forces, d_virial);
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// Along r -> (I + s eps_b) r + s v for the atoms and cell of every structure b, on the current system with its
+// forward (stages 1-3 over [0, n)) held: out = H v + Lambda eps (eV/A^2 x A resp. eV/A, caller's atom order) and the
+// virial's tangent [B, 6] (eV; xx,yy,zz,xy,yz,zx, the order and sign of s7b_engine_hvp_strain's).  Launches the four
+// tangent passes and the forward's own sums and results kernels on scratch; no forward buffer is written.
+int s7b_d3_hvp_strain(S7bD3* d, const double* d_v, const double* d_strain, double* d_out, double* d_dvirial, void* stream) {
+  if (!d || !d->have_system) return d3_fail("D3: no system set");
+  if (d->stages_done < 3)
+    return d3_fail("D3: the Hessian-vector product needs stages 1, 2 and 3 run over all atoms [0, n) of the current "
+                   "system first");
+  const int n = d->n, B = d->B;
+  if (n > 0 && !d_out) return d3_fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (d_dvirial) S7B_CUDA_CHECK(cudaMemsetAsync(d_dvirial, 0, (size_t)B * 48, st));
+  if (n == 0) return 0;
+  if (!d_v && !d_strain) {
+    S7B_CUDA_CHECK(cudaMemsetAsync(d_out, 0, (size_t)n * 24, st));
+    return 0;
+  }
+  const size_t N = (size_t)n, Bs = (size_t)B;
+  int rc = 0;
+  rc |= d->hv_v.ensure(N * 24); rc |= d->hv_dcn.ensure(N * 8); rc |= d->hv_dWt.ensure(N * 20); rc |= d->hv_dW1t.ensure(N * 20);
+  rc |= d->hv_ddc.ensure(N * 8); rc |= d->hv_force.ensure(N * 24); rc |= d->hv_spair.ensure(N * 48);
+  rc |= d->hv_schain.ensure(N * 48); rc |= d->hv_sigma.ensure(Bs * 48); rc |= d->hv_energy.ensure(Bs * 8);
+  rc |= d->hv_oute.ensure(Bs * 8); rc |= d->hv_dvir.ensure(Bs * 48);
+  if (rc) return d3_fail("cudaMalloc failed for the D3 Hessian-vector product");
+  const bool bt = d->batched;
+  const D3Params& P = bt ? d->Pe : d->P;
+  const D3Atoms A = d3_atoms(d);
+  D3Hvp H;
+  H.v = d->hv_v.as<double>();
+  H.strain = d_strain;
+  H.dcn = d->hv_dcn.as<double>();
+  H.dWt = d->hv_dWt.as<float>();
+  H.dW1t = d->hv_dW1t.as<float>();
+  H.ddc = d->hv_ddc.as<double>();
+  H.hforce = d->hv_force.as<double>();
+  H.spair = d->hv_spair.as<double>();
+  H.schain = d->hv_schain.as<double>();
+  const int grd = (n + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
+  d3_hvp_gather_kernel<<<(3 * n + 255) / 256, 256, 0, st>>>(n, d->idx_sorted.as<int>(), d_v, d->hv_v.as<double>());
+  if (bt) d3_hvp_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, H);
+  else d3_hvp_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, H);
+  d3_hvp_weights_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, d->ts.as<int>(), d->cn.as<double>(),
+                                                        (bt ? d->el_cnref : d->cnref).as<float>(),
+                                                        (bt ? d->el_mxc : d->mxc).as<int>(), H.dcn, H.dWt, H.dW1t);
+  if (bt) d3_hvp_pair_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, H);
+  else d3_hvp_pair_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, H);
+  if (bt) d3_hvp_chain_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, H);
+  else d3_hvp_chain_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, H);
+  // per-structure virial tangent (the pair sum sets it, the chain sum adds; dcn stands in for the energy terms)
+  d3_system_sums_kernel<<<B, kD3SumBlock, 0, st>>>(d->aptr.as<int>(), 0, n, H.dcn, H.spair, d->hv_energy.as<double>(),
+                                                   d->hv_sigma.as<double>());
+  d3_system_sums_kernel<<<B, kD3SumBlock, 0, st>>>(d->aptr.as<int>(), 0, n, nullptr, H.schain, d->hv_energy.as<double>(),
+                                                   d->hv_sigma.as<double>());
+  const int threads = std::max(3 * n, B);
+  d3_system_results_kernel<<<(threads + 255) / 256, 256, 0, st>>>(n, B, d->idx_sorted.as<int>(), H.hforce,
+                                                                  d->hv_energy.as<double>(), d->hv_sigma.as<double>(),
+                                                                  d->hv_oute.as<double>(), d_out,
+                                                                  d_dvirial ? d_dvirial : d->hv_dvir.as<double>());
   S7B_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

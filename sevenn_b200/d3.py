@@ -60,7 +60,7 @@ class D3Engine:
         with torch.cuda.device(self.device):
             check(self.lib.s7b_d3_create(ctypes.byref(self._h)))
         self._numbers = None
-        self.n = 0
+        self.n, self.B = 0, 1
 
     def __del__(self):
         try:
@@ -98,7 +98,7 @@ class D3Engine:
         pos = np.ascontiguousarray(positions, dtype=np.float64).reshape(-1, 3)
         c = np.ascontiguousarray(cell, dtype=np.float64).reshape(3, 3)
         pb = np.ascontiguousarray(np.broadcast_to(np.asarray(pbc, dtype=bool), (3,)).astype(np.int32))
-        self.n = len(types)
+        self.n, self.B = len(types), 1
         with self.torch.cuda.device(self.device):
             check(self.lib.s7b_d3_set_system(self._h, self.n, types.ctypes.data, pos.ctypes.data, c.ctypes.data, pb.ctypes.data, self._stream()))
         return self
@@ -127,6 +127,36 @@ class D3Engine:
         for stage in (1, 2, 3):
             self.run_stage(stage)
         return self.results()
+
+    def hvp_strain(self, v=None, strain=None):
+        """Second derivatives of the D3 energy along positions and a homogeneous strain together (C ABI
+        ``s7b_d3_hvp_strain``): along r -> (I + s eps_b) r + s v for the atoms and cell of every structure b, with the
+        forward of the last three stages over all atoms held.  v [n, 3] (Angstrom, caller's atom order) or None
+        (zero); strain [B, 3, 3] (general 3x3, applied as eps . r) or None (zero), B = the structure count of the last
+        ``D3Batch.compute``, else 1; numpy or torch (any device).  Returns (H v + Lambda eps [n, 3] in eV/A^2 x A resp.
+        eV/A, Lambda = d2E/dr de; dW [B, 6], the tangent of the virial in eV, order xx,yy,zz,xy,yz,zx, the order and
+        sign of ``B200Engine.hvp_strain``'s), float64 device tensors."""
+        torch = self.torch
+        n, B = self.n, self.B
+        if v is not None:
+            v = torch.as_tensor(v).to(self.device, torch.float64).contiguous()
+            if v.numel() != 3 * n:
+                raise ValueError(f'v has {tuple(v.shape)}, expected [{n}, 3] (atoms)')
+        if strain is not None:
+            strain = torch.as_tensor(strain).to(self.device, torch.float64).contiguous()
+            if strain.numel() != 9 * B:
+                raise ValueError(f'strain has {tuple(strain.shape)}, expected [{B}, 3, 3] (one per structure)')
+        out = torch.empty(n, 3, dtype=torch.float64, device=self.device)
+        dvir = torch.empty(B, 6, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self.lib.s7b_d3_hvp_strain(self._h, None if v is None else v.data_ptr(),
+                                             None if strain is None else strain.data_ptr(), out.data_ptr(),
+                                             dvir.data_ptr(), self._stream()))
+        return out, dvir
+
+    def hvp(self, v):
+        """H v = (d2E/dr dr) v of the D3 energy, [n, 3] float64 device tensor in eV/A^2 x A: ``hvp_strain(v)[0]``."""
+        return self.hvp_strain(v)[0]
 
 
 def distributed_d3(engine: D3Engine, numbers, positions, cell, pbc=(True, True, True), group=None):
@@ -231,7 +261,7 @@ class D3Batch:
         with self.torch.cuda.device(self.device):
             check(eng.lib.s7b_d3_set_element_tables(eng._h, *[a.ctypes.data for a in self._tables]))
             eng._set_damping()
-        self.cells = self.pbc = None
+        self.cells = self.pbc = self.atom_ptr = None
 
     def compute(self, numbers, positions, cells, pbc, system_idx=None, atom_ptr=None) -> dict:
         """numbers [n] atomic numbers, positions [n,3] (Angstrom, float32 or float64), cells [B,3,3] (rows), pbc
@@ -251,11 +281,20 @@ class D3Batch:
             st = eng._stream()
             check(eng.lib.s7b_d3_set_system_batch(eng._h, B, ap.ctypes.data, z.data_ptr(), pos.data_ptr(), cc.ctypes.data,
                                                   pb.ctypes.data, st))
-            eng.n = n
+            eng.n, eng.B = n, B
+            self.atom_ptr = ap
             for stage in (1, 2, 3):
                 check(eng.lib.s7b_d3_run_stage(eng._h, stage, 0, n, st))
             check(eng.lib.s7b_d3_system_results(eng._h, energy.data_ptr(), forces.data_ptr(), virial.data_ptr(), st))
         return dict(energy=energy, forces=forces, virial=virial)
+
+    def hvp_strain(self, v=None, strain=None):
+        """``D3Engine.hvp_strain`` on the last batch: v [n, 3] (Angstrom) or None, strain [B, 3, 3] (one per
+        structure of ``atom_ptr``) or None -> (out [n, 3], dW [B, 6]), float64 device tensors.  D3 has no pair between
+        the structures of a batch, so each structure's products are those of the structure alone."""
+        if self.atom_ptr is None:
+            raise RuntimeError('no batch: call compute first')
+        return self.engine.hvp_strain(v, strain)
 
 
 try:
@@ -285,25 +324,90 @@ class D3Calculator(_Base):
         self.rthr, self.cnthr = vdw_cutoff, cn_cutoff
         self.engine = D3Engine(damping_type, functional_name, vdw_cutoff, cn_cutoff, device=device)
 
+    def _inputs(self, atoms):
+        """(numbers, positions, cell, pbc, generated) that ``calculate`` evaluates ``atoms`` with; a structure without
+        a cell gets an orthogonal cell large enough, periodic (``generated``), and ``atoms`` is not modified."""
+        cell = np.asarray(atoms.get_cell(), dtype=np.float64).reshape(3, 3)
+        pbc = np.asarray(atoms.get_pbc(), dtype=bool)
+        pos = np.asarray(atoms.get_positions(), dtype=np.float64)
+        generated = cell.sum() == 0      # calculator.py:534-547: periodic "for minus positions"
+        if generated:
+            max_cutoff = np.sqrt(max(self.rthr, self.cnthr)) * AU_TO_ANG
+            cell = np.eye(3) * (pos.max(axis=0) - pos.min(axis=0) + max_cutoff + 1.0)
+            pbc = np.array([True, True, True])
+        return np.asarray(atoms.get_atomic_numbers()), pos, cell, pbc, generated
+
     def calculate(self, atoms=None, properties=None, system_changes=_all_changes):
         super().calculate(atoms, properties, system_changes)
         if atoms is None:
             raise ValueError('No atoms to evaluate')
-        cell = np.asarray(atoms.get_cell(), dtype=np.float64).reshape(3, 3)
-        pbc = np.asarray(atoms.get_pbc(), dtype=bool)
-        pos = np.asarray(atoms.get_positions(), dtype=np.float64)
-        if cell.sum() == 0:       # calculator.py:534-547: an orthogonal cell large enough, periodic "for minus positions"
+        numbers, pos, cell, pbc, generated = self._inputs(atoms)
+        if generated:
             print('Warning: D3Calculator requires a cell.\nWarning: An orthogonal cell large enough is generated.')
-            max_cutoff = np.sqrt(max(self.rthr, self.cnthr)) * AU_TO_ANG
-            cell = np.eye(3) * (pos.max(axis=0) - pos.min(axis=0) + max_cutoff + 1.0)
-            pbc = np.array([True, True, True])
             atoms.set_cell(cell)
             atoms.set_pbc(pbc)
-        energy, forces, s = self.engine.compute(np.asarray(atoms.get_atomic_numbers()), pos, cell, pbc)
+        energy, forces, s = self.engine.compute(numbers, pos, cell, pbc)
         vol = abs(np.linalg.det(cell))
         stress = -np.array([s[0], s[1], s[2], s[5], s[4], s[3]]) / vol        # calculator.py:515-526 + /volume (:608)
         self.results = {'free_energy': energy, 'energy': energy, 'forces': forces, 'stress': stress}
         return self.results
+
+    def _forward(self, atoms):
+        """the three stages on ``atoms`` (``calculate``'s cell rule, ``atoms`` unmodified), held for the products"""
+        numbers, pos, cell, pbc, _ = self._inputs(atoms)
+        self.engine.set_system(numbers, pos, cell, pbc)
+        for stage in (1, 2, 3):
+            self.engine.run_stage(stage)
+
+    def get_hessian(self, atoms=None) -> np.ndarray:
+        """Hessian d2E/dr dr of the D3 energy of ``atoms`` (default: the calculator's atoms), [3N, 3N] float64 in
+        eV/A^2, row 3i + a = H e_(i,a), from 3N Hessian-vector products (``D3Engine.hvp``).  A periodic cell gives the
+        Gamma-point (supercell) Hessian; a structure without a cell is evaluated in ``calculate``'s generated cell
+        (``atoms`` is not modified).  Not symmetrised (the two triangles agree to the fp32 error of the pair
+        arithmetic); ``.reshape(N, 3, N, 3)`` gives the force constants.  ``results`` is not touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        self._forward(atoms)
+        eng, torch = self.engine, self.engine.torch
+        n = eng.n
+        eye = torch.eye(3 * n, dtype=torch.float64, device=eng.device)
+        rows = [eng.hvp(eye[k].reshape(n, 3)).reshape(-1) for k in range(3 * n)]
+        if not rows:
+            return np.zeros((0, 0))
+        return torch.stack(rows).cpu().numpy()
+
+    def _strain_pieces(self, atoms, relaxed: bool):
+        """The raw second derivatives ``elastic.elastic_tensor`` assembles: (dvirial [6, 6], outs [6, N, 3], volume,
+        Hessian [3N, 3N] or None), from the six Voigt strain products and, when ``relaxed``, the Hessian."""
+        cell = np.asarray(atoms.get_cell(), dtype=np.float64).reshape(3, 3)
+        vol = abs(np.linalg.det(cell))
+        if not np.asarray(atoms.get_pbc(), dtype=bool).all() or not vol > 0:
+            raise ValueError('the elastic tensor needs a cell periodic in all three directions with a volume > 0')
+        from . import elastic
+        if relaxed:
+            hessian = self.get_hessian(atoms)          # leaves the engine on the atoms' forward
+        else:
+            hessian = None
+            self._forward(atoms)
+        outs, dvir = [], []
+        for eps in elastic.voigt_strains():
+            o, d = self.engine.hvp_strain(None, eps[None])
+            outs.append(o)
+            dvir.append(d[0])
+        torch = self.engine.torch
+        return torch.stack(dvir).cpu().numpy(), torch.stack(outs).cpu().numpy(), vol, hessian
+
+    def get_elastic_tensor(self, atoms=None, relaxed: bool = True) -> np.ndarray:
+        """Elastic tensor d2E/de de / V of the D3 energy of ``atoms`` (default: the calculator's atoms), [6, 6] float64
+        in eV/A^3, ASE Voigt order, engineering strains: ``SevenNetCalculator.get_elastic_tensor``'s definitions,
+        units and refusals (``sevenn_b200.elastic``).  Six strain products (``D3Engine.hvp_strain``), plus the Hessian
+        (3N products) when ``relaxed``.  All three directions must be periodic."""
+        from . import elastic
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        return elastic.elastic_tensor(*self._strain_pieces(atoms, relaxed))
 
 
 class SevenNetD3Calculator(_Base):
@@ -333,3 +437,24 @@ class SevenNetD3Calculator(_Base):
             out['stress'] = a['stress'] + b['stress']
         self.results = out
         return out
+
+    def get_hessian(self, atoms=None) -> np.ndarray:
+        """Hessian of the network plus D3 energy, [3N, 3N] float64 in eV/A^2: ``SevenNetCalculator.get_hessian`` +
+        ``D3Calculator.get_hessian``, summed in fp64."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        return self.sevennet_calc.get_hessian(atoms) + self.d3_calc.get_hessian(atoms)
+
+    def get_elastic_tensor(self, atoms=None, relaxed: bool = True) -> np.ndarray:
+        """Elastic tensor of the network plus D3 energy, [6, 6] float64 in eV/A^3 (``SevenNetCalculator.
+        get_elastic_tensor``'s definitions).  The two terms' strain products and Hessians are summed before the
+        assembly: the relaxed-ion tensor C0 - Lambda^T H+ Lambda / V is not linear in (Lambda, H), so it is not the
+        sum of the two terms' relaxed-ion tensors."""
+        from . import elastic
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        dv_a, outs_a, vol, h_a = self.sevennet_calc._strain_pieces(atoms, relaxed)
+        dv_b, outs_b, _, h_b = self.d3_calc._strain_pieces(atoms, relaxed)
+        return elastic.elastic_tensor(dv_a + dv_b, outs_a + outs_b, vol, h_a + h_b if relaxed else None)

@@ -66,7 +66,7 @@ EXPORTS = [
     's7b_conv_double_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
-    's7b_engine_hvp', 's7b_engine_hvp_strain',
+    's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain',
 ]
 
 
@@ -111,6 +111,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_d3_set_element_tables.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.s7b_d3_set_system_batch.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]
     lib.s7b_d3_system_results.argtypes = [vp, vp, vp, vp, vp]
+    lib.s7b_d3_hvp_strain.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.s7b_engine_set_param.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, vp, sz]
     lib.s7b_engine_set_graph.argtypes = [vp, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.s7b_engine_run_stage.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]
