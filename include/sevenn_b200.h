@@ -214,6 +214,19 @@ S7B_API int s7b_engine_hvp(S7bEngine* eng, const float* d_v, float* d_out, void*
 S7B_API int s7b_engine_hvp_strain(S7bEngine* eng, const float* d_v, const double* d_strain, float* d_out,
                                   double* d_dvirial, void* stream);
 
+/* Potential part of the energy-barycentre heat flux of every structure (Green-Kubo thermal conductivity, DESIGN.md
+ * §8.3), exact for a message-passing model: J_pot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i), j over the
+ * structure's atoms, i over every atom and periodic image U_j depends on (an image moves with its atom), U_j the
+ * atomic energies of the last s7b_engine_compute.  One tangent-forward pass of four channels on that graph and
+ * forward; a periodic cell needs no unfolding.  Device pointers:
+ *   d_v    [n_nodes,3] f32, the velocities;
+ *   d_jpot [B,3] f64, overwritten with J_pot in eV A x (the unit of v);
+ *   d_ju   [B,3] f64 or NULL, overwritten with sum_j U_j v_j (the potential-energy part of the convective flux).
+ * B = the structure count of a graph from s7b_engine_set_positions_batch, else 1.  Per-structure sums in fp64 and a
+ * fixed order: deterministic, and a batch member's result is the structure's alone.  Preconditions and refusals are
+ * those of s7b_engine_hvp.  E == 0 gives J_pot = 0.  Buffers are allocated on the first call and kept. */
+S7B_API int s7b_engine_heat_flux(S7bEngine* eng, const float* d_v, double* d_jpot, double* d_ju, void* stream);
+
 /* Device pointer to an engine-owned buffer (valid until the next set_graph that grows it):
  * "x" (layer t input after self_interaction_1, [n_nodes, dim_x(t)]), "dx", "gate_in", "mid",
  * "h", "energy" (double[1]), "atomic_energy" [n_local], "atomic_energy_f64" (double[n_local], the same

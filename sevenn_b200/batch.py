@@ -155,6 +155,24 @@ class DeviceBatch:
         forces = eng.buffer('forces', shape=(eng.n_nodes, 3)).clone()
         return dict(energy=energy, atomic_energy=ae, forces=forces, virial=virial, n_edges=eng.n_edges)
 
+    def heat_flux(self, velocities, masses=None, convective: bool = True):
+        """Heat flux of every structure of the batch of the last ``compute``, [B, 3] float64 device tensor
+        (``sevenn_b200.heat_flux``'s definition, DESIGN.md §8.3): J_pot + J_conv, J_pot = sum_j sum_i
+        (r_j - r_i) (dU_j/dr_i . v_i) over the structure's atoms j and every atom and periodic image i that U_j depends
+        on, J_conv = sum_j (U_j + m_j |v_j|^2 / 2) v_j.  velocities [n, 3], masses [n] (needed when ``convective``),
+        numpy or torch, in the atom order of ``compute``.  Units: eV A x (the unit of v); with ASE's units (v in
+        A/(ASE time), m in amu) m v^2 / 2 is in eV.  ``convective=False`` gives J_pot alone.  One tangent-forward pass
+        over the whole batch."""
+        eng, torch = self.engine, self.engine.torch
+        jpot, ju = eng.heat_flux(velocities)
+        if not convective:
+            return jpot
+        if masses is None:
+            raise ValueError('the convective flux needs the masses (or pass convective=False)')
+        from .heat_flux import kinetic_flux
+        jk = kinetic_flux(_host(velocities), _host(masses), self.atom_ptr)
+        return jpot + ju + torch.as_tensor(jk, dtype=torch.float64, device=jpot.device)
+
     def elastic_tensors(self, numbers, positions, cells, pbc, system_idx, relaxed: bool = True, d3=None) -> np.ndarray:
         """Elastic tensors of every structure, [B, 6, 6] float64 in eV/A^3 (``SevenNetCalculator.get_elastic_tensor``'s
         definition, units and Voigt order, per structure; inputs as ``compute``).  Every structure must be periodic in

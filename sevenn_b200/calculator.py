@@ -95,6 +95,10 @@ class SevenNetCalculator(_Base):
         self.type_map = self.engine.spec.type_map
         self.compute_atomic_virial = compute_atomic_virial
         self.sevennet_config = sevennet_config or dict(self.meta)
+        self._engine_inputs = None     # (positions, cell, pbc, numbers) of the engine's current graph and forward
+
+    def _remember(self, pos, cell, pbc, numbers):
+        self._engine_inputs = tuple(np.array(a, copy=True) for a in (pos, cell, pbc, numbers))
 
     def _inputs(self, atoms):
         """(species, positions, cell, pbc, atomic numbers) of ``atoms`` for the engine"""
@@ -116,6 +120,7 @@ class SevenNetCalculator(_Base):
         # neighbour list, graph build, model and force path all run on the GPU (one C-ABI call);
         # the reference builds the graph on the CPU every step (calculator.py:224-226)
         energy, energies, forces, virial, n_edges = self.engine.compute_positions(species, pos, cell, pbc)
+        self._remember(pos, cell, pbc, numbers)
         # the reference divides by atoms.cell.volume whatever the pbc flags are (dataload.py:121,
         # force_output.py:227-228); a missing cell (volume 0) has no stress
         vol = abs(np.linalg.det(cell))
@@ -143,10 +148,11 @@ class SevenNetCalculator(_Base):
         if atoms is None:
             raise ValueError('No atoms to evaluate')
         torch = self.engine.torch
-        species, pos, cell, pbc, _ = self._inputs(atoms)
+        species, pos, cell, pbc, numbers = self._inputs(atoms)
         n = len(species)
         self.engine.set_positions(species, pos, cell, pbc)
         self.engine.compute()
+        self._remember(pos, cell, pbc, numbers)
         eye = torch.eye(3 * n, dtype=torch.float32, device=self.engine.device)
         rows = [self.engine.hvp(eye[k].reshape(n, 3)).reshape(-1) for k in range(3 * n)]
         if not rows:
@@ -169,11 +175,42 @@ class SevenNetCalculator(_Base):
             raise ValueError('No atoms to evaluate')
         return elastic.elastic_tensor(*self._strain_pieces(atoms, relaxed))
 
+    def get_heat_flux(self, atoms=None, convective: bool = True) -> np.ndarray:
+        """Energy-barycentre heat flux of ``atoms`` (default: the calculator's atoms), [3] float64, for Green-Kubo
+        thermal conductivity (``sevenn_b200.heat_flux``, DESIGN.md §8.3):
+
+          J = J_pot + J_conv,  J_pot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i),  J_conv = sum_j (U_j + m_j |v_j|^2 / 2) v_j
+
+        with U_j the atomic energies ('energies'), j over the atoms, i over every atom and periodic image U_j depends
+        on (T layers x cutoff away), an image moving with its atom.  This is exact for the message-passing model; the
+        pairwise split of the per-atom virial (``compute_atomic_virial``, J = sum_k W_k v_k) is not.  Velocities and
+        masses come from ``atoms.get_velocities()`` and ``get_masses()``.  Units: eV A^2 / (ASE time); multiply by
+        ``ase.units.fs`` for eV A^2/fs.  ``convective=False`` gives J_pot alone.  One tangent-forward pass of four
+        channels; the energy/force step runs only when positions, numbers, cell or pbc differ from those of the last
+        calculation, so an MD observer that asked for forces this step adds only the flux pass.  ``results`` are not
+        touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        species, pos, cell, pbc, numbers = self._inputs(atoms)
+        last = self._engine_inputs
+        if last is None or not all(np.array_equal(a, b) for a, b in zip(last, (pos, cell, pbc, numbers))):
+            self.engine.set_positions(species, pos, cell, pbc)
+            self.engine.compute()
+            self._remember(pos, cell, pbc, numbers)
+        v = np.asarray(atoms.get_velocities(), dtype=np.float64).reshape(-1, 3)
+        jpot, ju = self.engine.heat_flux(v.astype(np.float32))
+        J = jpot[0].cpu().numpy()
+        if convective:
+            from .heat_flux import kinetic_flux
+            J = J + ju[0].cpu().numpy() + kinetic_flux(v, atoms.get_masses())[0]
+        return J
+
     def _strain_pieces(self, atoms, relaxed: bool):
         """The raw second derivatives ``elastic.elastic_tensor`` assembles: (dvirial [6, 6], outs [6, N, 3], volume,
         Hessian [3N, 3N] or None), from the six Voigt strain products and, when ``relaxed``, the Hessian."""
         from . import elastic
-        species, pos, cell, pbc, _ = self._inputs(atoms)
+        species, pos, cell, pbc, numbers = self._inputs(atoms)
         vol = abs(np.linalg.det(cell))
         if not pbc.all() or not vol > 0:
             raise ValueError('the elastic tensor needs a cell periodic in all three directions with a volume > 0')
@@ -183,6 +220,7 @@ class SevenNetCalculator(_Base):
             hessian = None
             self.engine.set_positions(species, pos, cell, pbc)
             self.engine.compute()
+            self._remember(pos, cell, pbc, numbers)
         outs, dvir = [], []
         for eps in elastic.voigt_strains():
             o, d = self.engine.hvp_strain(None, eps[None])

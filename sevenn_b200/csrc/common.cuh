@@ -73,6 +73,19 @@ struct ConvTangents {
   const float* w;
 };
 
+// Operands of the heat flux's four-channel convolution JVP (conv_flux_jvp_kernel): the channel c's array starts at
+// c times its stride.  T [n_nodes, dim_x] and R [3][n_nodes, dim_x] are the tangents of x (null: zero, the first
+// layer); w1 = dw/dr [E, W] (the layout of ConvArgs::w); dr [4][E]; dY [4][E, y_stride]; vec = edge_vec [E, 3].
+struct FluxTangents {
+  const float* T;
+  const float* R;
+  const float* w1;
+  const float* dr;
+  const float* dY;
+  const float* vec;
+  size_t x_stride, dr_stride, dY_stride, out_stride;
+};
+
 }  // namespace s7b
 
 #define S7B_CUDA_CHECK(expr)                                                            \

@@ -9,7 +9,9 @@ namespace s7b {
                                   float*, float*, float*, float*, cudaStream_t);             \
   int launch_conv_jvp_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const ConvTangents&, float*, cudaStream_t); \
   int launch_conv_bwdt_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const ConvTangents&, const float*, \
-                                   float*, float*, float*, cudaStream_t);
+                                   float*, float*, float*, cudaStream_t); \
+  int launch_conv_flux_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const FluxTangents&, int, int*, float*, \
+                                   cudaStream_t);
 S7B_DECL_GROUP(1, 0) S7B_DECL_GROUP(1, 1) S7B_DECL_GROUP(1, 2) S7B_DECL_GROUP(1, 3)
 S7B_DECL_GROUP(2, 0) S7B_DECL_GROUP(2, 1) S7B_DECL_GROUP(2, 2) S7B_DECL_GROUP(2, 3)
 S7B_DECL_GROUP(3, 0) S7B_DECL_GROUP(3, 1) S7B_DECL_GROUP(3, 2) S7B_DECL_GROUP(3, 3)
@@ -75,6 +77,16 @@ int launch_conv_bwd_tangent(int l1, int lf, int lo, const ConvArgs& a, const Con
   if (a.n_dst <= a.n_begin) return 0;      // empty centre range
   int rc = 2;
   if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(bwdt, l1, a, role, tan, gout, dx, dY_acc, dw, st)
+  return conv_status(rc);
+}
+
+// One walk of the heat flux's convolution JVP over the channels c0 .. c0 + *nch - 1 (*nch set from the kind)
+int launch_conv_flux(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0,
+                     int* nch, float* out, cudaStream_t st) {
+  *nch = 4;
+  if (a.n_dst <= a.n_begin) return 0;      // empty centre range
+  int rc = 2;
+  if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(flux, l1, a, role, f, c0, nch, out, st)
   return conv_status(rc);
 }
 

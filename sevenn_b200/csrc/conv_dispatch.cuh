@@ -148,6 +148,26 @@ static int bwdt_kind_rt(const ConvArgs& a, const ConvRole& role, const ConvTange
   return launch_bwdt_one<Kind, 1, 16>(a, role, tan, gout, dx, dY, dw, st);
 }
 
+// Heat flux (engine.cu s7b_engine_heat_flux): the runtime-width lane mapping of the JVP with one channel pair per
+// lane (NV = 1), flux_channels<Kind>() of the four tangent channels per walk
+template <class Kind, int LPN>
+static int launch_flux_one(const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0, int* nch,
+                           float* out, cudaStream_t st) {
+  constexpr int NCH = flux_channels<Kind>();
+  *nch = NCH;
+  conv_flux_jvp_kernel<Kind, 1, LPN, NCH><<<conv_grid<0, 1, LPN>(a, role), 32 * kConvWarpsPerBlock, 0, st>>>(
+      a, role, f, c0, out);
+  return cudaGetLastError() == cudaSuccess ? 0 : 1;
+}
+
+template <class Kind>
+static int flux_kind_rt(const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0, int* nch, float* out,
+                        cudaStream_t st) {
+  if (role.mul <= 0 || role.mul % 32 != 0) return kConvWrongMul;
+  if (role.mul % 64 == 0) return launch_flux_one<Kind, 32>(a, role, f, c0, nch, out, st);
+  return launch_flux_one<Kind, 16>(a, role, f, c0, nch, out, st);
+}
+
 // Paths (l2, l3) of the kind (l1, lmax_filter, lmax_out): the triangle rule with l2 <= LF, l3 <= LO
 constexpr int tp_npath(int l1, int lf, int lo) {
   int n = 0;
@@ -197,12 +217,19 @@ static int bwdt_role(const ConvArgs& a, const ConvRole& role, const ConvTangents
   else return bwdt_kind_rt<TPKind<L1, LF, LO>, MAXNV>(a, role, tan, gout, dx, dY, dw, st);
 }
 
+template <int L1, int LF, int LO>
+static int flux_role(const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0, int* nch, float* out,
+                     cudaStream_t st) {
+  if constexpr (tp_npath(L1, LF, LO) == 0) return kConvNoPath;
+  else return flux_kind_rt<TPKind<L1, LF, LO>>(a, role, f, c0, nch, out, st);
+}
+
 }  // namespace s7b
 
 // Defines  launch_conv_fwd_LF_LO / launch_conv_bwd_LF_LO  for l1 = 0..3.  SPEC = 1 for the groups of SevenNet-0
 // and SevenNet-l3i5, which also get the kernels specialised for the widths kConvMul (l1 = 3 only with LF = 3);
 // the other groups have only the runtime-width kernels.  launch_conv_jvp_LF_LO / launch_conv_bwdt_LF_LO: the
-// second-order kernels, runtime width in every group.
+// second-order kernels, runtime width in every group; launch_conv_flux_LF_LO: the heat flux's, likewise.
 #define S7B_CONV_SPEC_MUL(SPEC, LF, L1) ((SPEC) && ((L1) < 3 || (LF) >= 3) ? s7b::kConvMul[L1] : 0)
 #define S7B_DEFINE_CONV_GROUP(LF, LO, SPEC)                                                        \
   namespace s7b {                                                                                  \
@@ -245,6 +272,17 @@ static int bwdt_role(const ConvArgs& a, const ConvRole& role, const ConvTangents
       case 1: return bwdt_role<1, LF, LO, 1>(a, role, tan, gout, dx, dY, dw, st);                  \
       case 2: return bwdt_role<2, LF, LO, 1>(a, role, tan, gout, dx, dY, dw, st);                  \
       case 3: return bwdt_role<3, LF, LO, 1>(a, role, tan, gout, dx, dY, dw, st);                  \
+    }                                                                                              \
+    return 1;                                                                                      \
+  }                                                                                                \
+  int launch_conv_flux_##LF##_##LO(int l1, const ConvArgs& a, const ConvRole& role,                \
+                                   const FluxTangents& f, int c0, int* nch, float* out,            \
+                                   cudaStream_t st) {                                              \
+    switch (l1) {                                                                                  \
+      case 0: return flux_role<0, LF, LO>(a, role, f, c0, nch, out, st);                           \
+      case 1: return flux_role<1, LF, LO>(a, role, f, c0, nch, out, st);                           \
+      case 2: return flux_role<2, LF, LO>(a, role, f, c0, nch, out, st);                           \
+      case 3: return flux_role<3, LF, LO>(a, role, f, c0, nch, out, st);                           \
     }                                                                                              \
     return 1;                                                                                      \
   }                                                                                                \

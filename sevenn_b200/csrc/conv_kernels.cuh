@@ -558,6 +558,115 @@ conv_jvp_kernel(const ConvArgs a, const ConvRole role, const ConvTangents tan, f
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// heat flux (engine.cu s7b_engine_heat_flux, DESIGN.md §8.3): the JVP of conv_jvp_kernel for the channels
+// c = c0 .. c0 + NCH - 1 of the four (T, R_x, R_y, R_z), in one walk of the row.  x, Y, w and w' are read once per
+// edge and shared by the channels; per channel the operand tangents are formed in registers:
+//   dx_c = T[src]                                   (c = 0)
+//          R_a[src] - vec_a T[src]                  (c = 1 + a; f.T null: dx = 0 for every channel)
+//   dY_c = f.dY[c],  dw_c = w' f.dr[c][e]
+// out + c * f.out_stride: the channel's mid rows.  NCH is the largest of 4, 2, 1 whose accumulators fit the
+// register budget (flux_channels); the host walks each row 4 / NCH times.
+// ------------------------------------------------------------------------------------------
+template <class Kind>
+constexpr int flux_channels() {
+  return Kind::NACC * 4 <= 40 ? 4 : (Kind::NACC * 2 <= 50 ? 2 : 1);
+}
+
+template <class Kind, int NV, int LPN, int NCH>
+__global__ void S7B_FWD_BOUNDS
+conv_flux_jvp_kernel(const ConvArgs a, const ConvRole role, const FluxTangents f, int c0, float* __restrict__ out) {
+  const LaneMap<NV, LPN, 2> m(a);
+  if (m.nmax == 0 && !m.node_ok) return;      // whole warp beyond the last node (uniform)
+  const int mul = role.mul;
+  const bool hx = f.T != nullptr;
+
+  V2 acc[NCH][NV][Kind::NACC];
+#pragma unroll
+  for (int k = 0; k < NCH; ++k)
+#pragma unroll
+    for (int c = 0; c < NV; ++c)
+#pragma unroll
+      for (int q = 0; q < Kind::NACC; ++q) acc[k][c][q] = splat2(0.0f);
+
+  const unsigned xlane = role.x_off + m.uc0;
+  EdgeRecs<LPN> recs;
+  for (int it = 0; it < m.nmax; ++it) {
+    const bool valid = (LPN == 32) || (it < m.len);
+    const int e = valid ? m.e0 + it : 0;
+    if (it % LPN == 0) recs.fill(a, m.e0, m.len, it, m.sl);
+    const int4 rec = recs.get(it);
+    float Y[Kind::NY];
+    load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
+    float ev[3], dr[NCH];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) ev[q] = __ldg(f.vec + 3 * (size_t)e + q);
+#pragma unroll
+    for (int k = 0; k < NCH; ++k) dr[k] = __ldg(f.dr + (size_t)(c0 + k) * f.dr_stride + e);
+    const size_t xo = row_offset(rec.x, a.dim_x) + xlane;
+    const size_t wo = (size_t)e * a.w_numel + m.uc0;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+      const int u = 2 * LPN * c;                         // channel offset from m.uc0
+      V2 x[Kind::D1], T[Kind::D1], w[Kind::NPATH], w1[Kind::NPATH];
+#pragma unroll
+      for (int i = 0; i < Kind::D1; ++i) {
+        x[i] = ldg2(a.x + xo + (i * mul + u));
+        if (hx) T[i] = ldg2(f.T + xo + (i * mul + u));
+      }
+#pragma unroll
+      for (int p = 0; p < Kind::NPATH; ++p) {
+        w[p] = ldg2(a.w + wo + (role.w_off[p] + u));
+        w1[p] = ldg2(f.w1 + wo + (role.w_off[p] + u));
+        if (LPN != 32 && !valid) w[p] = w1[p] = splat2(0.0f);   // every term has w or w' as a factor
+      }
+#pragma unroll
+      for (int k = 0; k < NCH; ++k) {
+        const int ch = c0 + k;
+        float tY[Kind::NY];
+        load_Y<Kind>(f.dY + (size_t)ch * f.dY_stride + row_offset(e, y_stride(Kind::NY)), tY);
+        if constexpr (NCH == 1) {      // the widest kinds: the tangents replace T and w' in their registers
+          if (hx && ch > 0) {
+#pragma unroll
+            for (int i = 0; i < Kind::D1; ++i)
+              T[i] = fma_(-ev[ch - 1], T[i], ldg2(f.R + (size_t)(ch - 1) * f.x_stride + xo + (i * mul + u)));
+          }
+#pragma unroll
+          for (int p = 0; p < Kind::NPATH; ++p) w1[p] = mul_(w1[p], dr[k]);
+          TPTangent<Kind>::jvp(x, Y, w, T, tY, w1, hx, true, true, acc[k][c]);
+        } else {
+          V2 tx[Kind::D1], tw[Kind::NPATH];
+          if (hx) {
+#pragma unroll
+            for (int i = 0; i < Kind::D1; ++i) {
+              if (ch == 0) tx[i] = T[i];
+              else tx[i] = fma_(-ev[ch - 1], T[i], ldg2(f.R + (size_t)(ch - 1) * f.x_stride + xo + (i * mul + u)));
+            }
+          }
+#pragma unroll
+          for (int p = 0; p < Kind::NPATH; ++p) tw[p] = mul_(w1[p], dr[k]);
+          TPTangent<Kind>::jvp(x, Y, w, tx, tY, tw, hx, true, true, acc[k][c]);
+        }
+      }
+    }
+  }
+  if (!m.node_ok) return;
+#pragma unroll
+  for (int k = 0; k < NCH; ++k) {
+    float* __restrict__ orow = out + (size_t)(c0 + k) * f.out_stride + (size_t)m.n * a.dim_mid;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+      const int u = m.uc0 + 2 * LPN * c;
+#pragma unroll
+      for (int p = 0; p < Kind::NPATH; ++p) {
+#pragma unroll
+        for (int q = 0; q < 2 * Kind::path_l3(p) + 1; ++q)
+          VT<V2>::store(orow + role.out_off[p] + q * role.out_stride[p] + u, acc[k][c][Kind::acc_off(p) + q]);
+      }
+    }
+  }
+}
+
 // One walk of conv_bwd_tangent_kernel over the CSR row of this lane's node, computing the outputs in OUT
 // (kTanDw | kTanDx | kTanDY)
 enum { kTanDw = 1, kTanDx = 2, kTanDY = 4 };

@@ -21,6 +21,7 @@
 #include "edge_kernels.cuh"
 #include "hvp_kernels.cuh"
 #include "neighbor.cuh"
+#include "flux_kernels.cuh"
 #include "node_kernels.cuh"
 #include "tc_gemm.cuh"
 
@@ -56,6 +57,8 @@ int launch_conv_jvp(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& r
                     float* out, cudaStream_t st);
 int launch_conv_bwd_tangent(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
                             const float* gout, float* dx, float* dY_acc, float* dw, cudaStream_t st);
+int launch_conv_flux(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0,
+                     int* nch, float* out, cudaStream_t st);
 
 static int64_t g_alloc_gen = 0;   // bumped by every (re)allocation: captured CUDA graphs hold raw pointers
 
@@ -212,6 +215,19 @@ struct HvpBufs {
   }
 };
 
+// Buffers of the heat flux (s7b_engine_heat_flux), allocated on its first call and sized for one layer: every node
+// array holds the four channels (T, R_x, R_y, R_z) one after another, [4][n_nodes][widest row of any layer].
+struct FluxBufs {
+  DevBuf dr, dY;                  // [4][E], [4][E][ny_stride]: edge tangents
+  DevBuf emb2, hA, hB, w2;        // radial jet [2][E][.]: w and w' of one layer
+  DevBuf tx, dmid, tg, th;        // node tangents of one layer
+  DevBuf atom_ptr1;               // {0, n} of a one-structure graph
+  RowExp re;
+  void release() {
+    for (DevBuf* b : {&dr, &dY, &emb2, &hA, &hB, &w2, &tx, &dmid, &tg, &th, &atom_ptr1, &re.buf}) b->release();
+  }
+};
+
 // The global parameters ("bessel" lives in RadialDesc)
 struct GlobalParams {
   DevBuf embed_x0, embed_g0, readout, readout_lo, scale, shift;
@@ -292,6 +308,7 @@ struct S7bEngine {
   // second order: hvp_ready = an s7b_engine_compute ran since the last set_graph / set_param
   bool hvp_ready = false;
   HvpBufs hv;
+  FluxBufs fx;
 };
 
 struct S7bConvPlan {
@@ -1106,6 +1123,7 @@ void s7b_engine_destroy(S7bEngine* e) {
   for (auto* v : {&e->x, &e->g, &e->wbuf, &e->z1, &e->z2, &e->h1, &e->h2})
     for (auto& b : *v) b.release();
   e->hv.release();
+  e->fx.release();
   delete e;
 }
 
@@ -1940,6 +1958,136 @@ int s7b_engine_hvp_strain(S7bEngine* e, const float* d_v, const double* d_strain
                                               hv.fneg.as<float>(), hv.sys_energy.as<double>(), hv.dvir2.as<double>());
   S7B_LAUNCH_CHECK();
   hvp_sub_kernel<<<(6 * B + 255) / 256, 256, 0, st>>>(d_dvirial, hv.dvir2.as<double>(), 6 * B);
+  S7B_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- heat flux ---------------------------------------------------------------------------------------------------
+// J_pot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i) by one tangent-forward pass of four channels on the graph and
+// forward of the last compute (DESIGN.md §8.3).  Per layer t: w and w' from the radial MLP (hvp_radial_jet's first
+// two rows); tx = si1(th) (0 at t = 0, the embedding depends on the species only); dmid = the four-channel
+// convolution JVP; tg = sc(th) + si2(dmid); th = gate'(g) tg.  Then J_pot = sum_j scale_s readout(R_j).
+
+// w, w' of layer t as fx.w2 [2][E][W] from the radial basis jet fx.emb2 (rows 0 and 1 of [3][E][n_basis])
+static int flux_radial_jet(S7bEngine* e, int t, cudaStream_t st) {
+  const LayerParams& P = e->layer_params[t];
+  const int64_t E2 = 2 * e->n_edges;
+  const int nb = e->desc.n_basis, h0 = e->desc.radial_hidden[0], h1 = e->desc.radial_hidden[1], W = e->layers[t].W;
+  FluxBufs& fx = e->fx;
+  if (dense_gemm(fx.emb2.as<float>(), nb, fx.hA.as<float>(), h0, P.mlp[0].as<float>(), E2, kEpiNone, nullptr, nullptr, false, st)) return 1;
+  flux_silu_jet_kernel<<<grid1d((size_t)e->n_edges * h0, 256), 256, 0, st>>>(fx.hA.as<float>(), e->n_edges * h0);
+  S7B_LAUNCH_CHECK();
+  if (dense_gemm(fx.hA.as<float>(), h0, fx.hB.as<float>(), h1, P.mlp[1].as<float>(), E2, kEpiNone, nullptr, nullptr, false, st)) return 1;
+  flux_silu_jet_kernel<<<grid1d((size_t)e->n_edges * h1, 256), 256, 0, st>>>(fx.hB.as<float>(), e->n_edges * h1);
+  S7B_LAUNCH_CHECK();
+  return dense_gemm(fx.hB.as<float>(), h1, fx.w2.as<float>(), W, P.mlp[2].as<float>(), E2, kEpiNone, nullptr, nullptr, false, st);
+}
+
+// Widest rows of any layer: x, g, mid and h (h at least x: si1 of layer t reads the h of layer t - 1)
+static void flux_widths(const S7bEngine* e, size_t& mx, size_t& mg, size_t& mm, size_t& mh, size_t& mW) {
+  mx = mg = mm = mh = mW = 0;
+  for (const LayerCfg& L : e->layers) {
+    mx = std::max(mx, (size_t)L.x.dim);
+    mg = std::max(mg, (size_t)L.g.dim);
+    mm = std::max(mm, (size_t)L.mid.dim);
+    mh = std::max(mh, (size_t)L.dim_h);
+    mW = std::max(mW, (size_t)L.W);
+  }
+  mh = std::max(mh, mx);
+}
+
+static int flux_alloc(S7bEngine* e) {
+  FluxBufs& fx = e->fx;
+  const size_t E = (size_t)e->n_edges, N = (size_t)std::max(e->n_nodes, 1), ny = (size_t)e->ny_stride;
+  const size_t C = kFluxChannels;
+  size_t mx, mg, mm, mh, mW;
+  flux_widths(e, mx, mg, mm, mh, mW);
+  int rc = 0;
+  rc |= fx.dr.ensure(C * E * sizeof(float));
+  rc |= fx.dY.ensure(C * E * ny * sizeof(float));
+  rc |= fx.emb2.ensure(3 * E * e->desc.n_basis * sizeof(float));   // hvp_radial_basis_kernel writes w'' 's row too
+  rc |= fx.hA.ensure(2 * E * e->desc.radial_hidden[0] * sizeof(float));
+  rc |= fx.hB.ensure(2 * E * e->desc.radial_hidden[1] * sizeof(float));
+  rc |= fx.w2.ensure(2 * E * mW * sizeof(float));
+  rc |= fx.tx.ensure(C * N * mx * sizeof(float));
+  rc |= fx.dmid.ensure(C * N * mm * sizeof(float));
+  rc |= fx.tg.ensure(C * N * mg * sizeof(float));
+  rc |= fx.th.ensure(C * N * mh * sizeof(float));
+  rc |= fx.re.buf.ensure(N * 16 * sizeof(int));
+  return rc ? fail("cudaMalloc failed for the heat flux's buffers") : 0;
+}
+
+static int flux_pass(S7bEngine* e, const float* v, cudaStream_t st) {
+  const int T = e->desc.n_layers, LF = e->desc.lmax_filter, N = e->n_nodes;
+  const int64_t E = e->n_edges;
+  const int ny = e->ny_stride;
+  FluxBufs& fx = e->fx;
+  size_t mx, mg, mm, mh, mW;
+  flux_widths(e, mx, mg, mm, mh, mW);
+  const size_t sx = (size_t)N * mx, sg = (size_t)N * mg, sm = (size_t)N * mm, sh = (size_t)N * mh;
+  {
+    const int grd = (N * 32 + 255) / 256;
+    if (LF == 1) flux_edge_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>());
+    else if (LF == 2) flux_edge_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>());
+    else flux_edge_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>());
+    S7B_LAUNCH_CHECK();
+    hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, fx.emb2.as<float>());
+    S7B_LAUNCH_CHECK();
+  }
+  float* tx = fx.tx.as<float>();
+  float* tg = fx.tg.as<float>();
+  float* th = fx.th.as<float>();
+  float* dmid = fx.dmid.as<float>();
+  for (int t = 0; t < T; ++t) {
+    const LayerCfg& L = e->layers[t];
+    const LayerParams& P = e->layer_params[t];
+    if (flux_radial_jet(e, t, st)) return 1;
+    if (t > 0)
+      for (int c = 0; c < kFluxChannels; ++c)
+        if (node_linear(e, P.si1, fx.re, true, th + c * sh, tx + c * sx, false, st)) return 1;
+    ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
+    ca.w = fx.w2.as<float>();          // raw kernels on the MLP's weights, in both radial modes
+    const FluxTangents f{t > 0 ? tx : nullptr, t > 0 ? tx + sx : nullptr, fx.w2.as<float>() + (size_t)E * L.W,
+                         fx.dr.as<float>(), fx.dY.as<float>(), e->d_edge_vec, sx, (size_t)E, (size_t)E * ny, sm};
+    for (int l1 = 0; l1 < L.x.n_l; ++l1)
+      for (int c0 = 0, nch = kFluxChannels; c0 < kFluxChannels; c0 += nch)
+        if (launch_conv_flux(l1, LF, L.lmax_out, ca, L.roles[l1], f, c0, &nch, dmid, st)) return 1;
+    for (int c = 0; c < kFluxChannels; ++c) {
+      S7B_CUDA_CHECK(cudaMemsetAsync(tg + c * sg, 0, (size_t)N * L.g.dim * sizeof(float), st));
+      if (t > 0 && node_linear(e, P.sc, fx.re, true, th + c * sh, tg + c * sg, false, st)) return 1;
+      if (node_linear(e, P.si2, fx.re, true, dmid + c * sm, tg + c * sg, true, st)) return 1;
+      gate_jvp_kernel<<<grid1d((size_t)N * L.dim_h, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), tg + c * sg, th + c * sh, N);
+      S7B_LAUNCH_CHECK();
+    }
+  }
+  return 0;
+}
+
+int s7b_engine_heat_flux(S7bEngine* e, const float* d_v, double* d_jpot, double* d_ju, void* stream) {
+  if (hvp_check(e, "s7b_engine_heat_flux")) return 1;
+  if (!d_jpot || (e->n_nodes > 0 && !d_v)) return fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int B = std::max(e->n_systems, 1);
+  S7B_CUDA_CHECK(cudaMemsetAsync(d_jpot, 0, (size_t)B * 3 * sizeof(double), st));
+  if (d_ju) S7B_CUDA_CHECK(cudaMemsetAsync(d_ju, 0, (size_t)B * 3 * sizeof(double), st));
+  if (e->n_nodes == 0) return 0;
+  const int* atom_ptr = e->sys_atom_ptr.as<int>();
+  if (e->n_systems < 1) {
+    const int one[2] = {0, e->n_nodes};
+    if (e->fx.atom_ptr1.ensure(2 * sizeof(int))) return fail("cudaMalloc failed for the heat flux's buffers");
+    S7B_CUDA_CHECK(cudaMemcpyAsync(e->fx.atom_ptr1.p, one, sizeof(one), cudaMemcpyHostToDevice, st));
+    atom_ptr = e->fx.atom_ptr1.as<int>();
+  }
+  const bool edges = e->n_edges > 0;   // no edge: the atomic energies do not depend on the positions, J_pot = 0
+  if (edges && (flux_alloc(e) || flux_pass(e, d_v, st))) return 1;
+  if (!edges && !d_ju) return 0;
+  const LayerCfg& Lz = e->layers[e->desc.n_layers - 1];
+  size_t mx, mg, mm, mh, mW;
+  flux_widths(e, mx, mg, mm, mh, mW);
+  const GlobalParams& G = e->global_params;
+  flux_sums_kernel<<<B, kSysBlock, 0, st>>>(atom_ptr, edges ? e->fx.th.as<float>() : nullptr, (size_t)e->n_nodes * mh,
+                                            Lz.dim_h, G.readout.as<float>(), G.readout_lo.as<float>(), G.scale.as<float>(),
+                                            e->d_species, e->atomic_energy64.as<double>(), d_v, edges ? d_jpot : nullptr, d_ju);
   S7B_LAUNCH_CHECK();
   return 0;
 }

@@ -66,7 +66,7 @@ EXPORTS = [
     's7b_conv_double_backward',
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
-    's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain',
+    's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain', 's7b_engine_heat_flux',
 ]
 
 
@@ -118,6 +118,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_compute.argtypes = [vp, vp]
     lib.s7b_engine_hvp.argtypes = [vp, vp, vp, vp]
     lib.s7b_engine_hvp_strain.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.s7b_engine_heat_flux.argtypes = [vp, vp, vp, vp, vp]
     lib.s7b_engine_buffer.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(sz)]
     lib.s7b_engine_buffer.restype = vp
     lib.s7b_engine_compute_host.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -651,6 +652,27 @@ class B200Engine:
                                                  None if strain is None else strain.data_ptr(), out.data_ptr(),
                                                  dvir.data_ptr(), self._stream()))
         return out, dvir
+
+    def heat_flux(self, v):
+        """Heat flux of every structure on the graph and forward of the last ``compute`` (C ABI
+        ``s7b_engine_heat_flux``, DESIGN.md §8.3).  v [n_nodes, 3] velocities, numpy or torch (any device).  Returns
+        (jpot, ju), [B, 3] float64 device tensors, B = the structure count of a ``set_positions_batch`` graph, else 1:
+        jpot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i), the exact potential flux of the atomic energies U_j over
+        every atom and periodic image i they depend on, and ju = sum_j U_j v_j.  Units: eV A resp. eV, times the unit of
+        v.  One tangent-forward pass of four channels; uploads the radial MLP of a table-mode engine on first use, as
+        ``hvp``."""
+        torch = self.torch
+        n = self.n_nodes
+        B = max((self._graph or {}).get('n_systems', 0), 1)
+        v = torch.as_tensor(v).to(self.device, torch.float32).contiguous()
+        if v.numel() != 3 * n or (v.dim() == 2 and v.shape[1] != 3) or v.dim() > 2:
+            raise ValueError(f'v has {tuple(v.shape)}, expected [{n}, 3] (n_nodes)')
+        jpot = torch.empty(B, 3, dtype=torch.float64, device=self.device)
+        ju = torch.empty(B, 3, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._upload_hvp_mlp()
+            check(self.lib.s7b_engine_heat_flux(self._h, v.data_ptr(), jpot.data_ptr(), ju.data_ptr(), self._stream()))
+        return jpot, ju
 
     def buffer(self, name: str, layer: int = 0, dtype: str = 'f4', shape=None):
         """Zero-copy torch view of an engine buffer (valid until the next set_graph)."""
