@@ -381,7 +381,8 @@ S7B_API int s7b_d3_set_damping(S7bD3* d3, int32_t damping, double s6, double s8,
 S7B_API int s7b_d3_set_system(S7bD3* d3, int32_t n_atoms, const int32_t* types, const double* positions,
                               const double* cell9, const int32_t* pbc3, void* stream);
 S7B_API int s7b_d3_run_stage(S7bD3* d3, int32_t stage, int32_t i_begin, int32_t i_end, void* stream);
-/* device buffers in bin-sorted order: "cn", "dc6i" double[n]; "force" double[n,3] (hartree/bohr); "energy"
+/* device buffers in bin-sorted order: "cn", "dc6i" double[n]; "eatom" double[n] (hartree, the atomic energies
+ * -1/2 sum_{j,tau} C6_ij g(r_ij) of stage 2); "force" double[n,3] (hartree/bohr); "energy"
  * double[B]; "sigma" double[B,6]; "order" int32[n] (sorted position -> caller's atom index); "type" int32[n] (after
  * s7b_d3_set_system_batch: Z - 1 | local type << 8, the local type being the rank of Z among the elements of the
  * atom's structure; after s7b_d3_set_system: the type index).  B = 1 after
@@ -421,6 +422,18 @@ S7B_API int s7b_d3_system_results(S7bD3* d3, double* d_energy, double* d_forces,
  * Per-structure sums in a fixed order: deterministic, and independent of the other structures of the batch. */
 S7B_API int s7b_d3_hvp_strain(S7bD3* d3, const double* d_v, const double* d_strain, double* d_out, double* d_dvirial,
                               void* stream);
+/* Potential part of the energy-barycentre heat flux of D3's atomic energies (DESIGN.md §8.4), per structure of the
+ * current system: J_pot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i), j over the structure's atoms, i over every atom
+ * and periodic image U_j depends on (an image moves with its atom), U_j = -1/2 sum_{k,tau} C6_jk g(r_jk) the pair
+ * pass's atomic energies ("eatom"), with the forward of the last three stages held.  Two cell-list passes; a periodic
+ * cell needs no unfolding.  Device pointers:
+ *   d_v    [n,3] f64, the velocities (Angstrom x any time unit, caller's atom order);
+ *   d_jpot [B,3] f64, overwritten with J_pot in eV A x (the unit of v);
+ *   d_ju   [B,3] f64 or NULL, overwritten with sum_j U_j v_j (the potential-energy part of the convective flux).
+ * Preconditions and refusals are those of s7b_d3_hvp_strain.  With no atoms the outputs are zero-filled.  Scratch is
+ * allocated on the first call and kept; no forward buffer is written.  Per-structure sums in fp64 and a fixed order:
+ * deterministic, and a batch member's result is the structure's alone. */
+S7B_API int s7b_d3_heat_flux(S7bD3* d3, const double* d_v, double* d_jpot, double* d_ju, void* stream);
 
 /* The reference's own D3 entry points (pair_d3_for_ase.cu:2034-2082; ctypes signatures sevenn/calculator.py:430-483),
  * same names / arguments / call order, so its D3Calculator can load this library in place of pair_d3.so.

@@ -155,16 +155,23 @@ class DeviceBatch:
         forces = eng.buffer('forces', shape=(eng.n_nodes, 3)).clone()
         return dict(energy=energy, atomic_energy=ae, forces=forces, virial=virial, n_edges=eng.n_edges)
 
-    def heat_flux(self, velocities, masses=None, convective: bool = True):
+    def heat_flux(self, velocities, masses=None, convective: bool = True, d3=None):
         """Heat flux of every structure of the batch of the last ``compute``, [B, 3] float64 device tensor
         (``sevenn_b200.heat_flux``'s definition, DESIGN.md §8.3): J_pot + J_conv, J_pot = sum_j sum_i
         (r_j - r_i) (dU_j/dr_i . v_i) over the structure's atoms j and every atom and periodic image i that U_j depends
         on, J_conv = sum_j (U_j + m_j |v_j|^2 / 2) v_j.  velocities [n, 3], masses [n] (needed when ``convective``),
         numpy or torch, in the atom order of ``compute``.  Units: eV A x (the unit of v); with ASE's units (v in
         A/(ASE time), m in amu) m v^2 / 2 is in eV.  ``convective=False`` gives J_pot alone.  One tangent-forward pass
-        over the whole batch."""
+        over the whole batch.  ``d3`` (a ``d3.D3Batch`` whose last ``compute`` was on the same structures, as
+        ``SevenNetD3Model.forward`` leaves it) adds D3 dispersion's J_pot and sum_j U_j v_j (DESIGN.md §8.4); the
+        kinetic part is counted once."""
         eng, torch = self.engine, self.engine.torch
+        if d3 is not None and (d3.atom_ptr is None or not np.array_equal(np.asarray(d3.atom_ptr), np.asarray(self.atom_ptr))):
+            raise ValueError('d3: its last compute was not on the structures of this batch (atom_ptr differs)')
         jpot, ju = eng.heat_flux(velocities)
+        if d3 is not None:
+            jp3, ju3 = d3.heat_flux(velocities)
+            jpot, ju = jpot + jp3, ju + ju3
         if not convective:
             return jpot
         if masses is None:
@@ -321,3 +328,13 @@ class SevenNetD3Model(SevenNetModel):
         (``DeviceBatch.elastic_tensors`` with this model's ``D3Batch``)."""
         return self._batch.elastic_tensors(state.atomic_numbers, state.positions, self._cells(state), state.pbc,
                                            state.system_idx, relaxed, d3=self.d3)
+
+    def heat_flux(self, state, velocities, convective: bool = True):
+        """Heat flux of the network plus D3 energy of every structure of the state, [B, 3] float64 device tensor
+        (``DeviceBatch.heat_flux`` with this model's ``D3Batch``): the network's and D3's J_pot and sum_j U_j v_j,
+        plus the kinetic part once, with the masses from ``state.masses``.  velocities [n, 3] in the state's atom
+        order.  Runs the network's and D3's forward on the state first."""
+        cells = self._cells(state)
+        self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
+        self.d3.compute(state.atomic_numbers, state.positions, cells, state.pbc, atom_ptr=self._batch.atom_ptr)
+        return self._batch.heat_flux(velocities, state.masses if convective else None, convective, d3=self.d3)

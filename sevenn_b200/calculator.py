@@ -188,10 +188,19 @@ class SevenNetCalculator(_Base):
         ``ase.units.fs`` for eV A^2/fs.  ``convective=False`` gives J_pot alone.  One tangent-forward pass of four
         channels; the energy/force step runs only when positions, numbers, cell or pbc differ from those of the last
         calculation, so an MD observer that asked for forces this step adds only the flux pass.  ``results`` are not
-        touched."""
+        touched.  ``SevenNetD3Calculator.get_heat_flux`` adds D3 dispersion's."""
         atoms = atoms if atoms is not None else self.atoms
         if atoms is None:
             raise ValueError('No atoms to evaluate')
+        J, ju, v = self._flux_parts(atoms)
+        if convective:
+            from .heat_flux import kinetic_flux
+            J = J + ju + kinetic_flux(v, atoms.get_masses())[0]
+        return J
+
+    def _flux_parts(self, atoms):
+        """(J_pot [3], sum_j U_j v_j [3], velocities [n, 3]) of ``atoms``; the energy/force step runs only when
+        positions, numbers, cell or pbc differ from those of the last calculation"""
         species, pos, cell, pbc, numbers = self._inputs(atoms)
         last = self._engine_inputs
         if last is None or not all(np.array_equal(a, b) for a, b in zip(last, (pos, cell, pbc, numbers))):
@@ -200,11 +209,7 @@ class SevenNetCalculator(_Base):
             self._remember(pos, cell, pbc, numbers)
         v = np.asarray(atoms.get_velocities(), dtype=np.float64).reshape(-1, 3)
         jpot, ju = self.engine.heat_flux(v.astype(np.float32))
-        J = jpot[0].cpu().numpy()
-        if convective:
-            from .heat_flux import kinetic_flux
-            J = J + ju[0].cpu().numpy() + kinetic_flux(v, atoms.get_masses())[0]
-        return J
+        return jpot[0].cpu().numpy(), ju[0].cpu().numpy(), v
 
     def _strain_pieces(self, atoms, relaxed: bool):
         """The raw second derivatives ``elastic.elastic_tensor`` assembles: (dvirial [6, 6], outs [6, N, 3], volume,

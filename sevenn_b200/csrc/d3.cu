@@ -1,7 +1,8 @@
 // Host side of the D3 dispersion C ABI (include/sevenn_b200.h, "D3" section): parameters, cell list, the set-up of
 // one structure (host arrays) or of a batch (device arrays, s7b_d3_set_system_batch), stage launches, per-structure
-// results, the Hessian-vector product (s7b_d3_hvp_strain) and the reference-named entry points (pair_init ... pair_fin)
-// that sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh, d3_hvp_kernels.cuh.
+// results, the Hessian-vector product (s7b_d3_hvp_strain), the heat flux (s7b_d3_heat_flux) and the reference-named
+// entry points (pair_init ... pair_fin) that sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh,
+// d3_hvp_kernels.cuh, d3_flux_kernels.cuh.
 #include <dlfcn.h>
 
 #include <algorithm>
@@ -15,6 +16,7 @@
 
 #include "../../include/sevenn_b200.h"
 #include "common.cuh"
+#include "d3_flux_kernels.cuh"
 #include "d3_hvp_kernels.cuh"
 #include "d3_kernels.cuh"
 
@@ -62,6 +64,8 @@ struct S7bD3 {
   int stages_done = 0;
   // Hessian-vector product scratch, allocated on its first call
   D3Buf hv_v, hv_dcn, hv_dWt, hv_dW1t, hv_ddc, hv_force, hv_spair, hv_schain, hv_sigma, hv_energy, hv_oute, hv_dvir;
+  // heat-flux scratch, allocated on its first call
+  D3Buf fx_v, fx_cn4, fx_nb, fx_out, fx_energy, fx_sums;
   std::vector<double> host_force;      // reference ABI: pair_get_force returns a pointer
   double host_energy = 0.0, host_sigma[6] = {0, 0, 0, 0, 0, 0};
   // reference-ABI staging (pair_set_atom / pair_set_domain / pair_run_settings / pair_run_coeff)
@@ -141,7 +145,8 @@ void s7b_d3_destroy(S7bD3* d) {
                    &d->xs, &d->ts, &d->ss, &d->bin_of, &d->W, &d->dW, &d->logD, &d->near_, &d->cn, &d->dc6i,
                    &d->force, &d->eatom, &d->spair, &d->schain, &d->energy, &d->sigma, &d->out_force,
                    &d->hv_v, &d->hv_dcn, &d->hv_dWt, &d->hv_dW1t, &d->hv_ddc, &d->hv_force, &d->hv_spair,
-                   &d->hv_schain, &d->hv_sigma, &d->hv_energy, &d->hv_oute, &d->hv_dvir};
+                   &d->hv_schain, &d->hv_sigma, &d->hv_energy, &d->hv_oute, &d->hv_dvir,
+                   &d->fx_v, &d->fx_cn4, &d->fx_nb, &d->fx_out, &d->fx_energy, &d->fx_sums};
   for (D3Buf* b : bufs) b->release();
   delete d;
 }
@@ -396,7 +401,8 @@ int s7b_d3_run_stage(S7bD3* d, int32_t stage, int32_t i_begin, int32_t i_end, vo
 
 // device buffers, bin-sorted atom order: "cn" double[n], "dc6i" double[n], "force" double[n,3] (hartree/bohr),
 // "energy" double[B] (hartree), "sigma" double[B,6] (hartree; xx,yy,zz,xy,xz,yz), "order" int[n] (sorted -> caller index),
-// "type" int[n] (type word: after a batched set-up Z - 1 | local type << 8, else the type index)
+// "type" int[n] (type word: after a batched set-up Z - 1 | local type << 8, else the type index), "eatom" double[n]
+// (hartree, the atomic energies of the pair pass)
 void* s7b_d3_buffer(S7bD3* d, const char* name, size_t* numel) {
   if (!d || !name) return nullptr;
   const std::string nm(name);
@@ -409,6 +415,7 @@ void* s7b_d3_buffer(S7bD3* d, const char* name, size_t* numel) {
   else if (nm == "sigma") { p = d->sigma.p; n = (size_t)d->B * 6; }
   else if (nm == "order") { p = d->idx_sorted.p; n = d->n; }
   else if (nm == "type") { p = d->ts.p; n = d->n; }
+  else if (nm == "eatom") { p = d->eatom.p; n = d->n; }
   if (numel) *numel = n;
   return p;
 }
@@ -510,6 +517,49 @@ int s7b_d3_hvp_strain(S7bD3* d, const double* d_v, const double* d_strain, doubl
                                                                   d->hv_energy.as<double>(), d->hv_sigma.as<double>(),
                                                                   d->hv_oute.as<double>(), d_out,
                                                                   d_dvirial ? d_dvirial : d->hv_dvir.as<double>());
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// Potential part of the heat flux of D3's atomic energies, J_pot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i) per
+// structure, and sum_j U_j v_j, on the current system with its forward (stages 1-3 over [0, n)) held: two passes on
+// scratch (d3_flux_kernels.cuh), then the forward's own sums kernel; no forward buffer is written.
+int s7b_d3_heat_flux(S7bD3* d, const double* d_v, double* d_jpot, double* d_ju, void* stream) {
+  if (!d || !d->have_system) return d3_fail("D3: no system set");
+  if (d->stages_done < 3)
+    return d3_fail("D3: the heat flux needs stages 1, 2 and 3 run over all atoms [0, n) of the current system first");
+  const int n = d->n, B = d->B;
+  if (!d_jpot || (n > 0 && !d_v)) return d3_fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (n == 0) {
+    S7B_CUDA_CHECK(cudaMemsetAsync(d_jpot, 0, (size_t)B * 24, st));
+    if (d_ju) S7B_CUDA_CHECK(cudaMemsetAsync(d_ju, 0, (size_t)B * 24, st));
+    return 0;
+  }
+  const size_t N = (size_t)n, Bs = (size_t)B;
+  int rc = 0;
+  rc |= d->fx_v.ensure(N * 24); rc |= d->fx_cn4.ensure(N * 32); rc |= d->fx_nb.ensure(N * 32); rc |= d->fx_out.ensure(N * 48);
+  rc |= d->fx_energy.ensure(Bs * 8); rc |= d->fx_sums.ensure(Bs * 48);
+  if (rc) return d3_fail("cudaMalloc failed for the D3 heat flux");
+  const bool bt = d->batched;
+  const D3Params& P = bt ? d->Pe : d->P;
+  const D3Atoms A = d3_atoms(d);
+  D3Flux X;
+  X.v = d->fx_v.as<double>();
+  X.eatom = d->eatom.as<double>();
+  X.cn4 = d->fx_cn4.as<double>();
+  X.nb = d->fx_nb.as<float4>();
+  X.out = d->fx_out.as<double>();
+  const int grd = (n + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
+  d3_hvp_gather_kernel<<<(3 * n + 255) / 256, 256, 0, st>>>(n, d->idx_sorted.as<int>(), d_v, d->fx_v.as<double>());
+  if (bt) d3_flux_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, X);
+  else d3_flux_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, X);
+  if (bt) d3_flux_pair_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, X);
+  else d3_flux_pair_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, X);
+  // per structure: R in the sums' first three slots, eatom v in the last three (the energy sum goes to scratch)
+  d3_system_sums_kernel<<<B, kD3SumBlock, 0, st>>>(d->aptr.as<int>(), 0, n, X.eatom, X.out, d->fx_energy.as<double>(),
+                                                   d->fx_sums.as<double>());
+  d3_flux_results_kernel<<<(3 * B + 255) / 256, 256, 0, st>>>(B, d->fx_sums.as<double>(), d_jpot, d_ju);
   S7B_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

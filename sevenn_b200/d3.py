@@ -20,6 +20,7 @@ from .engine import _host, check, load_library
 
 _PARAMS = None
 AU_TO_ANG = 0.52917726
+AU_TO_EV = 27.21138505
 
 
 def d3_tables():
@@ -157,6 +158,34 @@ class D3Engine:
     def hvp(self, v):
         """H v = (d2E/dr dr) v of the D3 energy, [n, 3] float64 device tensor in eV/A^2 x A: ``hvp_strain(v)[0]``."""
         return self.hvp_strain(v)[0]
+
+    def atomic_energies(self):
+        """D3's atomic energies U_j = -1/2 sum_{k,tau} C6_jk g(r_jk) of the last pair stage (self images included; they
+        sum to the energy), [n] float64 device tensor in eV, caller's atom order"""
+        torch = self.torch
+        out = torch.zeros(self.n, dtype=torch.float64, device=self.device)
+        if self.n:
+            order = self.buffer('order', dtype='i4').long()
+            out[order] = self.buffer('eatom') * AU_TO_EV
+        return out
+
+    def heat_flux(self, v):
+        """Heat flux of D3's atomic energies (C ABI ``s7b_d3_heat_flux``, DESIGN.md §8.4) with the forward of the last
+        three stages over all atoms held.  v [n, 3] velocities (Angstrom x any time unit, caller's atom order), numpy or
+        torch (any device).  Returns (jpot, ju), [B, 3] float64 device tensors, B = the structure count of the last
+        ``D3Batch.compute``, else 1: jpot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i) over every atom and periodic
+        image i that U_j depends on, ju = sum_j U_j v_j (U_j = ``atomic_energies``).  Units: eV A x (the unit of v).
+        Two cell-list passes; a periodic cell needs no unfolding."""
+        torch = self.torch
+        n, B = self.n, self.B
+        v = torch.as_tensor(v).to(self.device, torch.float64).contiguous()
+        if v.numel() != 3 * n or (v.dim() == 2 and v.shape[1] != 3) or v.dim() > 2:
+            raise ValueError(f'v has {tuple(v.shape)}, expected [{n}, 3] (atoms)')
+        jpot = torch.empty(B, 3, dtype=torch.float64, device=self.device)
+        ju = torch.empty(B, 3, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self.lib.s7b_d3_heat_flux(self._h, v.data_ptr(), jpot.data_ptr(), ju.data_ptr(), self._stream()))
+        return jpot, ju
 
 
 def distributed_d3(engine: D3Engine, numbers, positions, cell, pbc=(True, True, True), group=None):
@@ -296,6 +325,13 @@ class D3Batch:
             raise RuntimeError('no batch: call compute first')
         return self.engine.hvp_strain(v, strain)
 
+    def heat_flux(self, v):
+        """``D3Engine.heat_flux`` on the last batch: v [n, 3] velocities -> (jpot [B, 3], ju [B, 3]), float64 device
+        tensors.  Each structure's flux is that of the structure alone."""
+        if self.atom_ptr is None:
+            raise RuntimeError('no batch: call compute first')
+        return self.engine.heat_flux(v)
+
 
 try:
     from ase.calculators.calculator import Calculator as _Base, all_changes as _all_changes
@@ -323,6 +359,10 @@ class D3Calculator(_Base):
         super().__init__(**kwargs)
         self.rthr, self.cnthr = vdw_cutoff, cn_cutoff
         self.engine = D3Engine(damping_type, functional_name, vdw_cutoff, cn_cutoff, device=device)
+        self._engine_inputs = None     # (numbers, positions, cell, pbc) of the engine's current forward
+
+    def _remember(self, numbers, pos, cell, pbc):
+        self._engine_inputs = tuple(np.array(a, copy=True) for a in (numbers, pos, cell, pbc))
 
     def _inputs(self, atoms):
         """(numbers, positions, cell, pbc, generated) that ``calculate`` evaluates ``atoms`` with; a structure without
@@ -347,6 +387,7 @@ class D3Calculator(_Base):
             atoms.set_cell(cell)
             atoms.set_pbc(pbc)
         energy, forces, s = self.engine.compute(numbers, pos, cell, pbc)
+        self._remember(numbers, pos, cell, pbc)
         vol = abs(np.linalg.det(cell))
         stress = -np.array([s[0], s[1], s[2], s[5], s[4], s[3]]) / vol        # calculator.py:515-526 + /volume (:608)
         self.results = {'free_energy': energy, 'energy': energy, 'forces': forces, 'stress': stress}
@@ -358,6 +399,34 @@ class D3Calculator(_Base):
         self.engine.set_system(numbers, pos, cell, pbc)
         for stage in (1, 2, 3):
             self.engine.run_stage(stage)
+        self._remember(numbers, pos, cell, pbc)
+
+    def _flux_parts(self, atoms):
+        """(J_pot [3], sum_j U_j v_j [3], velocities [n, 3]) of ``atoms``; the three stages run only when numbers,
+        positions, cell or pbc (as ``calculate`` evaluates them) differ from those of the engine's current forward"""
+        numbers, pos, cell, pbc, _ = self._inputs(atoms)
+        last = self._engine_inputs
+        if last is None or not all(np.array_equal(a, b) for a, b in zip(last, (numbers, pos, cell, pbc))):
+            self._forward(atoms)
+        v = np.asarray(atoms.get_velocities(), dtype=np.float64).reshape(-1, 3)
+        jpot, ju = self.engine.heat_flux(v)
+        return jpot[0].cpu().numpy(), ju[0].cpu().numpy(), v
+
+    def get_heat_flux(self, atoms=None, convective: bool = True) -> np.ndarray:
+        """Energy-barycentre heat flux of the D3 energy of ``atoms`` (default: the calculator's atoms), [3] float64
+        (``SevenNetCalculator.get_heat_flux``'s definition and units, DESIGN.md §8.4): J_pot + sum_j (U_j + m_j |v_j|^2
+        / 2) v_j with D3's atomic energies U_j (``D3Engine.atomic_energies``).  Velocities and masses come from
+        ``atoms``; ``convective=False`` gives J_pot alone.  A structure without a cell is evaluated in ``calculate``'s
+        generated cell (``atoms`` is not modified).  The three stages run only when positions, numbers, cell or pbc
+        differ from those of the last D3 forward; ``results`` is not touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        jpot, ju, v = self._flux_parts(atoms)
+        if not convective:
+            return jpot
+        from .heat_flux import kinetic_flux
+        return jpot + ju + kinetic_flux(v, atoms.get_masses())[0]
 
     def get_hessian(self, atoms=None) -> np.ndarray:
         """Hessian d2E/dr dr of the D3 energy of ``atoms`` (default: the calculator's atoms), [3N, 3N] float64 in
@@ -458,3 +527,18 @@ class SevenNetD3Calculator(_Base):
         dv_a, outs_a, vol, h_a = self.sevennet_calc._strain_pieces(atoms, relaxed)
         dv_b, outs_b, _, h_b = self.d3_calc._strain_pieces(atoms, relaxed)
         return elastic.elastic_tensor(dv_a + dv_b, outs_a + outs_b, vol, h_a + h_b if relaxed else None)
+
+    def get_heat_flux(self, atoms=None, convective: bool = True) -> np.ndarray:
+        """Energy-barycentre heat flux of the network plus D3 energy, [3] float64 (``SevenNetCalculator.
+        get_heat_flux``'s definition and units): the atomic energies are the network's plus D3's, so J_pot and
+        sum_j U_j v_j are the sums of the two terms', and the kinetic part sum_j m_j |v_j|^2 / 2 v_j is added once.
+        Each term's forward runs only when the atoms changed since its last one; ``results`` is not touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        jp_a, ju_a, v = self.sevennet_calc._flux_parts(atoms)
+        jp_b, ju_b, _ = self.d3_calc._flux_parts(atoms)
+        if not convective:
+            return jp_a + jp_b
+        from .heat_flux import kinetic_flux
+        return jp_a + jp_b + ju_a + ju_b + kinetic_flux(v, atoms.get_masses())[0]

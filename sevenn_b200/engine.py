@@ -67,6 +67,7 @@ EXPORTS = [
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
     's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain', 's7b_engine_heat_flux',
+    's7b_d3_heat_flux',
 ]
 
 
@@ -112,6 +113,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_d3_set_system_batch.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]
     lib.s7b_d3_system_results.argtypes = [vp, vp, vp, vp, vp]
     lib.s7b_d3_hvp_strain.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.s7b_d3_heat_flux.argtypes = [vp, vp, vp, vp, vp]
     lib.s7b_engine_set_param.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, vp, sz]
     lib.s7b_engine_set_graph.argtypes = [vp, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.s7b_engine_run_stage.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]

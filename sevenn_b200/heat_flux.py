@@ -14,8 +14,9 @@ eV, ASE time) m v^2 / 2 is in eV and ``J * ase.units.fs`` is in eV A^2/fs.
 The engine computes J_pot and sum_j U_j v_j in one tangent-forward CUDA pass of four channels
 (``B200Engine.heat_flux``, C ABI ``s7b_engine_heat_flux``): T_j = sum_i dh_j/dr_i . v_i and
 R_j,a = sum_i (r_j - r_i)_a (dh_j/dr_i . v_i) for every node feature h_j, carried through the layers with edge vectors
-only, so a periodic cell needs no unfolding; J_pot,a = sum_j scale_s readout(R_j,a).  This module adds the kinetic
-part, which needs the masses.
+only, so a periodic cell needs no unfolding; J_pot,a = sum_j scale_s readout(R_j,a).  D3 dispersion's atomic energies
+have their own two-pass flux (``d3.D3Engine.heat_flux``, DESIGN.md §8.4), which adds to this one.  This module adds the
+kinetic part, which needs the masses.
 """
 import numpy as np
 
