@@ -4,6 +4,8 @@
 #include "pair_e3gnn_b200.h"
 
 #include <string>
+#include <type_traits>
+#include <utility>
 
 #include "atom.h"
 #include "error.h"
@@ -16,12 +18,24 @@
 
 using namespace LAMMPS_NS;
 
+namespace {
+// Whether the LAMMPS Pair class carries the per-atom centroid virial (cvatom / centroidstressflag, LAMMPS since
+// stable_29Oct2020).  Against older Pair declarations the style builds without centroid support and LAMMPS keeps
+// its default for it.
+template <class P, class = void>
+struct HasCentroid : std::false_type {};
+template <class P>
+struct HasCentroid<P, std::void_t<decltype(std::declval<P &>().cvatom), decltype(std::declval<P &>().centroidstressflag)>>
+    : std::true_type {};
+}  // namespace
+
 PairE3GNNB200::PairE3GNNB200(LAMMPS *lmp) : Pair(lmp) {
   single_enable = 0;
   restartinfo = 0;
   one_coeff = 1;
   manybody_flag = 1;
   no_virial_fdotr_compute = 1;     // the virial comes from the edge forces, not from f . r
+  centroid_setup(this);
 }
 
 PairE3GNNB200::~PairE3GNNB200() {
@@ -161,5 +175,35 @@ void PairE3GNNB200::compute(int eflag, int vflag) {
     const int lm[6] = {0, 1, 2, 3, 5, 4};      // LAMMPS (xx, yy, zz, xy, xz, yz)
     for (int r = 0; r < nlocal; ++r)
       for (int q = 0; q < 6; ++q) vatom[ilist[r]][q] += vatom_buf[(size_t)r * 6 + lm[q]];
+  }
+  centroid_rows(this, nlocal, ilist);
+}
+
+// cvatom is the library's exact per-atom centroid virial (CENTROID_AVAIL, value 1 in LAMMPS's enum; the literal keeps
+// this branch free of names an older Pair does not declare)
+template <class P>
+void PairE3GNNB200::centroid_setup(P *self) {
+  if constexpr (HasCentroid<P>::value) self->centroidstressflag = 1;
+}
+
+// compute centroid/stress/atom (cvflag_atom): the library's centroid virial Wc_i[a][b] = sum_j (r_j - r_i)_a
+// dU_j/dr_i,b (row-major, DESIGN.md §8.5), exact for the message-passing model, so that compute heat/flux's
+// J_a = sum_b Wc_i[a][b] v_i,b is the model's potential flux.  The graph has no ghost rows (images map to their
+// owners), so every row is an owned atom's.  LAMMPS order: xx yy zz xy xz yz yx zx zy.
+template <class P>
+void PairE3GNNB200::centroid_rows(P *self, int nlocal, const int *ilist) {
+  if constexpr (HasCentroid<P>::value) {
+    if (!self->cvflag_atom) return;
+    cvatom_buf.resize((size_t)nlocal * 9);
+    if (s7b_engine_centroid_virial_host(engine, cvatom_buf.data(), nullptr))
+      error->one(FLERR, (std::string("e3gnn/b200: compute centroid/stress/atom needs the radial MLP in the model file "
+                                     "(export_flat(..., radial_mlp=True)): ") + s7b_last_error()).c_str());
+    const int lm[9] = {0, 4, 8, 1, 2, 5, 3, 6, 7};
+    for (int r = 0; r < nlocal; ++r)
+      for (int q = 0; q < 9; ++q) self->cvatom[ilist[r]][q] += cvatom_buf[(size_t)r * 9 + lm[q]];
+  } else {
+    (void)self;
+    (void)nlocal;
+    (void)ilist;
   }
 }

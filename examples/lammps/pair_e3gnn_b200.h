@@ -5,7 +5,9 @@
  *
  * Same user contract as the reference's serial `pair_style e3gnn` (sevenn/pair_e3gnn/pair_e3gnn.cpp:
  * 302-411): metal units, `newton_pair on`, a full neighbour list, an atom map (`atom_modify map yes`),
- * one process.  The model file comes from sevenn_b200/export.py:export_flat instead of `sevenn
+ * one process.  Per-atom virial: `compute stress/atom` gets the pairwise split of the reference; `compute
+ * centroid/stress/atom` gets the exact per-atom centroid virial, the one `compute heat/flux` needs for Green-Kubo
+ * (DESIGN.md §8.5; a Pair class without the centroid members builds the style without it).  The model file comes from sevenn_b200/export.py:export_flat instead of `sevenn
  * get_model` (TorchScript); there is no libtorch in this pair style.
  * Written against LAMMPS stable_2Aug2023.  LAMMPS is not in the image: this repository compiles it against the
  * minimal declarations in tests/mock_lammps/ and runs it there on the CPU against a toy double of the library
@@ -38,6 +40,8 @@ class PairE3GNNB200 : public Pair {
 
  protected:
   void allocate();
+  template <class P> void centroid_setup(P *self);
+  template <class P> void centroid_rows(P *self, int nlocal, const int *ilist);
 
   S7bEngine *engine = nullptr;
   double cutoff = 0.0;
@@ -45,6 +49,7 @@ class PairE3GNNB200 : public Pair {
   // host staging, reused between steps
   std::vector<int> species, edge_centre, edge_neighbour, row_of_atom;
   std::vector<float> edge_vec, forces, eatom_buf, vatom_buf;
+  std::vector<double> cvatom_buf;
   bool atomic_virial_on = false;
 };
 

@@ -227,6 +227,22 @@ S7B_API int s7b_engine_hvp_strain(S7bEngine* eng, const float* d_v, const double
  * those of s7b_engine_hvp.  E == 0 gives J_pot = 0.  Buffers are allocated on the first call and kept. */
 S7B_API int s7b_engine_heat_flux(S7bEngine* eng, const float* d_v, double* d_jpot, double* d_ju, void* stream);
 
+/* Per-atom centroid virial (DESIGN.md §8.5), the quantity LAMMPS's compute centroid/stress/atom holds:
+ *   Wc_i[a][b] = sum_j sum_{i'} (r_j - r_i')_a dU_j/dr_i',b      (eV; not symmetric)
+ * i' over atom i and every periodic image of it, j over the structure's atoms, U_j the atomic energies of the last
+ * s7b_engine_compute (per-species scale and shift included), r_j - r_i' the real vector between the two atoms.  Row a
+ * is the flux direction, column b the velocity / force direction.  It satisfies sum_i Wc_i = the virial
+ * -sum_e vec_e (x) f_e, and sum_i Wc_i v_i = J_pot of s7b_engine_heat_flux for any velocities; for a one-layer model
+ * Wc_k = -sum_{e: neighbour k} vec_e (x) f_e (the atomic_virial rows, unsymmetrised).  One reverse pass of four
+ * adjoint channels on that graph and forward; a periodic cell needs no unfolding.
+ *   d_out [n_nodes,9] f64 (device), overwritten, row-major per atom.
+ * A graph from s7b_engine_set_positions_batch gives each atom its structure's value (no edge joins two structures).
+ * Preconditions and refusals are those of s7b_engine_hvp (no ghost atoms: n_local == n_nodes).  E == 0 gives zeros.
+ * Buffers are those of s7b_engine_heat_flux, allocated on the first call of either and kept. */
+S7B_API int s7b_engine_centroid_virial(S7bEngine* eng, double* d_out, void* stream);
+/* The same into host memory host_out [n_nodes,9] (synchronises the stream), for hosts without a device allocator. */
+S7B_API int s7b_engine_centroid_virial_host(S7bEngine* eng, double* host_out, void* stream);
+
 /* Device pointer to an engine-owned buffer (valid until the next set_graph that grows it):
  * "x" (layer t input after self_interaction_1, [n_nodes, dim_x(t)]), "dx", "gate_in", "mid",
  * "h", "energy" (double[1]), "atomic_energy" [n_local], "atomic_energy_f64" (double[n_local], the same

@@ -180,6 +180,13 @@ class DeviceBatch:
         jk = kinetic_flux(_host(velocities), _host(masses), self.atom_ptr)
         return jpot + ju + torch.as_tensor(jk, dtype=torch.float64, device=jpot.device)
 
+    def centroid_virials(self):
+        """Per-atom centroid virial of every atom of the batch of the last ``compute``, [n, 3, 3] float64 device tensor
+        in eV, in the atom order of ``compute`` (``B200Engine.centroid_virial``, DESIGN.md §8.5).  The union graph has
+        no edge between structures, so each row is its structure's alone: summed over a structure's atoms it is that
+        structure's virial, and contracted with its velocities its J_pot.  D3 dispersion is not included."""
+        return self.engine.centroid_virial()
+
     def elastic_tensors(self, numbers, positions, cells, pbc, system_idx, relaxed: bool = True, d3=None) -> np.ndarray:
         """Elastic tensors of every structure, [B, 6, 6] float64 in eV/A^3 (``SevenNetCalculator.get_elastic_tensor``'s
         definition, units and Voigt order, per structure; inputs as ``compute``).  Every structure must be periodic in

@@ -198,15 +198,38 @@ class SevenNetCalculator(_Base):
             J = J + ju + kinetic_flux(v, atoms.get_masses())[0]
         return J
 
-    def _flux_parts(self, atoms):
-        """(J_pot [3], sum_j U_j v_j [3], velocities [n, 3]) of ``atoms``; the energy/force step runs only when
-        positions, numbers, cell or pbc differ from those of the last calculation"""
+    def get_centroid_virials(self, atoms=None) -> np.ndarray:
+        """Per-atom centroid virial of ``atoms`` (default: the calculator's atoms), [N, 3, 3] float64 in eV
+        (``B200Engine.centroid_virial``, DESIGN.md §8.5):
+
+          Wc_i[a, b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b
+
+        with U_j the atomic energies ('energies'), i' atom i and its periodic images.  Row a is the flux direction,
+        column b the velocity direction: sum_i Wc_i v_i is ``get_heat_flux(convective=False)`` for any velocities, and
+        sum_i Wc_i is the virial.  This is the quantity of LAMMPS's ``compute centroid/stress/atom`` (times -1 / V for
+        a stress); the symmetric pairwise split of ``compute_atomic_virial`` ('stresses') is not, for a model of more
+        than one layer.  One reverse pass of four channels; the energy/force step runs only when positions, numbers,
+        cell or pbc differ from those of the last calculation.  ``results`` are not touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        self._step_if_changed(atoms)
+        return self.engine.centroid_virial().cpu().numpy()
+
+    def _step_if_changed(self, atoms):
+        """Leave the engine on the graph and forward of ``atoms``: the energy/force step runs only when positions,
+        numbers, cell or pbc differ from those of the last calculation"""
         species, pos, cell, pbc, numbers = self._inputs(atoms)
         last = self._engine_inputs
         if last is None or not all(np.array_equal(a, b) for a, b in zip(last, (pos, cell, pbc, numbers))):
             self.engine.set_positions(species, pos, cell, pbc)
             self.engine.compute()
             self._remember(pos, cell, pbc, numbers)
+
+    def _flux_parts(self, atoms):
+        """(J_pot [3], sum_j U_j v_j [3], velocities [n, 3]) of ``atoms``; the energy/force step runs only when
+        positions, numbers, cell or pbc differ from those of the last calculation"""
+        self._step_if_changed(atoms)
         v = np.asarray(atoms.get_velocities(), dtype=np.float64).reshape(-1, 3)
         jpot, ju = self.engine.heat_flux(v.astype(np.float32))
         return jpot[0].cpu().numpy(), ju[0].cpu().numpy(), v

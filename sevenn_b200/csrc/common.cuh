@@ -86,6 +86,20 @@ struct FluxTangents {
   size_t x_stride, dr_stride, dY_stride, out_stride;
 };
 
+// Operands of the centroid virial's four-channel convolution backward (conv_centroid_bwd_kernel): the channel c's
+// array starts at c times its stride.  g [4][n_nodes, dim_mid]: the adjoints (A, B_x, B_y, B_z) of mid; w1 = dw/dr
+// [E, W]; vec = edge_vec [E, 3].  Accumulated: dx [4][n_nodes, dim_x] (null: not needed, the first layer),
+// dY [4][E, y_stride] (dE/dY_1..), dr [4][E] (dE/dr through w).
+struct CentroidAdjoints {
+  const float* g;
+  const float* w1;
+  const float* vec;
+  float* dx;
+  float* dY;
+  float* dr;
+  size_t g_stride, x_stride, dY_stride, dr_stride;
+};
+
 }  // namespace s7b
 
 #define S7B_CUDA_CHECK(expr)                                                            \

@@ -11,7 +11,9 @@ namespace s7b {
   int launch_conv_bwdt_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const ConvTangents&, const float*, \
                                    float*, float*, float*, cudaStream_t); \
   int launch_conv_flux_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const FluxTangents&, int, int*, float*, \
-                                   cudaStream_t);
+                                   cudaStream_t); \
+  int launch_conv_centroid_##LF##_##LO(int, const ConvArgs&, const ConvRole&, const CentroidAdjoints&, int, int*, \
+                                       cudaStream_t);
 S7B_DECL_GROUP(1, 0) S7B_DECL_GROUP(1, 1) S7B_DECL_GROUP(1, 2) S7B_DECL_GROUP(1, 3)
 S7B_DECL_GROUP(2, 0) S7B_DECL_GROUP(2, 1) S7B_DECL_GROUP(2, 2) S7B_DECL_GROUP(2, 3)
 S7B_DECL_GROUP(3, 0) S7B_DECL_GROUP(3, 1) S7B_DECL_GROUP(3, 2) S7B_DECL_GROUP(3, 3)
@@ -87,6 +89,17 @@ int launch_conv_flux(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& 
   if (a.n_dst <= a.n_begin) return 0;      // empty centre range
   int rc = 2;
   if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(flux, l1, a, role, f, c0, nch, out, st)
+  return conv_status(rc);
+}
+
+// One walk of the centroid virial's convolution backward over the channels c0 .. c0 + *nch - 1 (*nch set from the
+// kind)
+int launch_conv_centroid(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const CentroidAdjoints& g,
+                         int c0, int* nch, cudaStream_t st) {
+  *nch = 4;
+  if (a.n_dst <= a.n_begin) return 0;      // empty centre range
+  int rc = 2;
+  if (lf >= 1 && lf <= 3 && lo >= 0 && lo <= 3) S7B_GROUP_SWITCH(centroid, l1, a, role, g, c0, nch, st)
   return conv_status(rc);
 }
 

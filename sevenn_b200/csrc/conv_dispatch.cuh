@@ -168,6 +168,26 @@ static int flux_kind_rt(const ConvArgs& a, const ConvRole& role, const FluxTange
   return launch_flux_one<Kind, 16>(a, role, f, c0, nch, out, st);
 }
 
+// Centroid virial (engine.cu s7b_engine_centroid_virial): the lane mapping of the flux, centroid_channels<Kind>()
+// of the four adjoint channels per walk
+template <class Kind, int LPN>
+static int launch_centroid_one(const ConvArgs& a, const ConvRole& role, const CentroidAdjoints& g, int c0, int* nch,
+                               cudaStream_t st) {
+  constexpr int NCH = centroid_channels<Kind>();
+  *nch = NCH;
+  conv_centroid_bwd_kernel<Kind, LPN, NCH><<<conv_grid<0, 1, LPN>(a, role), 32 * kConvWarpsPerBlock, 0, st>>>(
+      a, role, g, c0);
+  return cudaGetLastError() == cudaSuccess ? 0 : 1;
+}
+
+template <class Kind>
+static int centroid_kind_rt(const ConvArgs& a, const ConvRole& role, const CentroidAdjoints& g, int c0, int* nch,
+                            cudaStream_t st) {
+  if (role.mul <= 0 || role.mul % 32 != 0) return kConvWrongMul;
+  if (role.mul % 64 == 0) return launch_centroid_one<Kind, 32>(a, role, g, c0, nch, st);
+  return launch_centroid_one<Kind, 16>(a, role, g, c0, nch, st);
+}
+
 // Paths (l2, l3) of the kind (l1, lmax_filter, lmax_out): the triangle rule with l2 <= LF, l3 <= LO
 constexpr int tp_npath(int l1, int lf, int lo) {
   int n = 0;
@@ -224,12 +244,20 @@ static int flux_role(const ConvArgs& a, const ConvRole& role, const FluxTangents
   else return flux_kind_rt<TPKind<L1, LF, LO>>(a, role, f, c0, nch, out, st);
 }
 
+template <int L1, int LF, int LO>
+static int centroid_role(const ConvArgs& a, const ConvRole& role, const CentroidAdjoints& g, int c0, int* nch,
+                         cudaStream_t st) {
+  if constexpr (tp_npath(L1, LF, LO) == 0) return kConvNoPath;
+  else return centroid_kind_rt<TPKind<L1, LF, LO>>(a, role, g, c0, nch, st);
+}
+
 }  // namespace s7b
 
 // Defines  launch_conv_fwd_LF_LO / launch_conv_bwd_LF_LO  for l1 = 0..3.  SPEC = 1 for the groups of SevenNet-0
 // and SevenNet-l3i5, which also get the kernels specialised for the widths kConvMul (l1 = 3 only with LF = 3);
 // the other groups have only the runtime-width kernels.  launch_conv_jvp_LF_LO / launch_conv_bwdt_LF_LO: the
-// second-order kernels, runtime width in every group; launch_conv_flux_LF_LO: the heat flux's, likewise.
+// second-order kernels, runtime width in every group; launch_conv_flux_LF_LO / launch_conv_centroid_LF_LO: the heat
+// flux's and the centroid virial's, likewise.
 #define S7B_CONV_SPEC_MUL(SPEC, LF, L1) ((SPEC) && ((L1) < 3 || (LF) >= 3) ? s7b::kConvMul[L1] : 0)
 #define S7B_DEFINE_CONV_GROUP(LF, LO, SPEC)                                                        \
   namespace s7b {                                                                                  \
@@ -283,6 +311,16 @@ static int flux_role(const ConvArgs& a, const ConvRole& role, const FluxTangents
       case 1: return flux_role<1, LF, LO>(a, role, f, c0, nch, out, st);                           \
       case 2: return flux_role<2, LF, LO>(a, role, f, c0, nch, out, st);                           \
       case 3: return flux_role<3, LF, LO>(a, role, f, c0, nch, out, st);                           \
+    }                                                                                              \
+    return 1;                                                                                      \
+  }                                                                                                \
+  int launch_conv_centroid_##LF##_##LO(int l1, const ConvArgs& a, const ConvRole& role,            \
+                                       const CentroidAdjoints& g, int c0, int* nch, cudaStream_t st) { \
+    switch (l1) {                                                                                  \
+      case 0: return centroid_role<0, LF, LO>(a, role, g, c0, nch, st);                            \
+      case 1: return centroid_role<1, LF, LO>(a, role, g, c0, nch, st);                            \
+      case 2: return centroid_role<2, LF, LO>(a, role, g, c0, nch, st);                            \
+      case 3: return centroid_role<3, LF, LO>(a, role, g, c0, nch, st);                            \
     }                                                                                              \
     return 1;                                                                                      \
   }                                                                                                \

@@ -667,6 +667,124 @@ conv_flux_jvp_kernel(const ConvArgs a, const ConvRole role, const FluxTangents f
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// centroid virial (engine.cu s7b_engine_centroid_virial, DESIGN.md §8.5): the backward of conv_bwd_kernel (stored
+// weights) for the channels c = c0 .. c0 + NCH - 1 of the four adjoints (A, B_x, B_y, B_z) of mid, in one walk of
+// the row.  The centre's A and B are held in registers; x, Y, w and w' are read once per edge and shared by the
+// channels.  Edge e (centre n, neighbour k, vector vec) gives channel c the adjoint
+//   g_c = A[n]                      (c = 0)
+//         B_a[n] - vec_a A[n]       (c = 1 + a, formed in registers)
+// and, with TP the edge's tensor product,
+//   dx[c][k]  += TP_x^T(g_c)                                 (RED.ADD.F32x2, c.dx not null)
+//   dY[c][e]  += sum_u dE/dY                                  (group reduction)
+//   dr[c][e]  += sum_{p,u} (dE/dw_{p,u}) w'_{p,u}            (dE/dr through w, folded in registers)
+// The per-edge sums go atomic when the role spans several CTAs (gridDim.y > 1), as in conv_bwd_kernel.  NCH is the
+// largest of 4, 2, 1 whose adjoints fit the register budget (centroid_channels); the host walks each row 4 / NCH
+// times.
+// ------------------------------------------------------------------------------------------
+template <class Kind>
+constexpr int centroid_channels() {
+  return Kind::NACC * 5 <= 50 ? 4 : (Kind::NACC * 3 <= 50 ? 2 : 1);
+}
+
+template <class Kind, int LPN, int NCH>
+__global__ void S7B_FWD_BOUNDS
+conv_centroid_bwd_kernel(const ConvArgs a, const ConvRole role, const CentroidAdjoints g, int c0) {
+  const LaneMap<1, LPN, 2> m(a);
+  if (m.nmax == 0) return;                    // uniform: no edges in any row of this warp
+  const int mul = role.mul;
+  const bool SPLIT = gridDim.y > 1;
+  const bool need_dx = g.dx != nullptr;
+
+  // A is held in registers where several channels share a walk; the widest kinds (one channel per walk) re-read it
+  // per edge from L1 instead (holding it spilled 100-900 bytes for the lmax-3 kinds)
+  constexpr bool A_REG = NCH > 1;
+  V2 gA[A_REG ? Kind::NACC : 1], gB[NCH][Kind::NACC];
+  const size_t ro = (size_t)(m.node_ok ? m.n : 0) * a.dim_mid + m.uc0;
+#pragma unroll
+  for (int p = 0; p < Kind::NPATH; ++p)
+#pragma unroll
+    for (int q = 0; q < 2 * Kind::path_l3(p) + 1; ++q) {
+      const size_t o = ro + role.out_off[p] + q * role.out_stride[p];
+      if constexpr (A_REG) gA[Kind::acc_off(p) + q] = ldg2(g.g + o);
+#pragma unroll
+      for (int k = 0; k < NCH; ++k) gB[k][Kind::acc_off(p) + q] = ldg2(g.g + (size_t)(c0 + k) * g.g_stride + o);
+    }
+
+  constexpr int NR = (Kind::NY <= 9) ? 8 : 16;   // values reduced with the transposing butterfly
+  constexpr int PER = LPN / NR;
+  const int idx = (m.sl / PER) % NR;                      // which reduced value ends up in this lane
+  const bool writer = (m.sl % PER) == 0 && idx + 1 < Kind::NY;
+  const unsigned xlane = role.x_off + m.uc0;
+  EdgeRecs<LPN> recs;
+  for (int it = 0; it < m.nmax; ++it) {
+    const bool valid = (LPN == 32) || (it < m.len);
+    const int e = valid ? m.e0 + it : 0;
+    if (it % LPN == 0) recs.fill(a, m.e0, m.len, it, m.sl);
+    const int4 rec = recs.get(it);
+    float Y[Kind::NY];
+    load_Y<Kind>(a.Y + row_offset(e, y_stride(Kind::NY)), Y);
+    float ev[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) ev[q] = __ldg(g.vec + 3 * (size_t)e + q);
+    const size_t xo = row_offset(rec.x, a.dim_x) + xlane;
+    const size_t wo = (size_t)e * a.w_numel + m.uc0;
+    V2 x[Kind::D1], w[Kind::NPATH], w1[Kind::NPATH];
+#pragma unroll
+    for (int i = 0; i < Kind::D1; ++i) x[i] = ldg2(a.x + xo + i * mul);
+#pragma unroll
+    for (int p = 0; p < Kind::NPATH; ++p) {
+      w[p] = ldg2(a.w + wo + role.w_off[p]);
+      w1[p] = ldg2(g.w1 + wo + role.w_off[p]);
+      if (LPN != 32 && !valid) w[p] = w1[p] = splat2(0.0f);   // every output has w or w' as a factor
+    }
+#pragma unroll
+    for (int k = 0; k < NCH; ++k) {
+      const int ch = c0 + k;
+      V2 gc[Kind::NACC], dY[Kind::NY], dwv[Kind::NPATH], dxv[Kind::D1];
+      const float s = ch > 0 ? -ev[ch - 1] : 0.0f;
+      if constexpr (A_REG) {
+#pragma unroll
+        for (int q = 0; q < Kind::NACC; ++q) gc[q] = ch > 0 ? fma_(s, gA[q], gB[k][q]) : gB[k][q];
+      } else {
+#pragma unroll
+        for (int p = 0; p < Kind::NPATH; ++p)
+#pragma unroll
+          for (int q = 0; q < 2 * Kind::path_l3(p) + 1; ++q) {
+            const int i = Kind::acc_off(p) + q;
+            gc[i] = ch > 0 ? fma_(s, ldg2(g.g + ro + role.out_off[p] + q * role.out_stride[p]), gB[k][i]) : gB[k][i];
+          }
+      }
+#pragma unroll
+      for (int j = 0; j < Kind::NY; ++j) dY[j] = splat2(0.0f);
+      Kind::bwd(x, Y, w, gc, dwv, dxv, dY);
+      V2 dr2 = splat2(0.0f);
+#pragma unroll
+      for (int p = 0; p < Kind::NPATH; ++p) dr2 = fma_(dwv[p], w1[p], dr2);
+      if (valid && need_dx) {
+        float* dxc = g.dx + (size_t)ch * g.x_stride + xo;
+#pragma unroll
+        for (int i = 0; i < Kind::D1; ++i) atomicAdd(reinterpret_cast<float2*>(dxc + i * mul), dxv[i]);
+      }
+      float red[NR];
+#pragma unroll
+      for (int j = 0; j < NR; ++j) red[j] = (j + 1 < Kind::NY) ? dY[j + 1].x + dY[j + 1].y : 0.0f;
+      group_reduce_multi<NR, LPN>(red, m.sl);
+      const float dEdr = group_sum<LPN>(dr2.x + dr2.y);
+      if (valid && writer) {
+        float* dst = g.dY + (size_t)ch * g.dY_stride + row_offset(e, y_stride(Kind::NY)) + idx;
+        if (SPLIT) atomicAdd(dst, red[0]);
+        else *dst += red[0];
+      }
+      if (valid && m.sl == 0) {
+        float* dst = g.dr + (size_t)ch * g.dr_stride + e;
+        if (SPLIT) atomicAdd(dst, dEdr);
+        else *dst += dEdr;
+      }
+    }
+  }
+}
+
 // One walk of conv_bwd_tangent_kernel over the CSR row of this lane's node, computing the outputs in OUT
 // (kTanDw | kTanDx | kTanDY)
 enum { kTanDw = 1, kTanDx = 2, kTanDY = 4 };

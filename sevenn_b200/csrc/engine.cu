@@ -22,6 +22,7 @@
 #include "hvp_kernels.cuh"
 #include "neighbor.cuh"
 #include "flux_kernels.cuh"
+#include "centroid_kernels.cuh"
 #include "node_kernels.cuh"
 #include "tc_gemm.cuh"
 
@@ -59,6 +60,8 @@ int launch_conv_bwd_tangent(int l1, int lf, int lo, const ConvArgs& a, const Con
                             const float* gout, float* dx, float* dY_acc, float* dw, cudaStream_t st);
 int launch_conv_flux(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0,
                      int* nch, float* out, cudaStream_t st);
+int launch_conv_centroid(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const CentroidAdjoints& g,
+                         int c0, int* nch, cudaStream_t st);
 
 static int64_t g_alloc_gen = 0;   // bumped by every (re)allocation: captured CUDA graphs hold raw pointers
 
@@ -216,15 +219,18 @@ struct HvpBufs {
 };
 
 // Buffers of the heat flux (s7b_engine_heat_flux), allocated on its first call and sized for one layer: every node
-// array holds the four channels (T, R_x, R_y, R_z) one after another, [4][n_nodes][widest row of any layer].
+// array holds the four channels (T, R_x, R_y, R_z) one after another, [4][n_nodes][widest row of any layer].  The
+// centroid virial (s7b_engine_centroid_virial) uses the same buffers for its four adjoint channels (A, B_x, B_y, B_z):
+// dr and dY then accumulate dE/dr and dE/dY over the layers, tx, dmid, tg and th hold the adjoints of x, mid, g and h.
 struct FluxBufs {
   DevBuf dr, dY;                  // [4][E], [4][E][ny_stride]: edge tangents
   DevBuf emb2, hA, hB, w2;        // radial jet [2][E][.]: w and w' of one layer
   DevBuf tx, dmid, tg, th;        // node tangents of one layer
   DevBuf atom_ptr1;               // {0, n} of a one-structure graph
+  DevBuf wc;                      // [n_nodes, 9] f64: the centroid virial of s7b_engine_centroid_virial_host
   RowExp re;
   void release() {
-    for (DevBuf* b : {&dr, &dY, &emb2, &hA, &hB, &w2, &tx, &dmid, &tg, &th, &atom_ptr1, &re.buf}) b->release();
+    for (DevBuf* b : {&dr, &dY, &emb2, &hA, &hB, &w2, &tx, &dmid, &tg, &th, &atom_ptr1, &wc, &re.buf}) b->release();
   }
 };
 
@@ -2089,6 +2095,92 @@ int s7b_engine_heat_flux(S7bEngine* e, const float* d_v, double* d_jpot, double*
                                             Lz.dim_h, G.readout.as<float>(), G.readout_lo.as<float>(), G.scale.as<float>(),
                                             e->d_species, e->atomic_energy64.as<double>(), d_v, edges ? d_jpot : nullptr, d_ju);
   S7B_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- centroid virial ---------------------------------------------------------------------------------------------
+// Wc_i = sum_j sum_{images i'} (r_j - r_i') (x) dU_j/dr_i' by one reverse pass of four adjoint channels on the graph
+// and forward of the last compute (DESIGN.md §8.5): A = dE/d(feature) and B_a = sum_m (r_m - r_j)_a dU_m/d(feature of
+// j).  At the readout A = scale * readout and B = 0; the node-local steps (gate, si2, sc, si1) carry B like any
+// adjoint; the convolution sends B_a - vec_a A to the neighbour (conv_centroid_bwd_kernel).  Per layer t, from the
+// last: w and w' from the radial MLP (flux_radial_jet); ag = gate'(g)^T ah; amid = si2^T ag; the four-channel
+// convolution backward -> ax and the per-edge dE/dY, dE/dr; ah(t-1) = sc^T ag + si1^T ax.  The embedding depends on
+// the species only, so the pass stops at layer 0.  centroid_scatter_kernel turns the per-edge sums into Wc.
+static int centroid_pass(S7bEngine* e, double* wc, cudaStream_t st) {
+  const int T = e->desc.n_layers, LF = e->desc.lmax_filter, N = e->n_nodes;
+  const int64_t E = e->n_edges;
+  const int ny = e->ny_stride;
+  FluxBufs& fx = e->fx;
+  size_t mx, mg, mm, mh, mW;
+  flux_widths(e, mx, mg, mm, mh, mW);
+  const size_t sx = (size_t)N * mx, sg = (size_t)N * mg, sm = (size_t)N * mm, sh = (size_t)N * mh;
+  float* ax = fx.tx.as<float>();
+  float* ag = fx.tg.as<float>();
+  float* ah = fx.th.as<float>();
+  float* amid = fx.dmid.as<float>();
+  hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, fx.emb2.as<float>());
+  S7B_LAUNCH_CHECK();
+  S7B_CUDA_CHECK(cudaMemsetAsync(fx.dY.p, 0, kFluxChannels * (size_t)E * ny * sizeof(float), st));
+  S7B_CUDA_CHECK(cudaMemsetAsync(fx.dr.p, 0, kFluxChannels * (size_t)E * sizeof(float), st));
+  const LayerCfg& Lz = e->layers[T - 1];
+  const GlobalParams& G = e->global_params;
+  hvp_readout_seed_kernel<<<grid1d((size_t)N * Lz.dim_h, 256), 256, 0, st>>>(G.readout.as<float>(), G.scale.as<float>(), e->d_species, N, Lz.dim_h, ah);
+  S7B_LAUNCH_CHECK();
+  for (int c = 1; c < kFluxChannels; ++c) S7B_CUDA_CHECK(cudaMemsetAsync(ah + c * sh, 0, (size_t)N * Lz.dim_h * sizeof(float), st));
+  for (int t = T - 1; t >= 0; --t) {
+    const LayerCfg& L = e->layers[t];
+    const LayerParams& P = e->layer_params[t];
+    if (flux_radial_jet(e, t, st)) return 1;
+    for (int c = 0; c < kFluxChannels; ++c) {
+      gate_bwd_kernel<<<grid1d((size_t)N * L.g.dim, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), ah + c * sh, ag + c * sg, N);
+      S7B_LAUNCH_CHECK();
+      if (node_linear(e, P.si2T, fx.re, true, ag + c * sg, amid + c * sm, false, st)) return 1;
+      if (t > 0) S7B_CUDA_CHECK(cudaMemsetAsync(ax + c * sx, 0, (size_t)N * L.x.dim * sizeof(float), st));
+    }
+    ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
+    ca.w = fx.w2.as<float>();          // raw kernels on the MLP's weights, in both radial modes
+    const CentroidAdjoints g{amid, fx.w2.as<float>() + (size_t)E * L.W, e->d_edge_vec, t > 0 ? ax : nullptr,
+                             fx.dY.as<float>(), fx.dr.as<float>(), sm, sx, (size_t)E * ny, (size_t)E};
+    for (int l1 = 0; l1 < L.x.n_l; ++l1)
+      for (int c0 = 0, nch = kFluxChannels; c0 < kFluxChannels; c0 += nch)
+        if (launch_conv_centroid(l1, LF, L.lmax_out, ca, L.roles[l1], g, c0, &nch, st)) return 1;
+    if (t > 0)
+      for (int c = 0; c < kFluxChannels; ++c) {
+        S7B_CUDA_CHECK(cudaMemsetAsync(ah + c * sh, 0, (size_t)N * L.x.dim * sizeof(float), st));
+        if (node_linear(e, P.scT, fx.re, true, ag + c * sg, ah + c * sh, false, st) ||
+            node_linear(e, P.si1T, fx.re, true, ax + c * sx, ah + c * sh, true, st))
+          return 1;
+      }
+  }
+  const int grd = (N * 32 + 255) / 256;
+  if (LF == 1) centroid_scatter_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc);
+  else if (LF == 2) centroid_scatter_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc);
+  else centroid_scatter_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc);
+  S7B_LAUNCH_CHECK();
+  return 0;
+}
+
+int s7b_engine_centroid_virial(S7bEngine* e, double* d_out, void* stream) {
+  if (hvp_check(e, "s7b_engine_centroid_virial")) return 1;
+  if (e->n_nodes > 0 && !d_out) return fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (e->n_nodes == 0) return 0;
+  S7B_CUDA_CHECK(cudaMemsetAsync(d_out, 0, (size_t)e->n_nodes * 9 * sizeof(double), st));
+  if (e->n_edges == 0) return 0;      // the atomic energies do not depend on the positions
+  if (flux_alloc(e)) return 1;
+  return centroid_pass(e, d_out, st);
+}
+
+int s7b_engine_centroid_virial_host(S7bEngine* e, double* host_out, void* stream) {
+  if (hvp_check(e, "s7b_engine_centroid_virial_host")) return 1;
+  if (e->n_nodes > 0 && !host_out) return fail("null argument");
+  if (e->n_nodes == 0) return 0;
+  const size_t bytes = (size_t)e->n_nodes * 9 * sizeof(double);
+  if (e->fx.wc.ensure(bytes)) return fail("cudaMalloc failed for the centroid virial's buffers");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (s7b_engine_centroid_virial(e, e->fx.wc.as<double>(), stream)) return 1;
+  S7B_CUDA_CHECK(cudaMemcpyAsync(host_out, e->fx.wc.p, bytes, cudaMemcpyDeviceToHost, st));
+  S7B_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }
 

@@ -67,7 +67,7 @@ EXPORTS = [
     's7b_engine_set_positions_batch', 's7b_engine_system_results',
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
     's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain', 's7b_engine_heat_flux',
-    's7b_d3_heat_flux',
+    's7b_d3_heat_flux', 's7b_engine_centroid_virial', 's7b_engine_centroid_virial_host',
 ]
 
 
@@ -121,6 +121,8 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_hvp.argtypes = [vp, vp, vp, vp]
     lib.s7b_engine_hvp_strain.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.s7b_engine_heat_flux.argtypes = [vp, vp, vp, vp, vp]
+    lib.s7b_engine_centroid_virial.argtypes = [vp, vp, vp]
+    lib.s7b_engine_centroid_virial_host.argtypes = [vp, vp, vp]
     lib.s7b_engine_buffer.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(sz)]
     lib.s7b_engine_buffer.restype = vp
     lib.s7b_engine_compute_host.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -675,6 +677,20 @@ class B200Engine:
             self._upload_hvp_mlp()
             check(self.lib.s7b_engine_heat_flux(self._h, v.data_ptr(), jpot.data_ptr(), ju.data_ptr(), self._stream()))
         return jpot, ju
+
+    def centroid_virial(self):
+        """Per-atom centroid virial on the graph and forward of the last ``compute`` (C ABI
+        ``s7b_engine_centroid_virial``, DESIGN.md §8.5): [n_nodes, 3, 3] float64 device tensor in eV,
+        Wc_i[a, b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b over the atomic energies U_j and every periodic image i'
+        of atom i.  sum_i Wc_i = the virial, and sum_i Wc_i v_i = ``heat_flux(v)``'s jpot for any v.  Not symmetric:
+        row a is the flux direction, column b the velocity direction.  One reverse pass of four channels; uploads the
+        radial MLP of a table-mode engine on first use, as ``hvp``."""
+        torch = self.torch
+        out = torch.empty(self.n_nodes, 3, 3, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._upload_hvp_mlp()
+            check(self.lib.s7b_engine_centroid_virial(self._h, out.data_ptr(), self._stream()))
+        return out
 
     def buffer(self, name: str, layer: int = 0, dtype: str = 'f4', shape=None):
         """Zero-copy torch view of an engine buffer (valid until the next set_graph)."""

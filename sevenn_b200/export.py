@@ -20,10 +20,15 @@ from .engine import default_table_knots, model_desc, prepare_params
 from .spec import build_spec
 
 
-def export_flat(path: str, meta: dict, arrays, radial: str = 'table', knots=None) -> None:
+def export_flat(path: str, meta: dict, arrays, radial: str = 'table', knots=None, radial_mlp: bool = False) -> None:
+    """``radial_mlp``: a 'table' file also carries the radial MLP (mlp0..2 of every layer), which the second-order
+    passes evaluate in both radial modes (s7b_engine_hvp, s7b_engine_heat_flux, s7b_engine_centroid_virial; a LAMMPS
+    run whose compute centroid/stress/atom makes pair_style e3gnn/b200 fill cvatom).  An 'mlp' file always has it."""
     spec = build_spec(meta)
     knots = (knots or default_table_knots(spec)) if radial == 'table' else 0
     params = prepare_params(spec, arrays, radial, knots)
+    if radial == 'table' and radial_mlp:
+        params.update({k: v for k, v in prepare_params(spec, arrays, 'mlp', 0).items() if k[0] in ('mlp0', 'mlp1', 'mlp2')})
     d = model_desc(spec, knots)
     with open(path, 'wb') as f:
         f.write(b'S7BMODEL')
