@@ -450,6 +450,16 @@ S7B_API int s7b_d3_hvp_strain(S7bD3* d3, const double* d_v, const double* d_stra
  * allocated on the first call and kept; no forward buffer is written.  Per-structure sums in fp64 and a fixed order:
  * deterministic, and a batch member's result is the structure's alone. */
 S7B_API int s7b_d3_heat_flux(S7bD3* d3, const double* d_v, double* d_jpot, double* d_ju, void* stream);
+/* Per-atom centroid virial of D3's atomic energies (DESIGN.md §8.6), with the forward of the last three stages held:
+ * Wc_i[a][b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b, j over the atoms of i's structure, i' atom i and its
+ * periodic images, U_j the pair pass's atomic energies ("eatom").  Not symmetric: row a is the flux direction, column
+ * b the velocity direction.  sum_i Wc_i over a structure is its virial (s7b_d3_system_results), sum_i Wc_i v_i its
+ * J_pot (s7b_d3_heat_flux), and the network's rows (s7b_engine_centroid_virial) add.  Two cell-list passes; a periodic
+ * cell needs no unfolding.  d_out [n,9] f64 device pointer, overwritten with Wc_i row-major in eV, caller's atom
+ * order.  Preconditions and refusals are those of s7b_d3_hvp_strain.  With no atoms nothing is launched.  Scratch is
+ * allocated on the first call and kept; no forward buffer is written.  Per-atom sums in fp64 and a fixed order:
+ * deterministic, and a batch member's rows are the structure's alone. */
+S7B_API int s7b_d3_centroid_virial(S7bD3* d3, double* d_out, void* stream);
 
 /* The reference's own D3 entry points (pair_d3_for_ase.cu:2034-2082; ctypes signatures sevenn/calculator.py:430-483),
  * same names / arguments / call order, so its D3Calculator can load this library in place of pair_d3.so.

@@ -180,12 +180,19 @@ class DeviceBatch:
         jk = kinetic_flux(_host(velocities), _host(masses), self.atom_ptr)
         return jpot + ju + torch.as_tensor(jk, dtype=torch.float64, device=jpot.device)
 
-    def centroid_virials(self):
+    def centroid_virials(self, d3=None):
         """Per-atom centroid virial of every atom of the batch of the last ``compute``, [n, 3, 3] float64 device tensor
         in eV, in the atom order of ``compute`` (``B200Engine.centroid_virial``, DESIGN.md §8.5).  The union graph has
         no edge between structures, so each row is its structure's alone: summed over a structure's atoms it is that
-        structure's virial, and contracted with its velocities its J_pot.  D3 dispersion is not included."""
-        return self.engine.centroid_virial()
+        structure's virial, and contracted with its velocities its J_pot.  ``d3`` (a ``d3.D3Batch`` whose last
+        ``compute`` was on the same structures, as ``SevenNetD3Model.forward`` leaves it) adds D3 dispersion's rows
+        (``D3Batch.centroid_virials``, DESIGN.md §8.6); without it D3 is not included."""
+        if d3 is not None and (d3.atom_ptr is None or not np.array_equal(np.asarray(d3.atom_ptr), np.asarray(self.atom_ptr))):
+            raise ValueError('d3: its last compute was not on the structures of this batch (atom_ptr differs)')
+        wc = self.engine.centroid_virial()
+        if d3 is not None:
+            wc = wc + d3.centroid_virials()
+        return wc
 
     def elastic_tensors(self, numbers, positions, cells, pbc, system_idx, relaxed: bool = True, d3=None) -> np.ndarray:
         """Elastic tensors of every structure, [B, 6, 6] float64 in eV/A^3 (``SevenNetCalculator.get_elastic_tensor``'s
@@ -345,3 +352,12 @@ class SevenNetD3Model(SevenNetModel):
         self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
         self.d3.compute(state.atomic_numbers, state.positions, cells, state.pbc, atom_ptr=self._batch.atom_ptr)
         return self._batch.heat_flux(velocities, state.masses if convective else None, convective, d3=self.d3)
+
+    def centroid_virials(self, state):
+        """Per-atom centroid virial of the network plus D3 energy of every atom of the state, [n, 3, 3] float64 device
+        tensor in eV, in the state's atom order (``DeviceBatch.centroid_virials`` with this model's ``D3Batch``).  Runs
+        the network's and D3's forward on the state first."""
+        cells = self._cells(state)
+        self._batch.compute(state.atomic_numbers, state.positions, cells, state.pbc, state.system_idx)
+        self.d3.compute(state.atomic_numbers, state.positions, cells, state.pbc, atom_ptr=self._batch.atom_ptr)
+        return self._batch.centroid_virials(d3=self.d3)

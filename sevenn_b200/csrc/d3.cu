@@ -1,8 +1,9 @@
 // Host side of the D3 dispersion C ABI (include/sevenn_b200.h, "D3" section): parameters, cell list, the set-up of
 // one structure (host arrays) or of a batch (device arrays, s7b_d3_set_system_batch), stage launches, per-structure
-// results, the Hessian-vector product (s7b_d3_hvp_strain), the heat flux (s7b_d3_heat_flux) and the reference-named
-// entry points (pair_init ... pair_fin) that sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh,
-// d3_hvp_kernels.cuh, d3_flux_kernels.cuh.
+// results, the Hessian-vector product (s7b_d3_hvp_strain), the heat flux (s7b_d3_heat_flux), the per-atom centroid
+// virial (s7b_d3_centroid_virial) and the reference-named entry points (pair_init ... pair_fin) that
+// sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh, d3_hvp_kernels.cuh, d3_flux_kernels.cuh,
+// d3_centroid_kernels.cuh.
 #include <dlfcn.h>
 
 #include <algorithm>
@@ -16,6 +17,7 @@
 
 #include "../../include/sevenn_b200.h"
 #include "common.cuh"
+#include "d3_centroid_kernels.cuh"
 #include "d3_flux_kernels.cuh"
 #include "d3_hvp_kernels.cuh"
 #include "d3_kernels.cuh"
@@ -66,6 +68,8 @@ struct S7bD3 {
   D3Buf hv_v, hv_dcn, hv_dWt, hv_dW1t, hv_ddc, hv_force, hv_spair, hv_schain, hv_sigma, hv_energy, hv_oute, hv_dvir;
   // heat-flux scratch, allocated on its first call
   D3Buf fx_v, fx_cn4, fx_nb, fx_out, fx_energy, fx_sums;
+  // centroid-virial scratch, allocated on its first call
+  D3Buf ct_beta, ct_nb, ct_out;
   std::vector<double> host_force;      // reference ABI: pair_get_force returns a pointer
   double host_energy = 0.0, host_sigma[6] = {0, 0, 0, 0, 0, 0};
   // reference-ABI staging (pair_set_atom / pair_set_domain / pair_run_settings / pair_run_coeff)
@@ -146,7 +150,8 @@ void s7b_d3_destroy(S7bD3* d) {
                    &d->force, &d->eatom, &d->spair, &d->schain, &d->energy, &d->sigma, &d->out_force,
                    &d->hv_v, &d->hv_dcn, &d->hv_dWt, &d->hv_dW1t, &d->hv_ddc, &d->hv_force, &d->hv_spair,
                    &d->hv_schain, &d->hv_sigma, &d->hv_energy, &d->hv_oute, &d->hv_dvir,
-                   &d->fx_v, &d->fx_cn4, &d->fx_nb, &d->fx_out, &d->fx_energy, &d->fx_sums};
+                   &d->fx_v, &d->fx_cn4, &d->fx_nb, &d->fx_out, &d->fx_energy, &d->fx_sums,
+                   &d->ct_beta, &d->ct_nb, &d->ct_out};
   for (D3Buf* b : bufs) b->release();
   delete d;
 }
@@ -560,6 +565,40 @@ int s7b_d3_heat_flux(S7bD3* d, const double* d_v, double* d_jpot, double* d_ju, 
   d3_system_sums_kernel<<<B, kD3SumBlock, 0, st>>>(d->aptr.as<int>(), 0, n, X.eatom, X.out, d->fx_energy.as<double>(),
                                                    d->fx_sums.as<double>());
   d3_flux_results_kernel<<<(3 * B + 255) / 256, 256, 0, st>>>(B, d->fx_sums.as<double>(), d_jpot, d_ju);
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// Per-atom centroid virial of D3's atomic energies, Wc_i = sum_j sum_i' (r_j - r_i') (x) dU_j/dr_i' [n,9] (eV,
+// caller's atom order), on the current system with its forward (stages 1-3 over [0, n)) held: two passes on scratch
+// (d3_centroid_kernels.cuh) that read the forward's spair rows, then the forward's unsort; no forward buffer is written.
+int s7b_d3_centroid_virial(S7bD3* d, double* d_out, void* stream) {
+  if (!d || !d->have_system) return d3_fail("D3: no system set");
+  if (d->stages_done < 3)
+    return d3_fail("D3: the centroid virial needs stages 1, 2 and 3 run over all atoms [0, n) of the current system "
+                   "first");
+  const int n = d->n;
+  if (n == 0) return 0;
+  if (!d_out) return d3_fail("null argument");
+  const size_t N = (size_t)n;
+  int rc = 0;
+  rc |= d->ct_beta.ensure(N * 24); rc |= d->ct_nb.ensure(N * 16); rc |= d->ct_out.ensure(N * 72);
+  if (rc) return d3_fail("cudaMalloc failed for the D3 centroid virial");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const bool bt = d->batched;
+  const D3Params& P = bt ? d->Pe : d->P;
+  const D3Atoms A = d3_atoms(d);
+  D3Centroid C;
+  C.beta = d->ct_beta.as<double>();
+  C.nb = d->ct_nb.as<float4>();
+  C.spair = d->spair.as<double>();
+  C.out = d->ct_out.as<double>();
+  const int grd = (n + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
+  if (bt) d3_centroid_moment_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, C);
+  else d3_centroid_moment_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, C);
+  if (bt) d3_centroid_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, C);
+  else d3_centroid_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, C);
+  d3_unsort_kernel<<<(n * 9 + 255) / 256, 256, 0, st>>>(n, 9, d->idx_sorted.as<int>(), C.out, 1.0, d_out);
   S7B_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -187,6 +187,19 @@ class D3Engine:
             check(self.lib.s7b_d3_heat_flux(self._h, v.data_ptr(), jpot.data_ptr(), ju.data_ptr(), self._stream()))
         return jpot, ju
 
+    def centroid_virial(self):
+        """Per-atom centroid virial of D3's atomic energies (C ABI ``s7b_d3_centroid_virial``, DESIGN.md §8.6) with the
+        forward of the last three stages over all atoms held: [n, 3, 3] float64 device tensor in eV, caller's atom
+        order, Wc_i[a, b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b over atom i and its periodic images i'
+        (U_j = ``atomic_energies``).  sum_i Wc_i over a structure is its virial, and sum_i Wc_i v_i is ``heat_flux(v)``'s
+        jpot for any v.  Not symmetric: row a is the flux direction, column b the velocity direction.  Two cell-list
+        passes; a periodic cell needs no unfolding."""
+        torch = self.torch
+        out = torch.empty(self.n, 3, 3, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self.lib.s7b_d3_centroid_virial(self._h, out.data_ptr(), self._stream()))
+        return out
+
 
 def distributed_d3(engine: D3Engine, numbers, positions, cell, pbc=(True, True, True), group=None):
     """The same system on every rank (positions replicated: the 50 A interaction range is of the order of the
@@ -332,6 +345,13 @@ class D3Batch:
             raise RuntimeError('no batch: call compute first')
         return self.engine.heat_flux(v)
 
+    def centroid_virials(self):
+        """``D3Engine.centroid_virial`` on the last batch: [n, 3, 3] float64 device tensor in eV, in the atom order of
+        ``compute``.  Each row is that of its structure alone."""
+        if self.atom_ptr is None:
+            raise RuntimeError('no batch: call compute first')
+        return self.engine.centroid_virial()
+
 
 try:
     from ase.calculators.calculator import Calculator as _Base, all_changes as _all_changes
@@ -401,13 +421,18 @@ class D3Calculator(_Base):
             self.engine.run_stage(stage)
         self._remember(numbers, pos, cell, pbc)
 
-    def _flux_parts(self, atoms):
-        """(J_pot [3], sum_j U_j v_j [3], velocities [n, 3]) of ``atoms``; the three stages run only when numbers,
-        positions, cell or pbc (as ``calculate`` evaluates them) differ from those of the engine's current forward"""
+    def _forward_if_changed(self, atoms):
+        """Leave the engine on the forward of ``atoms``: the three stages run only when numbers, positions, cell or
+        pbc (as ``calculate`` evaluates them) differ from those of the engine's current forward"""
         numbers, pos, cell, pbc, _ = self._inputs(atoms)
         last = self._engine_inputs
         if last is None or not all(np.array_equal(a, b) for a, b in zip(last, (numbers, pos, cell, pbc))):
             self._forward(atoms)
+
+    def _flux_parts(self, atoms):
+        """(J_pot [3], sum_j U_j v_j [3], velocities [n, 3]) of ``atoms``; the three stages run only when numbers,
+        positions, cell or pbc (as ``calculate`` evaluates them) differ from those of the engine's current forward"""
+        self._forward_if_changed(atoms)
         v = np.asarray(atoms.get_velocities(), dtype=np.float64).reshape(-1, 3)
         jpot, ju = self.engine.heat_flux(v)
         return jpot[0].cpu().numpy(), ju[0].cpu().numpy(), v
@@ -427,6 +452,19 @@ class D3Calculator(_Base):
             return jpot
         from .heat_flux import kinetic_flux
         return jpot + ju + kinetic_flux(v, atoms.get_masses())[0]
+
+    def get_centroid_virials(self, atoms=None) -> np.ndarray:
+        """Per-atom centroid virial of the D3 energy of ``atoms`` (default: the calculator's atoms), [N, 3, 3] float64
+        in eV (``D3Engine.centroid_virial``, DESIGN.md §8.6): Wc_i[a, b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b with
+        D3's atomic energies U_j.  sum_i Wc_i is the virial and sum_i Wc_i v_i is ``get_heat_flux(convective=False)``.  A
+        structure without a cell is evaluated in ``calculate``'s generated cell (``atoms`` is not modified).  The three
+        stages run only when positions, numbers, cell or pbc differ from those of the last D3 forward; ``results`` is
+        not touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        self._forward_if_changed(atoms)
+        return self.engine.centroid_virial().cpu().numpy()
 
     def get_hessian(self, atoms=None) -> np.ndarray:
         """Hessian d2E/dr dr of the D3 energy of ``atoms`` (default: the calculator's atoms), [3N, 3N] float64 in
@@ -542,3 +580,13 @@ class SevenNetD3Calculator(_Base):
             return jp_a + jp_b
         from .heat_flux import kinetic_flux
         return jp_a + jp_b + ju_a + ju_b + kinetic_flux(v, atoms.get_masses())[0]
+
+    def get_centroid_virials(self, atoms=None) -> np.ndarray:
+        """Per-atom centroid virial of the network plus D3 energy, [N, 3, 3] float64 in eV (``SevenNetCalculator.
+        get_centroid_virials``'s definition): the atomic energies are the network's plus D3's, so Wc is the sum of
+        the two terms', in fp64.  Each term's forward runs only when the atoms changed since its last one; ``results``
+        is not touched."""
+        atoms = atoms if atoms is not None else self.atoms
+        if atoms is None:
+            raise ValueError('No atoms to evaluate')
+        return self.sevennet_calc.get_centroid_virials(atoms) + self.d3_calc.get_centroid_virials(atoms)
