@@ -100,6 +100,15 @@ struct CentroidAdjoints {
   size_t g_stride, x_stride, dY_stride, dr_stride;
 };
 
+// The kernel families of the fused convolution, one launcher type each (conv_dispatch.cuh): X(family, ...) for each
+#define S7B_CONV_FAMILIES(X, ...) X(ConvFwd, __VA_ARGS__) X(ConvBwd, __VA_ARGS__) X(ConvJvp, __VA_ARGS__) \
+  X(ConvBwdTangent, __VA_ARGS__) X(ConvFlux, __VA_ARGS__) X(ConvCentroid, __VA_ARGS__)
+
+// Launch family F's kernel for the l1 role of the kinds (l1, lf, lo) over the centres [a.n_begin, a.n_dst)
+// (conv_dispatch.cu): 0 when launched or when there is nothing to launch, 1 with the error set.
+template <class F>
+int launch_conv(int l1, int lf, int lo, const F& f, const ConvArgs& a, const ConvRole& role, cudaStream_t st);
+
 }  // namespace s7b
 
 #define S7B_CUDA_CHECK(expr)                                                            \

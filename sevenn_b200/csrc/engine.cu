@@ -13,11 +13,13 @@
 #include <functional>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/sevenn_b200.h"
 #include "common.cuh"
 #include "conv_kernels.cuh"
+#include "conv_dispatch.cuh"
 #include "edge_kernels.cuh"
 #include "hvp_kernels.cuh"
 #include "neighbor.cuh"
@@ -48,20 +50,15 @@ static int fail(const std::string& m) {
     S7B_CUDA_CHECK(cudaGetLastError());             \
   } while (0)
 
-// ---- conv launch dispatch (defined in conv_dispatch_*.cu) ---------------------------------
-int launch_conv_fwd(int l1, int lf, int lo, bool table, const ConvArgs& a, const ConvRole& role,
-                    float* out, cudaStream_t st);
-int launch_conv_bwd(int l1, int lf, int lo, bool table, bool need_dx, const ConvArgs& a,
-                    const ConvRole& role, const float* gout, float* dx, float* dY_acc,
-                    float* dEdr_acc, float* dw, cudaStream_t st);
-int launch_conv_jvp(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
-                    float* out, cudaStream_t st);
-int launch_conv_bwd_tangent(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const ConvTangents& tan,
-                            const float* gout, float* dx, float* dY_acc, float* dw, cudaStream_t st);
-int launch_conv_flux(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const FluxTangents& f, int c0,
-                     int* nch, float* out, cudaStream_t st);
-int launch_conv_centroid(int l1, int lf, int lo, const ConvArgs& a, const ConvRole& role, const CentroidAdjoints& g,
-                         int c0, int* nch, cudaStream_t st);
+// Calls launch(std::integral_constant<int, LMAX>()) with the edge kernels' LMAX for lmax_filter: 1 -> 1, 2 -> 2,
+// anything else -> 3
+
+template <class Launch>
+static void with_lmax_filter(int lmax_filter, const Launch& launch) {
+  if (lmax_filter == 1) launch(std::integral_constant<int, 1>());
+  else if (lmax_filter == 2) launch(std::integral_constant<int, 2>());
+  else launch(std::integral_constant<int, 3>());
+}
 
 static int64_t g_alloc_gen = 0;   // bumped by every (re)allocation: captured CUDA graphs hold raw pointers
 
@@ -837,7 +834,7 @@ static int dense_gemm(const float* A, int K, float* C, int N, const float* W, in
 static int conv_forward(const LayerCfg& L, int lmax_filter, bool table, ConvArgs a, float* out,
                         cudaStream_t st) {
   for (int l1 = 0; l1 < L.x.n_l; ++l1)
-    if (launch_conv_fwd(l1, lmax_filter, L.lmax_out, table, a, L.roles[l1], out, st)) return 1;
+    if (launch_conv(l1, lmax_filter, L.lmax_out, ConvFwd{table, out}, a, L.roles[l1], st)) return 1;
   return 0;
 }
 
@@ -1390,9 +1387,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         const int grd = (int)((Ecap + blk - 1) / blk);
         float* emb = table ? nullptr : e->emb.as<float>();
         ProfScope ps(e->prof, st, "edge_fwd");
-        if (LF == 1) edge_fwd_kernel<1><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, e->d_src, nE, e->ny_stride, e->rec.as<int4>(), e->Y.as<float>(), e->rlen.as<float>(), emb);
-        else if (LF == 2) edge_fwd_kernel<2><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, e->d_src, nE, e->ny_stride, e->rec.as<int4>(), e->Y.as<float>(), e->rlen.as<float>(), emb);
-        else edge_fwd_kernel<3><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, e->d_src, nE, e->ny_stride, e->rec.as<int4>(), e->Y.as<float>(), e->rlen.as<float>(), emb);
+        with_lmax_filter(LF, [&](auto lf) { edge_fwd_kernel<lf><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, e->d_src, nE, e->ny_stride, e->rec.as<int4>(), e->Y.as<float>(), e->rlen.as<float>(), emb); });
         S7B_LAUNCH_CHECK();
         int max_lx = 0;
         for (auto& L : e->layers) max_lx = std::max(max_lx, L.x.n_l);
@@ -1462,7 +1457,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
           cudaStream_t s1 = (par && l1 > 0) ? e->side[l1] : st;
           if (par && l1 > 0) S7B_CUDA_CHECK(cudaStreamWaitEvent(s1, e->ev_fork, 0));
           ProfScope ps(e->prof, s1, "conv_fwd", t, l1);
-          if (launch_conv_fwd(l1, LF, L.lmax_out, table, ca, L.roles[l1], e->mid.as<float>(), s1)) return 1;
+          if (launch_conv(l1, LF, L.lmax_out, ConvFwd{table, e->mid.as<float>()}, ca, L.roles[l1], s1)) return 1;
           if (par && l1 > 0) {
             S7B_CUDA_CHECK(cudaEventRecord(e->ev_join[l1], s1));
             S7B_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_join[l1], 0));
@@ -1565,7 +1560,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
           cudaStream_t s1 = (par && l1 > 0) ? e->side[l1] : st;
           if (par && l1 > 0) S7B_CUDA_CHECK(cudaStreamWaitEvent(s1, e->ev_fork, 0));
           ProfScope ps(e->prof, s1, "conv_bwd", t, l1);
-          if (launch_conv_bwd(l1, LF, L.lmax_out, table, t > 0, ca, L.roles[l1], e->mid.as<float>(), e->dx.as<float>(), dY, dEdr, table ? nullptr : e->dwbuf.as<float>(), s1)) return 1;
+          if (launch_conv(l1, LF, L.lmax_out, ConvBwd{table, t > 0, e->mid.as<float>(), e->dx.as<float>(), dY, dEdr, table ? nullptr : e->dwbuf.as<float>()}, ca, L.roles[l1], s1)) return 1;
           if (par && l1 > 0) {
             S7B_CUDA_CHECK(cudaEventRecord(e->ev_join[l1], s1));
             S7B_CUDA_CHECK(cudaStreamWaitEvent(st, e->ev_join[l1], 0));
@@ -1616,9 +1611,7 @@ static int run_stage_impl(S7bEngine* e, int stage, int t, void* stream) {
         const float* dEdr = table ? e->dEdr_acc.as<float>() : nullptr;
         const float* demb = table ? nullptr : e->demb_acc.as<float>();
         ProfScope ps(e->prof, st, "edge_bwd_force_scatter");
-        if (LF == 1) edge_bwd_kernel<1><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, nE, Ecap, e->ny_stride, max_lx, e->dY_acc.as<float>(), dEdr, demb, e->fedge.as<float>());
-        else if (LF == 2) edge_bwd_kernel<2><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, nE, Ecap, e->ny_stride, max_lx, e->dY_acc.as<float>(), dEdr, demb, e->fedge.as<float>());
-        else edge_bwd_kernel<3><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, nE, Ecap, e->ny_stride, max_lx, e->dY_acc.as<float>(), dEdr, demb, e->fedge.as<float>());
+        with_lmax_filter(LF, [&](auto lf) { edge_bwd_kernel<lf><<<grd, blk, 0, st>>>(e->radial, e->d_edge_vec, nE, Ecap, e->ny_stride, max_lx, e->dY_acc.as<float>(), dEdr, demb, e->fedge.as<float>()); });
         S7B_LAUNCH_CHECK();
         force_scatter_kernel<<<(Nl * 32 + blk - 1) / blk, blk, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, e->fedge.as<float>(), Nl, e->forces.as<float>(), e->virial.as<double>(), av ? e->atomic_virial.as<float>() : nullptr);
         S7B_LAUNCH_CHECK();
@@ -1823,9 +1816,7 @@ static int hvp_pass(S7bEngine* e, const float* v, const double* strain, const in
   // ---- edge tangents and the radial basis jet (layer independent)
   {
     const int grd = (N * 32 + 255) / 256;
-    if (LF == 1) hvp_edge_fwd_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
-    else if (LF == 2) hvp_edge_fwd_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
-    else hvp_edge_fwd_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>());
+    with_lmax_filter(LF, [&](auto lf) { hvp_edge_fwd_kernel<lf><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, strain, atom_ptr, n_sys, N, ny, hv.dvec.as<float>(), hv.dr.as<float>(), hv.dY.as<float>()); });
     S7B_LAUNCH_CHECK();
     hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, hv.emb3.as<float>());
     S7B_LAUNCH_CHECK();
@@ -1845,7 +1836,7 @@ static int hvp_pass(S7bEngine* e, const float* v, const double* strain, const in
     const ConvArgs ca = conv_args(t);
     const ConvTangents tan{t > 0 ? hv.tx[t].as<float>() : nullptr, hv.dY.as<float>(), hv.dw.as<float>()};
     for (int l1 = 0; l1 < L.x.n_l; ++l1)
-      if (launch_conv_jvp(l1, LF, L.lmax_out, ca, L.roles[l1], tan, hv.dmid.as<float>(), st)) return 1;
+      if (launch_conv(l1, LF, L.lmax_out, ConvJvp{tan, hv.dmid.as<float>()}, ca, L.roles[l1], st)) return 1;
     S7B_CUDA_CHECK(cudaMemsetAsync(hv.tg[t].p, 0, (size_t)N * L.g.dim * sizeof(float), st));
     if (t > 0 && node_linear(e, P.sc, hv.re, true, hv.th.as<float>(), hv.tg[t].as<float>(), false, st)) return 1;
     if (node_linear(e, P.si2, hv.re, true, hv.dmid.as<float>(), hv.tg[t].as<float>(), true, st)) return 1;
@@ -1878,9 +1869,9 @@ static int hvp_pass(S7bEngine* e, const float* v, const double* strain, const in
       const ConvRole& role = L.roles[l1];
       // primal adjoints (dE/dx, dE/dY, dE/dw) and their tangent: the backward of the tangent adjoint dmid plus
       // the second-order terms of the operand tangents contracted with the primal adjoint
-      if (launch_conv_bwd(l1, LF, L.lmax_out, false, t > 0, ca, role, hv.amid.as<float>(), hv.ax.as<float>(), hv.gY.as<float>(), nullptr, hv.aw.as<float>(), st) ||
-          launch_conv_bwd(l1, LF, L.lmax_out, false, t > 0, ca, role, hv.damid.as<float>(), hv.dax.as<float>(), hv.dgY.as<float>(), nullptr, hv.daw1.as<float>(), st) ||
-          launch_conv_bwd_tangent(l1, LF, L.lmax_out, ca, role, tan, hv.amid.as<float>(), hv.dax.as<float>(), hv.dgY.as<float>(), hv.daw2.as<float>(), st))
+      if (launch_conv(l1, LF, L.lmax_out, ConvBwd{false, t > 0, hv.amid.as<float>(), hv.ax.as<float>(), hv.gY.as<float>(), nullptr, hv.aw.as<float>()}, ca, role, st) ||
+          launch_conv(l1, LF, L.lmax_out, ConvBwd{false, t > 0, hv.damid.as<float>(), hv.dax.as<float>(), hv.dgY.as<float>(), nullptr, hv.daw1.as<float>()}, ca, role, st) ||
+          launch_conv(l1, LF, L.lmax_out, ConvBwdTangent{tan, hv.amid.as<float>(), hv.dax.as<float>(), hv.dgY.as<float>(), hv.daw2.as<float>()}, ca, role, st))
         return 1;
     }
     const float* w3 = hv.w3.as<float>();
@@ -1898,9 +1889,7 @@ static int hvp_pass(S7bEngine* e, const float* v, const double* strain, const in
   }
   // ---- edge backward tangent and the force scatter of its negative: H v
   const int grd = (int)((E + 255) / 256);
-  if (LF == 1) hvp_edge_bwd_kernel<1><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>());
-  else if (LF == 2) hvp_edge_bwd_kernel<2><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>());
-  else hvp_edge_bwd_kernel<3><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>());
+  with_lmax_filter(LF, [&](auto lf) { hvp_edge_bwd_kernel<lf><<<grd, 256, 0, st>>>(e->d_edge_vec, hv.dvec.as<float>(), E, ny, hv.gY.as<float>(), hv.dgY.as<float>(), hv.ar.as<float>(), hv.dar.as<float>(), hv.fneg.as<float>()); });
   S7B_LAUNCH_CHECK();
   S7B_CUDA_CHECK(cudaMemsetAsync(hv.virial.p, 0, 6 * sizeof(double), st));
   force_scatter_kernel<<<(N * 32 + 255) / 256, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, hv.fneg.as<float>(), N, out, hv.virial.as<double>(), nullptr);
@@ -2033,9 +2022,7 @@ static int flux_pass(S7bEngine* e, const float* v, cudaStream_t st) {
   const size_t sx = (size_t)N * mx, sg = (size_t)N * mg, sm = (size_t)N * mm, sh = (size_t)N * mh;
   {
     const int grd = (N * 32 + 255) / 256;
-    if (LF == 1) flux_edge_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>());
-    else if (LF == 2) flux_edge_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>());
-    else flux_edge_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>());
+    with_lmax_filter(LF, [&](auto lf) { flux_edge_kernel<lf><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, v, N, E, ny, fx.dr.as<float>(), fx.dY.as<float>()); });
     S7B_LAUNCH_CHECK();
     hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, fx.emb2.as<float>());
     S7B_LAUNCH_CHECK();
@@ -2057,7 +2044,7 @@ static int flux_pass(S7bEngine* e, const float* v, cudaStream_t st) {
                          fx.dr.as<float>(), fx.dY.as<float>(), e->d_edge_vec, sx, (size_t)E, (size_t)E * ny, sm};
     for (int l1 = 0; l1 < L.x.n_l; ++l1)
       for (int c0 = 0, nch = kFluxChannels; c0 < kFluxChannels; c0 += nch)
-        if (launch_conv_flux(l1, LF, L.lmax_out, ca, L.roles[l1], f, c0, &nch, dmid, st)) return 1;
+        if (launch_conv(l1, LF, L.lmax_out, ConvFlux{f, c0, &nch, dmid}, ca, L.roles[l1], st)) return 1;
     for (int c = 0; c < kFluxChannels; ++c) {
       S7B_CUDA_CHECK(cudaMemsetAsync(tg + c * sg, 0, (size_t)N * L.g.dim * sizeof(float), st));
       if (t > 0 && node_linear(e, P.sc, fx.re, true, th + c * sh, tg + c * sg, false, st)) return 1;
@@ -2143,7 +2130,7 @@ static int centroid_pass(S7bEngine* e, double* wc, cudaStream_t st) {
                              fx.dY.as<float>(), fx.dr.as<float>(), sm, sx, (size_t)E * ny, (size_t)E};
     for (int l1 = 0; l1 < L.x.n_l; ++l1)
       for (int c0 = 0, nch = kFluxChannels; c0 < kFluxChannels; c0 += nch)
-        if (launch_conv_centroid(l1, LF, L.lmax_out, ca, L.roles[l1], g, c0, &nch, st)) return 1;
+        if (launch_conv(l1, LF, L.lmax_out, ConvCentroid{g, c0, &nch}, ca, L.roles[l1], st)) return 1;
     if (t > 0)
       for (int c = 0; c < kFluxChannels; ++c) {
         S7B_CUDA_CHECK(cudaMemsetAsync(ah + c * sh, 0, (size_t)N * L.x.dim * sizeof(float), st));
@@ -2153,9 +2140,7 @@ static int centroid_pass(S7bEngine* e, double* wc, cudaStream_t st) {
       }
   }
   const int grd = (N * 32 + 255) / 256;
-  if (LF == 1) centroid_scatter_kernel<1><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc);
-  else if (LF == 2) centroid_scatter_kernel<2><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc);
-  else centroid_scatter_kernel<3><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc);
+  with_lmax_filter(LF, [&](auto lf) { centroid_scatter_kernel<lf><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc); });
   S7B_LAUNCH_CHECK();
   return 0;
 }
@@ -2759,8 +2744,8 @@ int s7b_conv_backward(const S7bConvPlan* p, const float* x, const float* sh, con
   a.inv_h = 1.0f;
   int rc = 0;
   for (int l1 = 0; l1 < L.x.n_l && !rc; ++l1)
-    rc = launch_conv_bwd(l1, p->lmax_filter, L.lmax_out, false, true, a, L.roles[l1], grad_out, grad_x,
-                         dY + (size_t)l1 * n_edges * p->ny_stride, nullptr, grad_weight, st);
+    rc = launch_conv(l1, p->lmax_filter, L.lmax_out, ConvBwd{false, true, grad_out, grad_x,
+                     dY + (size_t)l1 * n_edges * p->ny_stride, nullptr, grad_weight}, a, L.roles[l1], st);
   if (!rc) {
     conv_unpack_grad_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(dY, L.x.n_l, n_sh, p->ny_stride, n_edges, grad_sh);
     ++g_launches;
@@ -2819,10 +2804,10 @@ int s7b_conv_double_backward(const S7bConvPlan* p, const float* x, const float* 
   const ConvTangents tan{tan_x, tYpk, tan_weight};
   int rc = 0;
   for (int l1 = 0; l1 < L.x.n_l && !rc; ++l1)
-    rc = launch_conv_jvp(l1, p->lmax_filter, L.lmax_out, a, L.roles[l1], tan, grad_grad_out, st);
+    rc = launch_conv(l1, p->lmax_filter, L.lmax_out, ConvJvp{tan, grad_grad_out}, a, L.roles[l1], st);
   for (int l1 = 0; l1 < L.x.n_l && !rc; ++l1)
-    rc = launch_conv_bwd_tangent(l1, p->lmax_filter, L.lmax_out, a, L.roles[l1], tan, grad_out, grad_x,
-                                 dY + (size_t)l1 * n_edges * p->ny_stride, grad_weight, st);
+    rc = launch_conv(l1, p->lmax_filter, L.lmax_out, ConvBwdTangent{tan, grad_out, grad_x,
+                     dY + (size_t)l1 * n_edges * p->ny_stride, grad_weight}, a, L.roles[l1], st);
   if (!rc) {
     conv_unpack_grad_kernel<<<(int)((n_edges + 255) / 256), 256, 0, st>>>(dY, L.x.n_l, n_sh, p->ny_stride, n_edges, grad_sh);
     ++g_launches;
