@@ -91,7 +91,23 @@ enum {
   S7B_STAGE_FWD_CONV_INTERIOR = 10,
   S7B_STAGE_FWD_LAYER_A2 = 11,
   S7B_STAGE_BWD_LAYER_A1 = 12,
-  S7B_STAGE_BWD_LAYER_A2 = 13
+  S7B_STAGE_BWD_LAYER_A2 = 13,
+  /* Per-atom centroid virial on a graph with ghost atoms (s7b_engine_centroid_virial's pass, cut at the exchanges;
+   * DESIGN.md §8.7), after FWD_END of the current graph and parameters (the backward stages may run in between):
+   *   CV_BEGIN | for t = T-1..0: CV_LAYER_A(t) [t > 0: reverse-add ghost rows of "cv_dx0".."cv_dx3" (t)]
+   *                               CV_LAYER_B(t) (t > 0) | CV_END [caller reverse-adds ghost rows of "centroid_virial", fp64]
+   * Needs the radial MLP ('mlp0'..'mlp2', also on a table-mode engine).  "cv_dx0".."cv_dx3" (layer t) are the four
+   * adjoint channels A, B_x, B_y, B_z of x(t), fp32 [n_nodes, dim_x(t)] each; after CV_END "centroid_virial" is
+   * [n_nodes, 9] f64, row-major per atom (read its rows with s7b_engine_read_rows_f64_host); owned rows plus the
+   * ghost rows reverse-added into their owners give s7b_engine_centroid_virial of the whole system.  Ghost rows may
+   * be one per remote atom or one per periodic image (images of owned atoms included).  CV_BEGIN allocates the heat
+   * flux's buffers on first use.  These stages always launch directly (never from a "stage_graphs" graph) and are
+   * refused inside a stream capture; a refused call launches nothing and changes no buffer.  A forward stage other
+   * than FWD_END, set_graph or set_param (except 'mlp*' of a table-mode engine) make them wait for the next FWD_END. */
+  S7B_STAGE_CV_BEGIN = 14,
+  S7B_STAGE_CV_LAYER_A = 15,
+  S7B_STAGE_CV_LAYER_B = 16,
+  S7B_STAGE_CV_END = 17
 };
 
 S7B_API const char* s7b_last_error(void);
@@ -237,7 +253,8 @@ S7B_API int s7b_engine_heat_flux(S7bEngine* eng, const float* d_v, double* d_jpo
  * adjoint channels on that graph and forward; a periodic cell needs no unfolding.
  *   d_out [n_nodes,9] f64 (device), overwritten, row-major per atom.
  * A graph from s7b_engine_set_positions_batch gives each atom its structure's value (no edge joins two structures).
- * Preconditions and refusals are those of s7b_engine_hvp (no ghost atoms: n_local == n_nodes).  E == 0 gives zeros.
+ * Preconditions and refusals are those of s7b_engine_hvp (no ghost atoms: n_local == n_nodes; graphs with ghosts use the
+ * stages CV_BEGIN .. CV_END).  E == 0 gives zeros.
  * Buffers are those of s7b_engine_heat_flux, allocated on the first call of either and kept. */
 S7B_API int s7b_engine_centroid_virial(S7bEngine* eng, double* d_out, void* stream);
 /* The same into host memory host_out [n_nodes,9] (synchronises the stream), for hosts without a device allocator. */
@@ -249,7 +266,8 @@ S7B_API int s7b_engine_centroid_virial_host(S7bEngine* eng, double* host_out, vo
  * per-atom energies before their rounding to float), "forces" [n_nodes,3], "edge_force" [E,3],
  * "virial" (double[6], = -sum r (x) f), "edge_Y", "edge_rec".  "dY_acc" [E, ny_stride] / "dEdr_acc" [E]: the
  * backward's per-edge sums of the l1 role `layer` (0 <= layer < the largest n_l of x; -1 = role 0); NULL for
- * any other layer.  *numel receives the element count (0 with NULL). */
+ * any other layer.  "cv_dx0".."cv_dx3" (layer t) and "centroid_virial" (double): see the CV stages, NULL before the
+ * first CV_BEGIN on a graph of this size.  *numel receives the element count (0 with NULL). */
 S7B_API void* s7b_engine_buffer(S7bEngine* eng, const char* name, int layer, size_t* numel);
 
 /* Host-buffer entry point, the analogue of PairE3GNN::compute (pair_e3gnn.cpp:74-289):
@@ -272,6 +290,9 @@ S7B_API int s7b_engine_read_rows_host(S7bEngine* eng, const char* name, int laye
                                       int32_t width, float* host_out, void* stream);
 S7B_API int s7b_engine_write_rows_host(S7bEngine* eng, const char* name, int layer, int32_t row_begin, int32_t n_rows,
                                        int32_t width, const float* host_in, void* stream);
+/* rows [row_begin, row_begin + n_rows) of the f64 buffer "centroid_virial" (width 9) to the host, as read_rows_host */
+S7B_API int s7b_engine_read_rows_f64_host(S7bEngine* eng, const char* name, int layer, int32_t row_begin, int32_t n_rows,
+                                          int32_t width, double* host_out, void* stream);
 /* energy (1 double) and virial (6 doubles: xx,yy,zz,xy,yz,zx of -sum r (x) f) of the last BWD_END; either may be NULL */
 S7B_API int s7b_engine_read_scalars_host(S7bEngine* eng, double* energy, double* virial6, void* stream);
 

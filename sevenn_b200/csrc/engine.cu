@@ -310,6 +310,9 @@ struct S7bEngine {
   int64_t sg_captures = 0, sg_replays = 0;
   // second order: hvp_ready = an s7b_engine_compute ran since the last set_graph / set_param
   bool hvp_ready = false;
+  // staged centroid virial (stages CV_*): fwd_ready = FWD_END (or a compute) ran since the last set_graph / set_param
+  // and forward stage; cv_begun = CV_BEGIN ran since then
+  bool fwd_ready = false, cv_begun = false;
   HvpBufs hv;
   FluxBufs fx;
 };
@@ -1150,7 +1153,7 @@ int s7b_engine_set_param(S7bEngine* e, const char* name, int layer, const float*
   const std::string nm(name);
   // a parameter the step reads leaves the last compute's intermediates stale for s7b_engine_hvp; the radial MLP of a
   // table-mode engine is read by the HVP alone
-  if (!(e->desc.table_knots > 0 && nm.compare(0, 3, "mlp") == 0)) e->hvp_ready = false;
+  if (!(e->desc.table_knots > 0 && nm.compare(0, 3, "mlp") == 0)) e->hvp_ready = e->fwd_ready = e->cv_begun = false;
   const int T = e->desc.n_layers, S = e->desc.num_species, nb = e->desc.n_basis;
   const std::string what = (layer >= 0 ? "layer " + std::to_string(layer) + ": " : std::string()) + "parameter " + nm;
   auto bad_size = [&](size_t expect) {
@@ -1254,7 +1257,7 @@ int s7b_engine_set_graph(S7bEngine* e, int32_t n_nodes, int32_t n_local, int64_t
   if (!e) return fail("null engine");
   if (n_local < 0 || n_nodes < n_local || n_edges < 0) return fail("bad graph sizes");
   if (n_edges >= ((int64_t)1 << 31)) return fail("more than 2^31-1 edges per GPU are not supported");
-  e->hvp_ready = false;
+  e->hvp_ready = e->fwd_ready = e->cv_begun = false;
   e->n_nodes = n_nodes;
   e->n_local = n_local;
   e->n_interior = n_local;
@@ -1663,8 +1666,7 @@ static int capture_graph(S7bEngine* e, const std::function<int(cudaStream_t)>& f
 // fixed launch sequence: with option "stage_graphs" each (stage, layer) is captured once and replayed on the
 // caller's stream -- ~22 graph launches per step instead of ~170 kernel launches.  An entry whose key keeps
 // changing (positions-in MD: new graph arrays every step) stops capturing after three wasted captures.
-int s7b_engine_run_stage(S7bEngine* e, int stage, int t, void* stream) {
-  if (!e) return fail("null engine");
+static int run_stage_graphs(S7bEngine* e, int stage, int t, void* stream) {
   const bool table = e->desc.table_knots > 0;
   if (!g_opt_stage_graphs || e->capturing || !table || e->prof.enabled || !e->radial_ready)
     return run_stage_impl(e, stage, t, stream);
@@ -1698,6 +1700,22 @@ int s7b_engine_run_stage(S7bEngine* e, int stage, int t, void* stream) {
   return 0;
 }
 
+static int cv_stage(S7bEngine* e, int stage, int t, void* stream);
+
+// The centroid-virial stages run eagerly, never from a stage graph (cv_stage).  Every forward stage invalidates the
+// forward the CV stages read until FWD_END completes it again; the backward stages leave it alone.
+int s7b_engine_run_stage(S7bEngine* e, int stage, int t, void* stream) {
+  if (!e) return fail("null engine");
+  if (stage >= S7B_STAGE_CV_BEGIN && stage <= S7B_STAGE_CV_END) return cv_stage(e, stage, t, stream);
+  const bool fwd = stage == S7B_STAGE_FWD_BEGIN || stage == S7B_STAGE_FWD_LAYER || stage == S7B_STAGE_FWD_END ||
+                   stage == S7B_STAGE_FWD_LAYER_A || stage == S7B_STAGE_FWD_LAYER_SC ||
+                   stage == S7B_STAGE_FWD_CONV_INTERIOR || stage == S7B_STAGE_FWD_LAYER_A2;
+  if (fwd) e->fwd_ready = e->cv_begun = false;
+  const int rc = run_stage_graphs(e, stage, t, stream);
+  if (stage == S7B_STAGE_FWD_END) e->fwd_ready = rc == 0;
+  return rc;
+}
+
 static int run_all_stages(S7bEngine* e, void* stream) {
   const int T = e->desc.n_layers;
   if (run_stage_impl(e, S7B_STAGE_FWD_BEGIN, 0, stream)) return 1;
@@ -1719,11 +1737,11 @@ static int run_all_stages(S7bEngine* e, void* stream) {
 // neighbour count replay the same graph.
 int s7b_engine_compute(S7bEngine* e, void* stream) {
   if (!e) return fail("null engine");
-  e->hvp_ready = false;
+  e->hvp_ready = e->fwd_ready = e->cv_begun = false;
   const bool table = e->desc.table_knots > 0;
   if (!g_opt_cuda_graph || !table || e->prof.enabled) {
     const int rc = run_all_stages(e, stream);
-    e->hvp_ready = rc == 0;
+    e->hvp_ready = e->fwd_ready = rc == 0;
     return rc;
   }
   if (!e->radial_ready) return fail("parameter 'bessel' was not set");
@@ -1743,7 +1761,7 @@ int s7b_engine_compute(S7bEngine* e, void* stream) {
   S7B_CUDA_CHECK(cudaStreamWaitEvent(st, e->g_out, 0));
   g_launches += e->g_launches_per_replay;
   ++e->g_replays;
-  e->hvp_ready = true;
+  e->hvp_ready = e->fwd_ready = true;
   return 0;
 }
 
@@ -1897,16 +1915,21 @@ static int hvp_pass(S7bEngine* e, const float* v, const double* strain, const in
   return 0;
 }
 
-// The preconditions both entry points share; `who` names the caller in the messages.
-static int hvp_check(S7bEngine* e, const char* who) {
-  if (!e) return fail("null engine");
-  if (!e->hvp_ready) return fail(std::string(who) + " needs an s7b_engine_compute on the current graph and parameters");
-  if (e->n_local < e->n_nodes) return fail(std::string(who) + " does not run on graphs with ghost atoms (n_local < n_nodes)");
+// The second-order passes and the centroid virial evaluate the radial MLP in both radial modes
+static int mlp_check(const S7bEngine* e, const char* who) {
   for (int t = 0; t < e->desc.n_layers; ++t)
     for (int j = 0; j < 3; ++j)
       if (!e->layer_params[t].mlp[j].p)
         return fail(std::string(who) + " evaluates the radial MLP: parameter mlp" + std::to_string(j) + " of layer " + std::to_string(t) + " is missing");
   return 0;
+}
+
+// The preconditions both entry points share; `who` names the caller in the messages.
+static int hvp_check(S7bEngine* e, const char* who) {
+  if (!e) return fail("null engine");
+  if (!e->hvp_ready) return fail(std::string(who) + " needs an s7b_engine_compute on the current graph and parameters");
+  if (e->n_local < e->n_nodes) return fail(std::string(who) + " does not run on graphs with ghost atoms (n_local < n_nodes)");
+  return mlp_check(e, who);
 }
 
 int s7b_engine_hvp(S7bEngine* e, const float* d_v, float* d_out, void* stream) {
@@ -2093,56 +2116,144 @@ int s7b_engine_heat_flux(S7bEngine* e, const float* d_v, double* d_jpot, double*
 // last: w and w' from the radial MLP (flux_radial_jet); ag = gate'(g)^T ah; amid = si2^T ag; the four-channel
 // convolution backward -> ax and the per-edge dE/dY, dE/dr; ah(t-1) = sc^T ag + si1^T ax.  The embedding depends on
 // the species only, so the pass stops at layer 0.  centroid_scatter_kernel turns the per-edge sums into Wc.
-static int centroid_pass(S7bEngine* e, double* wc, cudaStream_t st) {
-  const int T = e->desc.n_layers, LF = e->desc.lmax_filter, N = e->n_nodes;
-  const int64_t E = e->n_edges;
-  const int ny = e->ny_stride;
-  FluxBufs& fx = e->fx;
+//
+// The pass is cut where a graph with ghost atoms needs an exchange (DESIGN.md §8.7): centroid_begin, then per layer
+// centroid_layer_a (ends with ax of every row, ghosts included), the caller's reverse-add of ax's ghost rows,
+// centroid_layer_b; centroid_scatter last.  The node-local steps and the seed run on the owned rows [0, n_local) only:
+// g[t] has no ghost rows, and a ghost's energy is its owner's.  Every array of FluxBufs keeps its n_nodes rows per
+// channel.  Without ghosts (s7b_engine_centroid_virial) the pieces launch what the one-piece pass did.
+
+// Channel c of a FluxBufs node array: [n_nodes][widest row] floats apart
+struct CentroidPlanes {
+  float *ax, *ag, *ah, *amid;
+  size_t sx, sg, sm, sh;
+};
+
+static CentroidPlanes centroid_planes(S7bEngine* e) {
+  const size_t N = (size_t)e->n_nodes;
   size_t mx, mg, mm, mh, mW;
   flux_widths(e, mx, mg, mm, mh, mW);
-  const size_t sx = (size_t)N * mx, sg = (size_t)N * mg, sm = (size_t)N * mm, sh = (size_t)N * mh;
-  float* ax = fx.tx.as<float>();
-  float* ag = fx.tg.as<float>();
-  float* ah = fx.th.as<float>();
-  float* amid = fx.dmid.as<float>();
+  FluxBufs& fx = e->fx;
+  return {fx.tx.as<float>(), fx.tg.as<float>(), fx.th.as<float>(), fx.dmid.as<float>(), N * mx, N * mg, N * mm, N * mh};
+}
+
+// The radial basis jet, zero edge sums, A = scale * readout on the owned rows and B = 0
+static int centroid_begin(S7bEngine* e, cudaStream_t st) {
+  const int T = e->desc.n_layers, Nl = e->n_local;
+  const int64_t E = e->n_edges;
+  FluxBufs& fx = e->fx;
+  const CentroidPlanes p = centroid_planes(e);
   hvp_radial_basis_kernel<<<(int)((E + 255) / 256), 256, 0, st>>>(e->radial, e->d_edge_vec, E, fx.emb2.as<float>());
   S7B_LAUNCH_CHECK();
-  S7B_CUDA_CHECK(cudaMemsetAsync(fx.dY.p, 0, kFluxChannels * (size_t)E * ny * sizeof(float), st));
+  S7B_CUDA_CHECK(cudaMemsetAsync(fx.dY.p, 0, kFluxChannels * (size_t)E * e->ny_stride * sizeof(float), st));
   S7B_CUDA_CHECK(cudaMemsetAsync(fx.dr.p, 0, kFluxChannels * (size_t)E * sizeof(float), st));
   const LayerCfg& Lz = e->layers[T - 1];
   const GlobalParams& G = e->global_params;
-  hvp_readout_seed_kernel<<<grid1d((size_t)N * Lz.dim_h, 256), 256, 0, st>>>(G.readout.as<float>(), G.scale.as<float>(), e->d_species, N, Lz.dim_h, ah);
+  hvp_readout_seed_kernel<<<grid1d((size_t)Nl * Lz.dim_h, 256), 256, 0, st>>>(G.readout.as<float>(), G.scale.as<float>(), e->d_species, Nl, Lz.dim_h, p.ah);
   S7B_LAUNCH_CHECK();
-  for (int c = 1; c < kFluxChannels; ++c) S7B_CUDA_CHECK(cudaMemsetAsync(ah + c * sh, 0, (size_t)N * Lz.dim_h * sizeof(float), st));
-  for (int t = T - 1; t >= 0; --t) {
-    const LayerCfg& L = e->layers[t];
-    const LayerParams& P = e->layer_params[t];
-    if (flux_radial_jet(e, t, st)) return 1;
-    for (int c = 0; c < kFluxChannels; ++c) {
-      gate_bwd_kernel<<<grid1d((size_t)N * L.g.dim, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), ah + c * sh, ag + c * sg, N);
-      S7B_LAUNCH_CHECK();
-      if (node_linear(e, P.si2T, fx.re, true, ag + c * sg, amid + c * sm, false, st)) return 1;
-      if (t > 0) S7B_CUDA_CHECK(cudaMemsetAsync(ax + c * sx, 0, (size_t)N * L.x.dim * sizeof(float), st));
-    }
-    ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
-    ca.w = fx.w2.as<float>();          // raw kernels on the MLP's weights, in both radial modes
-    const CentroidAdjoints g{amid, fx.w2.as<float>() + (size_t)E * L.W, e->d_edge_vec, t > 0 ? ax : nullptr,
-                             fx.dY.as<float>(), fx.dr.as<float>(), sm, sx, (size_t)E * ny, (size_t)E};
-    for (int l1 = 0; l1 < L.x.n_l; ++l1)
-      for (int c0 = 0, nch = kFluxChannels; c0 < kFluxChannels; c0 += nch)
-        if (launch_conv(l1, LF, L.lmax_out, ConvCentroid{g, c0, &nch}, ca, L.roles[l1], st)) return 1;
-    if (t > 0)
-      for (int c = 0; c < kFluxChannels; ++c) {
-        S7B_CUDA_CHECK(cudaMemsetAsync(ah + c * sh, 0, (size_t)N * L.x.dim * sizeof(float), st));
-        if (node_linear(e, P.scT, fx.re, true, ag + c * sg, ah + c * sh, false, st) ||
-            node_linear(e, P.si1T, fx.re, true, ax + c * sx, ah + c * sh, true, st))
-          return 1;
-      }
+  for (int c = 1; c < kFluxChannels; ++c) S7B_CUDA_CHECK(cudaMemsetAsync(p.ah + c * p.sh, 0, (size_t)Nl * Lz.dim_h * sizeof(float), st));
+  return 0;
+}
+
+// Layer t from ah: w and w', ag = gate'^T ah, amid = si2^T ag (owned rows), ax = 0 on every row, then the
+// four-channel convolution walk over the owned centres -> ax of every row and the per-edge sums
+static int centroid_layer_a(S7bEngine* e, int t, cudaStream_t st) {
+  const int LF = e->desc.lmax_filter, N = e->n_nodes, Nl = e->n_local;
+  const int64_t E = e->n_edges;
+  FluxBufs& fx = e->fx;
+  const CentroidPlanes p = centroid_planes(e);
+  const LayerCfg& L = e->layers[t];
+  const LayerParams& P = e->layer_params[t];
+  if (flux_radial_jet(e, t, st)) return 1;
+  for (int c = 0; c < kFluxChannels; ++c) {
+    gate_bwd_kernel<<<grid1d((size_t)Nl * L.g.dim, 256), 256, 0, st>>>(L.gate, e->g[t].as<float>(), p.ah + c * p.sh, p.ag + c * p.sg, Nl);
+    S7B_LAUNCH_CHECK();
+    if (node_linear(e, P.si2T, fx.re, true, p.ag + c * p.sg, p.amid + c * p.sm, false, st)) return 1;
+    if (t > 0) S7B_CUDA_CHECK(cudaMemsetAsync(p.ax + c * p.sx, 0, (size_t)N * L.x.dim * sizeof(float), st));
   }
-  const int grd = (N * 32 + 255) / 256;
-  with_lmax_filter(LF, [&](auto lf) { centroid_scatter_kernel<lf><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), E, ny, N, wc); });
+  ConvArgs ca = make_conv_args(e, t, e->x[t].as<float>());
+  ca.w = fx.w2.as<float>();          // raw kernels on the MLP's weights, in both radial modes
+  const CentroidAdjoints g{p.amid, fx.w2.as<float>() + (size_t)E * L.W, e->d_edge_vec, t > 0 ? p.ax : nullptr,
+                           fx.dY.as<float>(), fx.dr.as<float>(), p.sm, p.sx, (size_t)E * e->ny_stride, (size_t)E};
+  for (int l1 = 0; l1 < L.x.n_l; ++l1)
+    for (int c0 = 0, nch = kFluxChannels; c0 < kFluxChannels; c0 += nch)
+      if (launch_conv(l1, LF, L.lmax_out, ConvCentroid{g, c0, &nch}, ca, L.roles[l1], st)) return 1;
+  return 0;
+}
+
+// ah(t-1) = sc^T ag + si1^T ax on the owned rows (t > 0; ax complete on them)
+static int centroid_layer_b(S7bEngine* e, int t, cudaStream_t st) {
+  const int N = e->n_nodes;
+  FluxBufs& fx = e->fx;
+  const CentroidPlanes p = centroid_planes(e);
+  const LayerCfg& L = e->layers[t];
+  const LayerParams& P = e->layer_params[t];
+  for (int c = 0; c < kFluxChannels; ++c) {
+    S7B_CUDA_CHECK(cudaMemsetAsync(p.ah + c * p.sh, 0, (size_t)N * L.x.dim * sizeof(float), st));
+    if (node_linear(e, P.scT, fx.re, true, p.ag + c * p.sg, p.ah + c * p.sh, false, st) ||
+        node_linear(e, P.si1T, fx.re, true, p.ax + c * p.sx, p.ah + c * p.sh, true, st))
+      return 1;
+  }
+  return 0;
+}
+
+// Wc += the centre and neighbour ends of every edge of the owned centres (wc zeroed by the caller)
+static int centroid_scatter(S7bEngine* e, double* wc, cudaStream_t st) {
+  const int Nl = e->n_local;
+  FluxBufs& fx = e->fx;
+  const int grd = (Nl * 32 + 255) / 256;
+  with_lmax_filter(e->desc.lmax_filter, [&](auto lf) { centroid_scatter_kernel<lf><<<grd, 256, 0, st>>>(e->d_rowptr, e->d_src, e->d_edge_vec, fx.dY.as<float>(), fx.dr.as<float>(), e->n_edges, e->ny_stride, Nl, wc); });
   S7B_LAUNCH_CHECK();
   return 0;
+}
+
+static int centroid_pass(S7bEngine* e, double* wc, cudaStream_t st) {
+  if (centroid_begin(e, st)) return 1;
+  for (int t = e->desc.n_layers - 1; t >= 0; --t)
+    if (centroid_layer_a(e, t, st) || (t > 0 && centroid_layer_b(e, t, st))) return 1;
+  return centroid_scatter(e, wc, st);
+}
+
+// Stages CV_BEGIN .. CV_END (include/sevenn_b200.h).  Every check comes before the first launch, so a refused call
+// launches nothing and changes no buffer.  Always eager: CV_BEGIN may allocate, which a stream capture forbids.
+static int cv_stage(S7bEngine* e, int stage, int t, void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int T = e->desc.n_layers, Nn = e->n_nodes;
+  const int64_t E = e->n_edges;
+  const char* who = stage == S7B_STAGE_CV_BEGIN ? "stage CV_BEGIN" : stage == S7B_STAGE_CV_LAYER_A ? "stage CV_LAYER_A"
+                    : stage == S7B_STAGE_CV_LAYER_B ? "stage CV_LAYER_B" : "stage CV_END";
+  if (!e->fwd_ready) return fail(std::string(who) + " needs FWD_END (or an s7b_engine_compute) on the current graph and parameters");
+  if (mlp_check(e, who)) return 1;
+  if (stage != S7B_STAGE_CV_BEGIN && !e->cv_begun) return fail(std::string(who) + " needs CV_BEGIN first");
+  if (stage == S7B_STAGE_CV_LAYER_A && (t < 0 || t >= T)) return fail("CV_LAYER_A needs 0 <= layer < n_layers");
+  if (stage == S7B_STAGE_CV_LAYER_B && (t <= 0 || t >= T)) return fail("CV_LAYER_B needs 1 <= layer < n_layers");
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) { cudaGetLastError(); return fail(std::string(who) + ": bad stream"); }
+  if (cs != cudaStreamCaptureStatusNone) return fail(std::string(who) + " does not run inside a stream capture");
+  switch (stage) {
+    case S7B_STAGE_CV_BEGIN:
+      e->cv_begun = false;
+      if (flux_alloc(e) || e->fx.wc.ensure((size_t)std::max(Nn, 1) * 9 * sizeof(double)))
+        return fail("cudaMalloc failed for the centroid virial's buffers");
+      if (Nn > 0 && E > 0 && centroid_begin(e, st)) return 1;
+      e->cv_begun = true;
+      return 0;
+    case S7B_STAGE_CV_LAYER_A:
+      if (Nn == 0) return 0;
+      if (E > 0) return centroid_layer_a(e, t, st);
+      if (t > 0) {                 // no edge: ax stays zero, and so do its ghost rows the caller reverse-adds
+        const CentroidPlanes p = centroid_planes(e);
+        for (int c = 0; c < kFluxChannels; ++c)
+          S7B_CUDA_CHECK(cudaMemsetAsync(p.ax + c * p.sx, 0, (size_t)Nn * e->layers[t].x.dim * sizeof(float), st));
+      }
+      return 0;
+    case S7B_STAGE_CV_LAYER_B:
+      return Nn > 0 && E > 0 ? centroid_layer_b(e, t, st) : 0;
+    default:      // CV_END
+      if (Nn == 0) return 0;
+      S7B_CUDA_CHECK(cudaMemsetAsync(e->fx.wc.p, 0, (size_t)Nn * 9 * sizeof(double), st));
+      return E > 0 ? centroid_scatter(e, e->fx.wc.as<double>(), st) : 0;
+  }
 }
 
 int s7b_engine_centroid_virial(S7bEngine* e, double* d_out, void* stream) {
@@ -2241,6 +2352,19 @@ void* s7b_engine_buffer(S7bEngine* e, const char* name, int layer, size_t* numel
   else if (nm == "nl_vec") { p = e->hs_vec.p; n = (size_t)e->nl_n_edges * 3; }
   else if (nm == "edge_len") { p = e->rlen.p; n = (size_t)e->n_edges; }
   else if (nm == "edge_emb") { p = e->emb.p; n = (size_t)e->n_edges * e->desc.n_basis; }
+  else if (nm.size() == 6 && nm.compare(0, 5, "cv_dx") == 0 && nm[5] >= '0' && nm[5] < '0' + kFluxChannels && in_range(layer)) {
+    // channel c of the centroid pass's adjoint of x(layer), [n_nodes, dim_x]: once CV_BEGIN sized it for this graph
+    size_t mx, mg, mm, mh, mW;
+    flux_widths(e, mx, mg, mm, mh, mW);
+    const size_t plane = (size_t)e->n_nodes * mx;
+    if (e->fx.tx.p && e->fx.tx.bytes >= kFluxChannels * plane * sizeof(float)) {
+      p = e->fx.tx.as<float>() + (nm[5] - '0') * plane;
+      n = (size_t)e->n_nodes * e->layers[layer].x.dim;
+    }
+  } else if (nm == "centroid_virial" && e->fx.wc.p && e->fx.wc.bytes >= (size_t)e->n_nodes * 9 * sizeof(double)) {
+    p = e->fx.wc.p;              // double [n_nodes, 9]
+    n = (size_t)e->n_nodes * 9;
+  }
   else if (nm == "dY_acc" || nm == "dEdr_acc") {
     // the backward's per-edge sums, one part per l1 role (E_cap rows apart); layer = the part, -1 = part 0
     int max_lx = 0;
@@ -2522,6 +2646,7 @@ static int rows_host_copy(S7bEngine* e, const char* name, int layer, int32_t row
   if (!host || width <= 0 || row_begin < 0) return fail("bad row range");
   const std::string nm(name ? name : "");
   if (nm == "energy" || nm == "virial") return fail("energy / virial are doubles: read them with s7b_engine_buffer");
+  if (nm == "centroid_virial") return fail("centroid_virial holds doubles: read it with s7b_engine_read_rows_f64_host");
   size_t numel = 0;
   float* base = static_cast<float*>(s7b_engine_buffer(e, name, layer, &numel));
   if (!base) return fail(std::string("no such buffer: ") + nm);
@@ -2543,6 +2668,24 @@ int s7b_engine_read_rows_host(S7bEngine* e, const char* name, int layer, int32_t
 int s7b_engine_write_rows_host(S7bEngine* e, const char* name, int layer, int32_t row_begin, int32_t n_rows, int32_t width,
                                const float* host_in, void* stream) {
   return rows_host_copy(e, name, layer, row_begin, n_rows, width, const_cast<float*>(host_in), false, stream);
+}
+
+int s7b_engine_read_rows_f64_host(S7bEngine* e, const char* name, int layer, int32_t row_begin, int32_t n_rows,
+                                  int32_t width, double* host_out, void* stream) {
+  if (!e) return fail("null engine");
+  if (n_rows <= 0) return 0;
+  if (!host_out || width <= 0 || row_begin < 0) return fail("bad row range");
+  const std::string nm(name ? name : "");
+  if (nm != "centroid_virial") return fail(std::string("not a double buffer with rows: ") + nm);
+  size_t numel = 0;
+  double* base = static_cast<double*>(s7b_engine_buffer(e, name, layer, &numel));
+  if (!base) return fail(std::string("no such buffer: ") + nm);
+  if ((size_t)(row_begin + (int64_t)n_rows) * width > numel) return fail("row range exceeds the buffer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  S7B_CUDA_CHECK(cudaMemcpyAsync(host_out, base + (size_t)row_begin * width, (size_t)n_rows * width * sizeof(double),
+                                 cudaMemcpyDeviceToHost, st));
+  S7B_CUDA_CHECK(cudaStreamSynchronize(st));
+  return 0;
 }
 
 int s7b_engine_read_scalars_host(S7bEngine* e, double* energy, double* virial6, void* stream) {

@@ -34,7 +34,8 @@ _lib = None
 S7B_MAX_LAYERS, S7B_MAX_L = 8, 4
 (STAGE_FWD_BEGIN, STAGE_FWD_LAYER, STAGE_FWD_END, STAGE_BWD_LAYER_A, STAGE_BWD_LAYER_B,
  STAGE_BWD_END, STAGE_FWD_LAYER_A, STAGE_FWD_LAYER_SC, STAGE_BWD_LAYER_B1, STAGE_BWD_LAYER_B2,
- STAGE_FWD_CONV_INTERIOR, STAGE_FWD_LAYER_A2, STAGE_BWD_LAYER_A1, STAGE_BWD_LAYER_A2) = range(14)
+ STAGE_FWD_CONV_INTERIOR, STAGE_FWD_LAYER_A2, STAGE_BWD_LAYER_A1, STAGE_BWD_LAYER_A2,
+ STAGE_CV_BEGIN, STAGE_CV_LAYER_A, STAGE_CV_LAYER_B, STAGE_CV_END) = range(18)
 
 
 class S7bModelDesc(ctypes.Structure):
@@ -68,7 +69,7 @@ EXPORTS = [
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
     's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain', 's7b_engine_heat_flux',
     's7b_d3_heat_flux', 's7b_engine_centroid_virial', 's7b_engine_centroid_virial_host',
-    's7b_d3_centroid_virial',
+    's7b_d3_centroid_virial', 's7b_engine_read_rows_f64_host',
 ]
 
 
@@ -143,6 +144,7 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_set_graph_host.argtypes = [vp, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.s7b_engine_read_rows_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, i32, i32, i32, vp, vp]
     lib.s7b_engine_write_rows_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, i32, i32, i32, vp, vp]
+    lib.s7b_engine_read_rows_f64_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, i32, i32, i32, vp, vp]
     lib.s7b_engine_read_scalars_host.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double), vp]
     lib.s7b_conv_plan_create.argtypes = [i32, ctypes.POINTER(i32), i32, i32, ctypes.POINTER(vp)]
     lib.s7b_conv_plan_destroy.argtypes = [vp]
@@ -561,6 +563,14 @@ class B200Engine:
         with self.torch.cuda.device(self.device):
             check(self.lib.s7b_engine_read_rows_host(self._h, name.encode(), int(layer), int(row_begin), int(n_rows), int(width),
                                                      out.ctypes.data, self._stream()))
+        return out
+
+    def read_rows_f64(self, name: str, layer: int, row_begin: int, n_rows: int, width: int) -> np.ndarray:
+        """rows of an f64 engine buffer ("centroid_virial", width 9) to the host (``s7b_engine_read_rows_f64_host``)"""
+        out = np.empty((n_rows, width), dtype=np.float64)
+        with self.torch.cuda.device(self.device):
+            check(self.lib.s7b_engine_read_rows_f64_host(self._h, name.encode(), int(layer), int(row_begin), int(n_rows),
+                                                         int(width), out.ctypes.data, self._stream()))
         return out
 
     def write_rows(self, name: str, layer: int, row_begin: int, rows: np.ndarray):
