@@ -422,7 +422,8 @@ S7B_API int s7b_d3_run_stage(S7bD3* d3, int32_t stage, int32_t i_begin, int32_t 
  * -1/2 sum_{j,tau} C6_ij g(r_ij) of stage 2); "force" double[n,3] (hartree/bohr); "energy"
  * double[B]; "sigma" double[B,6]; "order" int32[n] (sorted position -> caller's atom index); "type" int32[n] (after
  * s7b_d3_set_system_batch: Z - 1 | local type << 8, the local type being the rank of Z among the elements of the
- * atom's structure; after s7b_d3_set_system: the type index).  B = 1 after
+ * atom's structure; after s7b_d3_set_system: the type index); "ct_nb" float[n,4], "fx_nb" float[n,8], "ct_out"
+ * double[n,9], "fx_out" double[n,6]: the rows the range passes exchange (s7b_d3_centroid_pass).  B = 1 after
  * s7b_d3_set_system.  Stage 2 sets energy / sigma to the pair sums of its range, stage 3 adds its virial. */
 S7B_API void* s7b_d3_buffer(S7bD3* d3, const char* name, size_t* numel);
 /* energy (eV), forces [n,3] (eV/A, caller's atom order), sigma6 (eV: xx,yy,zz,xy,xz,yz of sum f (x) r); one structure */
@@ -481,6 +482,25 @@ S7B_API int s7b_d3_heat_flux(S7bD3* d3, const double* d_v, double* d_jpot, doubl
  * allocated on the first call and kept; no forward buffer is written.  Per-atom sums in fp64 and a fixed order:
  * deterministic, and a batch member's rows are the structure's alone. */
 S7B_API int s7b_d3_centroid_virial(S7bD3* d3, double* d_out, void* stream);
+/* The heat flux and the centroid virial over atom ranges of the bin-sorted order, for a forward that several GPUs
+ * share (stages 1-3 over one range [lo, hi) per GPU, "cn" and "dc6i" all-gathered between them).  Each is two passes,
+ * one warp per atom and a fixed order, so the rows they write equal those of the one-shot call bit for bit:
+ *   centroid: pass 1 over [i_begin, i_end) -> all-gather "ct_nb" -> pass 2 over the same range -> all-gather
+ *             "ct_out" (double [n,9], eV, Wc rows in sorted order; "order" maps them to the caller's);
+ *   flux:     pass 1 over the range with d_v (device double [n,3], every atom's velocity in the caller's order)
+ *             -> all-gather "fx_nb" -> pass 2 -> all-gather "fx_out" -> s7b_d3_heat_flux_sums, which sums all n
+ *             rows per structure into d_jpot / d_ju as s7b_d3_heat_flux does.
+ * The library cannot see the gathers: the caller must do them, and a pass or the sums read stale or unset rows of
+ * "ct_nb" / "fx_nb" / "ct_out" / "fx_out" otherwise.  Refused (nothing launched, no buffer changed) unless stages 1, 2
+ * and 3 ran in order over one range [lo, hi) since the last set_system[_batch], set_params, set_element_tables or
+ * set_damping (a full forward is [0, n)) and the pass range lies inside it; pass 2 further needs a pass 1 of its kind
+ * over a range containing its own since the last forward stage, and the sums a flux pass 2.  Pass 1 allocates the
+ * scratch on first use, an empty range included, so every rank has the buffers the gathers address.  The one-shot
+ * calls run these passes over [0, n) and keep their own refusal of a partial-range forward. */
+S7B_API int s7b_d3_centroid_pass(S7bD3* d3, int32_t pass, int32_t i_begin, int32_t i_end, void* stream);
+S7B_API int s7b_d3_heat_flux_pass(S7bD3* d3, int32_t pass, const double* d_v, int32_t i_begin, int32_t i_end,
+                                  void* stream);
+S7B_API int s7b_d3_heat_flux_sums(S7bD3* d3, double* d_jpot, double* d_ju, void* stream);
 
 /* The reference's own D3 entry points (pair_d3_for_ase.cu:2034-2082; ctypes signatures sevenn/calculator.py:430-483),
  * same names / arguments / call order, so its D3Calculator can load this library in place of pair_d3.so.

@@ -1,9 +1,9 @@
 // Host side of the D3 dispersion C ABI (include/sevenn_b200.h, "D3" section): parameters, cell list, the set-up of
 // one structure (host arrays) or of a batch (device arrays, s7b_d3_set_system_batch), stage launches, per-structure
-// results, the Hessian-vector product (s7b_d3_hvp_strain), the heat flux (s7b_d3_heat_flux), the per-atom centroid
-// virial (s7b_d3_centroid_virial) and the reference-named entry points (pair_init ... pair_fin) that
-// sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh, d3_hvp_kernels.cuh, d3_flux_kernels.cuh,
-// d3_centroid_kernels.cuh.
+// results, the Hessian-vector product (s7b_d3_hvp_strain), the heat flux (s7b_d3_heat_flux, or by range passes), the
+// per-atom centroid virial (s7b_d3_centroid_virial, or by range passes) and the reference-named entry points
+// (pair_init ... pair_fin) that sevenn/calculator.py:430-483 binds with ctypes.  Kernels: d3_kernels.cuh,
+// d3_hvp_kernels.cuh, d3_flux_kernels.cuh, d3_centroid_kernels.cuh.
 #include <dlfcn.h>
 
 #include <algorithm>
@@ -61,9 +61,12 @@ struct S7bD3 {
   // the current system; grids / aptr / lrows / nloc are swapped in from their st_ scratch once the checks have passed
   D3Buf grids, aptr, lrows, nloc, bin_off, rtab, idx_sorted, bin_start;
   D3Buf xs, ts, ss, bin_of, W, dW, logD, near_, cn, dc6i, force, eatom, spair, schain, energy, sigma, out_force;
-  // stages run in sequence over all atoms [0, n) since the current system and tables were set (0..3): the
-  // Hessian-vector product reads cn, W, dW and dc6i of all atoms and needs 3
-  int stages_done = 0;
+  // the forward: stages 1..fw_stage run in order over one atom range [fw_lo, fw_hi) since the current system, tables
+  // and damping were set (fw_stage 0..3).  The Hessian-vector product and the one-shot flux and centroid virial read
+  // cn, W, dW and dc6i of all atoms and need 3 over [0, n); the range passes need 3 over a range containing theirs
+  int fw_stage = 0, fw_lo = 0, fw_hi = 0;
+  // the range passes run since the last forward stage: 0 none, 1 pass 1 over [lo, hi), 2 then pass 2 inside it
+  int fx_pass = 0, fx_lo = 0, fx_hi = 0, ct_pass = 0, ct_lo = 0, ct_hi = 0;
   // Hessian-vector product scratch, allocated on its first call
   D3Buf hv_v, hv_dcn, hv_dWt, hv_dW1t, hv_ddc, hv_force, hv_spair, hv_schain, hv_sigma, hv_energy, hv_oute, hv_dvir;
   // heat-flux scratch, allocated on its first call
@@ -79,6 +82,8 @@ struct S7bD3 {
   int ref_pbc[3] = {1, 1, 1}, ref_ntypes = 0;
   std::string ref_damp = "damp_bj", ref_func = "pbe";
 };
+
+static bool d3_full_forward(const S7bD3* d) { return d->fw_stage == 3 && d->fw_lo == 0 && d->fw_hi == d->n; }
 
 static D3Atoms d3_atoms(const S7bD3* d) {
   D3Atoms A;
@@ -162,7 +167,7 @@ int s7b_d3_set_params(S7bD3* d, int32_t ntypes, const double* rcov, const double
   if (ntypes < 1 || ntypes > kD3MaxTypes) return d3_fail("D3: 1.." + std::to_string(kD3MaxTypes) + " atom types are supported");
   if (d3_upload_tables(d->P, ntypes, rcov, r2r4, r0ab, c6ref, cnref, mxc, d->r0ab, d->c6ref, d->cnref, d->mxc)) return 1;
   d->have_params = true;
-  d->stages_done = 0;
+  d->fw_stage = d->fx_pass = d->ct_pass = 0;
   return 0;
 }
 
@@ -172,7 +177,7 @@ int s7b_d3_set_element_tables(S7bD3* d, const double* rcov, const double* r2r4, 
   if (d3_upload_tables(d->Pe, kD3Elements, rcov, r2r4, r0ab, c6ref, cnref, mxc, d->el_r0ab, d->el_c6ref, d->el_cnref, d->el_mxc))
     return 1;
   d->have_elements = true;
-  d->stages_done = 0;
+  d->fw_stage = d->fx_pass = d->ct_pass = 0;
   return 0;
 }
 
@@ -189,7 +194,7 @@ int s7b_d3_set_damping(S7bD3* d, int32_t damping, double s6, double s8, double a
     P->cnthr = (double)(float)cn_cutoff_au2;
   }
   d->have_damping = true;
-  d->stages_done = 0;
+  d->fw_stage = d->fx_pass = d->ct_pass = 0;
   return 0;
 }
 
@@ -283,7 +288,7 @@ static int d3_setup(S7bD3* d, int B, const int32_t* atom_ptr, const std::vector<
   std::swap(d->lrows, d->st_lrows);
   std::swap(d->nloc, d->st_nloc);
   d->have_system = false;
-  d->stages_done = 0;
+  d->fw_stage = d->fx_pass = d->ct_pass = 0;
   rc = 0;
   rc |= d->bin_off.ensure((Bs + 1) * 4); rc |= d->rtab.ensure(Bs * 24); rc |= d->idx_sorted.ensure(N * 4);
   rc |= d->bin_start.ensure(((size_t)nbins + 1) * 4);
@@ -400,14 +405,17 @@ int s7b_d3_run_stage(S7bD3* d, int32_t stage, int32_t i_begin, int32_t i_end, vo
     return d3_fail("D3: unknown stage");
   }
   S7B_CUDA_CHECK(cudaGetLastError());
-  d->stages_done = (i_begin == 0 && i_end == n && stage <= d->stages_done + 1) ? stage : 0;
+  if (stage == 1) { d->fw_lo = i_begin; d->fw_hi = i_end; }
+  d->fw_stage = (stage == 1 || (stage <= d->fw_stage + 1 && i_begin == d->fw_lo && i_end == d->fw_hi)) ? stage : 0;
+  d->fx_pass = d->ct_pass = 0;
   return 0;
 }
 
 // device buffers, bin-sorted atom order: "cn" double[n], "dc6i" double[n], "force" double[n,3] (hartree/bohr),
 // "energy" double[B] (hartree), "sigma" double[B,6] (hartree; xx,yy,zz,xy,xz,yz), "order" int[n] (sorted -> caller index),
 // "type" int[n] (type word: after a batched set-up Z - 1 | local type << 8, else the type index), "eatom" double[n]
-// (hartree, the atomic energies of the pair pass)
+// (hartree, the atomic energies of the pair pass); the records the range passes exchange: "ct_nb" float[n,4],
+// "fx_nb" float[n,8], "ct_out" double[n,9] (eV), "fx_out" double[n,6] (null before the first pass of their kind)
 void* s7b_d3_buffer(S7bD3* d, const char* name, size_t* numel) {
   if (!d || !name) return nullptr;
   const std::string nm(name);
@@ -421,6 +429,10 @@ void* s7b_d3_buffer(S7bD3* d, const char* name, size_t* numel) {
   else if (nm == "order") { p = d->idx_sorted.p; n = d->n; }
   else if (nm == "type") { p = d->ts.p; n = d->n; }
   else if (nm == "eatom") { p = d->eatom.p; n = d->n; }
+  else if (nm == "ct_nb") { p = d->ct_nb.p; n = (size_t)d->n * 4; }
+  else if (nm == "fx_nb") { p = d->fx_nb.p; n = (size_t)d->n * 8; }
+  else if (nm == "ct_out") { p = d->ct_out.p; n = (size_t)d->n * 9; }
+  else if (nm == "fx_out") { p = d->fx_out.p; n = (size_t)d->n * 6; }
   if (numel) *numel = n;
   return p;
 }
@@ -469,7 +481,7 @@ int s7b_d3_system_results(S7bD3* d, double* d_energy, double* d_forces, double* 
 // tangent passes and the forward's own sums and results kernels on scratch; no forward buffer is written.
 int s7b_d3_hvp_strain(S7bD3* d, const double* d_v, const double* d_strain, double* d_out, double* d_dvirial, void* stream) {
   if (!d || !d->have_system) return d3_fail("D3: no system set");
-  if (d->stages_done < 3)
+  if (!d3_full_forward(d))
     return d3_fail("D3: the Hessian-vector product needs stages 1, 2 and 3 run over all atoms [0, n) of the current "
                    "system first");
   const int n = d->n, B = d->B;
@@ -526,12 +538,128 @@ int s7b_d3_hvp_strain(S7bD3* d, const double* d_v, const double* d_strain, doubl
   return 0;
 }
 
+}  // extern "C"
+
+// ---- heat flux and centroid virial: two passes each, over an atom range of the bin-sorted order ---------------------
+// Each pass is one warp per atom with no atomics and a fixed order, and reads of its centre the per-atom values a range
+// forward leaves valid for its range (eatom, spair, dc6i) and its own pass-1 row, and of a neighbour only the packed
+// float record of pass 1 (fx_nb, ct_nb) and what stage 2 computed for all atoms.  So the passes of several ranges,
+// with the records gathered between them, write each row bit for bit as one pass over [0, n) does.
+
+// refusals shared by the range passes; pass 2 also needs pass 1 of its kind (state 1 or 2) over a range containing its
+static int d3_pass_check(const S7bD3* d, int pass, int i_begin, int i_end, int state, int lo, int hi, const char* what) {
+  if (!d || !d->have_system) return d3_fail("D3: no system set");
+  if (pass != 1 && pass != 2) return d3_fail(std::string("D3: the ") + what + " has passes 1 and 2");
+  if (d->fw_stage < 3)
+    return d3_fail(std::string("D3: the ") + what + " pass needs stages 1, 2 and 3 run in order over one atom range "
+                   "since the last set-up, table or damping change");
+  if (i_begin < d->fw_lo || i_end > d->fw_hi || i_begin > i_end)
+    return d3_fail(std::string("D3: the ") + what + " pass range [" + std::to_string(i_begin) + ", " +
+                   std::to_string(i_end) + ") is not inside the forward's range [" + std::to_string(d->fw_lo) + ", " +
+                   std::to_string(d->fw_hi) + ")");
+  if (pass == 2 && (state < 1 || i_begin < lo || i_end > hi))
+    return d3_fail(std::string("D3: the ") + what + " pass 2 needs pass 1 over a range containing its own since the "
+                   "last forward stage");
+  return 0;
+}
+
+static int d3_flux_scratch(S7bD3* d) {
+  const size_t N = (size_t)d->n, Bs = (size_t)d->B;
+  int rc = 0;
+  rc |= d->fx_v.ensure(N * 24); rc |= d->fx_cn4.ensure(N * 32); rc |= d->fx_nb.ensure(N * 32); rc |= d->fx_out.ensure(N * 48);
+  rc |= d->fx_energy.ensure(Bs * 8); rc |= d->fx_sums.ensure(Bs * 48);
+  return rc ? d3_fail("cudaMalloc failed for the D3 heat flux") : 0;
+}
+
+static int d3_centroid_scratch(S7bD3* d) {
+  const size_t N = (size_t)d->n;
+  int rc = 0;
+  rc |= d->ct_beta.ensure(N * 24); rc |= d->ct_nb.ensure(N * 16); rc |= d->ct_out.ensure(N * 72);
+  return rc ? d3_fail("cudaMalloc failed for the D3 centroid virial") : 0;
+}
+
+static D3Flux d3_flux_args(const S7bD3* d) {
+  D3Flux X;
+  X.v = d->fx_v.as<double>();
+  X.eatom = d->eatom.as<double>();
+  X.cn4 = d->fx_cn4.as<double>();
+  X.nb = d->fx_nb.as<float4>();
+  X.out = d->fx_out.as<double>();
+  return X;
+}
+
+static D3Centroid d3_centroid_args(const S7bD3* d) {
+  D3Centroid C;
+  C.beta = d->ct_beta.as<double>();
+  C.nb = d->ct_nb.as<float4>();
+  C.spair = d->spair.as<double>();
+  C.out = d->ct_out.as<double>();
+  return C;
+}
+
+// flux pass 1: the velocities of all atoms to the sorted order in bohr, then d3_flux_cn_kernel over the range;
+// pass 2: d3_flux_pair_kernel over the range.  Scratch allocated, no checks.
+static int d3_flux_launch(S7bD3* d, int pass, const double* d_v, int i_begin, int i_end, cudaStream_t st) {
+  const int n = d->n, cnt = i_end - i_begin;
+  const int grd = (cnt + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
+  const bool bt = d->batched;
+  const D3Params& P = bt ? d->Pe : d->P;
+  const D3Atoms A = d3_atoms(d);
+  const D3Flux X = d3_flux_args(d);
+  if (pass == 1) {
+    if (n > 0) d3_hvp_gather_kernel<<<(3 * n + 255) / 256, 256, 0, st>>>(n, d->idx_sorted.as<int>(), d_v, d->fx_v.as<double>());
+    if (cnt > 0) {
+      if (bt) d3_flux_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, i_begin, i_end, X);
+      else d3_flux_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, i_begin, i_end, X);
+    }
+  } else if (cnt > 0) {
+    if (bt) d3_flux_pair_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, i_begin, i_end, X);
+    else d3_flux_pair_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, i_begin, i_end, X);
+  }
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// per structure over all n rows of fx_out: R in the sums' first three slots, eatom v in the last three (the energy sum
+// goes to scratch), then J_pot and sum U v in eV A x (the unit of v)
+static int d3_flux_sums_launch(S7bD3* d, double* d_jpot, double* d_ju, cudaStream_t st) {
+  const int B = d->B;
+  d3_system_sums_kernel<<<B, kD3SumBlock, 0, st>>>(d->aptr.as<int>(), 0, d->n, d->eatom.as<double>(), d->fx_out.as<double>(),
+                                                   d->fx_energy.as<double>(), d->fx_sums.as<double>());
+  d3_flux_results_kernel<<<(3 * B + 255) / 256, 256, 0, st>>>(B, d->fx_sums.as<double>(), d_jpot, d_ju);
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// centroid pass 1: d3_centroid_moment_kernel over the range; pass 2: d3_centroid_cn_kernel over the range (ct_out rows
+// in eV, sorted order).  Scratch allocated, no checks.
+static int d3_centroid_launch(S7bD3* d, int pass, int i_begin, int i_end, cudaStream_t st) {
+  const int cnt = i_end - i_begin;
+  if (cnt == 0) return 0;
+  const int grd = (cnt + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
+  const bool bt = d->batched;
+  const D3Params& P = bt ? d->Pe : d->P;
+  const D3Atoms A = d3_atoms(d);
+  const D3Centroid C = d3_centroid_args(d);
+  if (pass == 1) {
+    if (bt) d3_centroid_moment_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, i_begin, i_end, C);
+    else d3_centroid_moment_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, i_begin, i_end, C);
+  } else {
+    if (bt) d3_centroid_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, i_begin, i_end, C);
+    else d3_centroid_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, i_begin, i_end, C);
+  }
+  S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" {
+
 // Potential part of the heat flux of D3's atomic energies, J_pot = sum_j sum_i (r_j - r_i) (dU_j/dr_i . v_i) per
-// structure, and sum_j U_j v_j, on the current system with its forward (stages 1-3 over [0, n)) held: two passes on
-// scratch (d3_flux_kernels.cuh), then the forward's own sums kernel; no forward buffer is written.
+// structure, and sum_j U_j v_j, on the current system with its forward (stages 1-3 over [0, n)) held: the two passes
+// over [0, n) on scratch (d3_flux_kernels.cuh), then the sums; no forward buffer is written.
 int s7b_d3_heat_flux(S7bD3* d, const double* d_v, double* d_jpot, double* d_ju, void* stream) {
   if (!d || !d->have_system) return d3_fail("D3: no system set");
-  if (d->stages_done < 3)
+  if (!d3_full_forward(d))
     return d3_fail("D3: the heat flux needs stages 1, 2 and 3 run over all atoms [0, n) of the current system first");
   const int n = d->n, B = d->B;
   if (!d_jpot || (n > 0 && !d_v)) return d3_fail("null argument");
@@ -541,65 +669,61 @@ int s7b_d3_heat_flux(S7bD3* d, const double* d_v, double* d_jpot, double* d_ju, 
     if (d_ju) S7B_CUDA_CHECK(cudaMemsetAsync(d_ju, 0, (size_t)B * 24, st));
     return 0;
   }
-  const size_t N = (size_t)n, Bs = (size_t)B;
-  int rc = 0;
-  rc |= d->fx_v.ensure(N * 24); rc |= d->fx_cn4.ensure(N * 32); rc |= d->fx_nb.ensure(N * 32); rc |= d->fx_out.ensure(N * 48);
-  rc |= d->fx_energy.ensure(Bs * 8); rc |= d->fx_sums.ensure(Bs * 48);
-  if (rc) return d3_fail("cudaMalloc failed for the D3 heat flux");
-  const bool bt = d->batched;
-  const D3Params& P = bt ? d->Pe : d->P;
-  const D3Atoms A = d3_atoms(d);
-  D3Flux X;
-  X.v = d->fx_v.as<double>();
-  X.eatom = d->eatom.as<double>();
-  X.cn4 = d->fx_cn4.as<double>();
-  X.nb = d->fx_nb.as<float4>();
-  X.out = d->fx_out.as<double>();
-  const int grd = (n + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
-  d3_hvp_gather_kernel<<<(3 * n + 255) / 256, 256, 0, st>>>(n, d->idx_sorted.as<int>(), d_v, d->fx_v.as<double>());
-  if (bt) d3_flux_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, X);
-  else d3_flux_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, X);
-  if (bt) d3_flux_pair_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, X);
-  else d3_flux_pair_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, X);
-  // per structure: R in the sums' first three slots, eatom v in the last three (the energy sum goes to scratch)
-  d3_system_sums_kernel<<<B, kD3SumBlock, 0, st>>>(d->aptr.as<int>(), 0, n, X.eatom, X.out, d->fx_energy.as<double>(),
-                                                   d->fx_sums.as<double>());
-  d3_flux_results_kernel<<<(3 * B + 255) / 256, 256, 0, st>>>(B, d->fx_sums.as<double>(), d_jpot, d_ju);
-  S7B_CUDA_CHECK(cudaGetLastError());
+  if (d3_flux_scratch(d) || d3_flux_launch(d, 1, d_v, 0, n, st) || d3_flux_launch(d, 2, nullptr, 0, n, st)) return 1;
+  d->fx_pass = 2; d->fx_lo = 0; d->fx_hi = n;
+  return d3_flux_sums_launch(d, d_jpot, d_ju, st);
+}
+
+// One pass of the heat flux over [i_begin, i_end) of a range forward: see the header
+int s7b_d3_heat_flux_pass(S7bD3* d, int32_t pass, const double* d_v, int32_t i_begin, int32_t i_end, void* stream) {
+  if (d3_pass_check(d, pass, i_begin, i_end, d ? d->fx_pass : 0, d ? d->fx_lo : 0, d ? d->fx_hi : 0, "heat flux")) return 1;
+  if (pass == 1 && d->n > 0 && !d_v) return d3_fail("null argument");
+  if (d3_flux_scratch(d) || d3_flux_launch(d, pass, d_v, i_begin, i_end, reinterpret_cast<cudaStream_t>(stream))) return 1;
+  if (pass == 1) { d->fx_pass = 1; d->fx_lo = i_begin; d->fx_hi = i_end; }
+  else d->fx_pass = 2;
   return 0;
 }
 
+int s7b_d3_heat_flux_sums(S7bD3* d, double* d_jpot, double* d_ju, void* stream) {
+  if (!d || !d->have_system) return d3_fail("D3: no system set");
+  if (d->fx_pass < 2) return d3_fail("D3: the heat flux sums need flux pass 2 since the last forward stage");
+  if (!d_jpot) return d3_fail("null argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (d->n == 0) {
+    S7B_CUDA_CHECK(cudaMemsetAsync(d_jpot, 0, (size_t)d->B * 24, st));
+    if (d_ju) S7B_CUDA_CHECK(cudaMemsetAsync(d_ju, 0, (size_t)d->B * 24, st));
+    return 0;
+  }
+  return d3_flux_sums_launch(d, d_jpot, d_ju, st);
+}
+
 // Per-atom centroid virial of D3's atomic energies, Wc_i = sum_j sum_i' (r_j - r_i') (x) dU_j/dr_i' [n,9] (eV,
-// caller's atom order), on the current system with its forward (stages 1-3 over [0, n)) held: two passes on scratch
-// (d3_centroid_kernels.cuh) that read the forward's spair rows, then the forward's unsort; no forward buffer is written.
+// caller's atom order), on the current system with its forward (stages 1-3 over [0, n)) held: the two passes over
+// [0, n) on scratch (d3_centroid_kernels.cuh) that read the forward's spair rows, then the forward's unsort; no forward
+// buffer is written.
 int s7b_d3_centroid_virial(S7bD3* d, double* d_out, void* stream) {
   if (!d || !d->have_system) return d3_fail("D3: no system set");
-  if (d->stages_done < 3)
+  if (!d3_full_forward(d))
     return d3_fail("D3: the centroid virial needs stages 1, 2 and 3 run over all atoms [0, n) of the current system "
                    "first");
   const int n = d->n;
   if (n == 0) return 0;
   if (!d_out) return d3_fail("null argument");
-  const size_t N = (size_t)n;
-  int rc = 0;
-  rc |= d->ct_beta.ensure(N * 24); rc |= d->ct_nb.ensure(N * 16); rc |= d->ct_out.ensure(N * 72);
-  if (rc) return d3_fail("cudaMalloc failed for the D3 centroid virial");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const bool bt = d->batched;
-  const D3Params& P = bt ? d->Pe : d->P;
-  const D3Atoms A = d3_atoms(d);
-  D3Centroid C;
-  C.beta = d->ct_beta.as<double>();
-  C.nb = d->ct_nb.as<float4>();
-  C.spair = d->spair.as<double>();
-  C.out = d->ct_out.as<double>();
-  const int grd = (n + kD3WarpsPerBlock - 1) / kD3WarpsPerBlock, blk = 32 * kD3WarpsPerBlock;
-  if (bt) d3_centroid_moment_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, C);
-  else d3_centroid_moment_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->dW.as<float>(), d->R1_vdw, n, C);
-  if (bt) d3_centroid_cn_kernel<true><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, C);
-  else d3_centroid_cn_kernel<false><<<grd, blk, 0, st>>>(d->grid1, A, P, d->R1_cn, n, C);
-  d3_unsort_kernel<<<(n * 9 + 255) / 256, 256, 0, st>>>(n, 9, d->idx_sorted.as<int>(), C.out, 1.0, d_out);
+  if (d3_centroid_scratch(d) || d3_centroid_launch(d, 1, 0, n, st) || d3_centroid_launch(d, 2, 0, n, st)) return 1;
+  d->ct_pass = 2; d->ct_lo = 0; d->ct_hi = n;
+  d3_unsort_kernel<<<(n * 9 + 255) / 256, 256, 0, st>>>(n, 9, d->idx_sorted.as<int>(), d->ct_out.as<double>(), 1.0, d_out);
   S7B_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// One pass of the centroid virial over [i_begin, i_end) of a range forward: see the header
+int s7b_d3_centroid_pass(S7bD3* d, int32_t pass, int32_t i_begin, int32_t i_end, void* stream) {
+  if (d3_pass_check(d, pass, i_begin, i_end, d ? d->ct_pass : 0, d ? d->ct_lo : 0, d ? d->ct_hi : 0, "centroid virial"))
+    return 1;
+  if (d3_centroid_scratch(d) || d3_centroid_launch(d, pass, i_begin, i_end, reinterpret_cast<cudaStream_t>(stream))) return 1;
+  if (pass == 1) { d->ct_pass = 1; d->ct_lo = i_begin; d->ct_hi = i_end; }
+  else d->ct_pass = 2;
   return 0;
 }
 

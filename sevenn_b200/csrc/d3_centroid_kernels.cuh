@@ -1,5 +1,5 @@
-// Kernels of the D3 per-atom centroid virial (d3.cu s7b_d3_centroid_virial, DESIGN.md §8.6), on the forward's cell
-// list and sweep, with the forward's per-atom factors held.
+// Kernels of the D3 per-atom centroid virial (d3.cu s7b_d3_centroid_virial, s7b_d3_centroid_pass; DESIGN.md §8.6),
+// on the forward's cell list and sweep, with the forward's per-atom factors held.
 //
 // U_j = -1/2 sum_{k,tau} C6_jk(CN_j, CN_k) g(r_jk), self images included, as d3_pair_kernel's eatom, and
 // Wc_i[a][b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b over atom i and its images i'.  With vec = r_k + tau - r_i,
@@ -32,11 +32,11 @@ struct D3Centroid {           // bin-sorted atom order
 template <bool kBatch>
 __global__ void __launch_bounds__(32 * kD3WarpsPerBlock, kD3CentroidMomentBlocks)
 d3_centroid_moment_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, const float* __restrict__ dW, int3 R1,
-                          int n, D3Centroid C) {
+                          int i_begin, int i_end, D3Centroid C) {
   __shared__ float sdV[kD3WarpsPerBlock][kD3MaxTypes][5];       // dV_i[t][b] over local types t, as d3_pair_kernel
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * kD3WarpsPerBlock + wib;
-  if (i >= n) return;
+  const int i = i_begin + blockIdx.x * kD3WarpsPerBlock + wib;
+  if (i >= i_end) return;
   const int ti = d3_row<kBatch>(A.type[i]), sb = kBatch ? A.sys[i] : 0;
   const int nloc = kBatch ? A.nloc[sb] : P.nrows;
   for (int q = lane; q < nloc * 5; q += 32) {
@@ -79,10 +79,11 @@ d3_centroid_moment_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, co
 // end in fp64.
 template <bool kBatch>
 __global__ void __launch_bounds__(32 * kD3WarpsPerBlock, kD3CentroidCnBlocks)
-d3_centroid_cn_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, int3 R1, int n, D3Centroid C) {
-  const int i = blockIdx.x * kD3WarpsPerBlock + (threadIdx.x >> 5);
+d3_centroid_cn_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, int3 R1, int i_begin, int i_end,
+                      D3Centroid C) {
+  const int i = i_begin + blockIdx.x * kD3WarpsPerBlock + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (i >= n) return;
+  if (i >= i_end) return;
   const float rci = P.rcov[d3_row<kBatch>(A.type[i])];
   const float cn2 = (float)P.cnthr;
   double w[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, su[3] = {0, 0, 0};

@@ -1,5 +1,6 @@
-// Kernels of the D3 heat flux (d3.cu s7b_d3_heat_flux): the potential part of the energy-barycentre flux of D3's
-// atomic energies (DESIGN.md §8.4), on the forward's cell list and sweep, with the forward's per-atom factors held.
+// Kernels of the D3 heat flux (d3.cu s7b_d3_heat_flux, s7b_d3_heat_flux_pass): the potential part of the
+// energy-barycentre flux of D3's atomic energies (DESIGN.md §8.4), on the forward's cell list and sweep, with the
+// forward's per-atom factors held.
 //
 // U_j = -1/2 sum_{k,tau} C6_jk(CN_j, CN_k) g(r_jk), self images included, as d3_pair_kernel's eatom.  For velocities v
 // and the moment M_j[X] = sum_i (r_j - r_i) (dX/dr_i . v_i) (i over every atom and image, an image moving with its
@@ -32,10 +33,10 @@ struct D3Flux {               // bin-sorted atom order
 // ---- pass 1: dCN_j and the moment P_j of CN_j ---------------------------------------------------------------------
 template <bool kBatch>
 __global__ void __launch_bounds__(32 * kD3WarpsPerBlock, kD3FluxCnBlocks)
-d3_flux_cn_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, int3 R1, int n, D3Flux X) {
-  const int i = blockIdx.x * kD3WarpsPerBlock + (threadIdx.x >> 5);
+d3_flux_cn_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, int3 R1, int i_begin, int i_end, D3Flux X) {
+  const int i = i_begin + blockIdx.x * kD3WarpsPerBlock + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (i >= n) return;
+  if (i >= i_end) return;
   const float rci = P.rcov[d3_row<kBatch>(A.type[i])];
   const float vi[3] = {(float)X.v[3 * i], (float)X.v[3 * i + 1], (float)X.v[3 * i + 2]};
   double dcn = 0.0, px = 0.0, py = 0.0, pz = 0.0;
@@ -63,12 +64,12 @@ d3_flux_cn_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, int3 R1, i
 // ---- pass 2: R_j = M_j[U_j] and eatom_j v_j -----------------------------------------------------------------------
 template <bool kBatch>
 __global__ void __launch_bounds__(32 * kD3WarpsPerBlock, kD3FluxPairBlocks)
-d3_flux_pair_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, const float* __restrict__ dW, int3 R1, int n,
-                    D3Flux X) {
+d3_flux_pair_kernel(const NLGrid g1, const D3Atoms A, const D3Params P, const float* __restrict__ dW, int3 R1,
+                    int i_begin, int i_end, D3Flux X) {
   __shared__ float sV[kD3WarpsPerBlock][kD3MaxTypes][5];        // V_i[t][b] over local types t, as d3_pair_kernel
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * kD3WarpsPerBlock + wib;
-  if (i >= n) return;
+  const int i = i_begin + blockIdx.x * kD3WarpsPerBlock + wib;
+  if (i >= i_end) return;
   const int ti = d3_row<kBatch>(A.type[i]), sb = kBatch ? A.sys[i] : 0;
   const int nloc = kBatch ? A.nloc[sb] : P.nrows;
   for (int q = lane; q < nloc * 5; q += 32) {

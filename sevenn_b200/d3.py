@@ -201,36 +201,94 @@ class D3Engine:
         return out
 
 
+def _rank_range(n, world, rank):
+    """(chunk, lo, hi): rank's contiguous slice [lo, hi) of n bin-sorted atoms cut into `world` chunks (the last may
+    be short or empty)"""
+    chunk = (n + world - 1) // world
+    return chunk, min(rank * chunk, n), min((rank + 1) * chunk, n)
+
+
+def _gather_range(engine, name, width, lo, hi, chunk, group, dtype='f8'):
+    """all-gather the rows [lo, hi) of every rank into the engine's device buffer `name` ([n] or [n, width] of
+    `dtype`), in place: each rank's slice is padded to `chunk` rows for the collective"""
+    import torch
+    import torch.distributed as dist
+    world, n = dist.get_world_size(group), engine.n
+    buf = engine.buffer(name, dtype=dtype, shape=(n, width) if width > 1 else (n,))
+    padded = torch.zeros((world * chunk,) + tuple(buf.shape[1:]), dtype=buf.dtype, device=buf.device)
+    mine = torch.zeros((chunk,) + tuple(buf.shape[1:]), dtype=buf.dtype, device=buf.device)
+    mine[:hi - lo] = buf[lo:hi]
+    dist.all_gather_into_tensor(padded, mine, group=group)
+    buf.copy_(padded[:n])
+
+
 def distributed_d3(engine: D3Engine, numbers, positions, cell, pbc=(True, True, True), group=None):
     """The same system on every rank (positions replicated: the 50 A interaction range is of the order of the
     box), each rank evaluating a contiguous slice of the bin-sorted atoms; ``cn`` and ``dc6i`` are
     all-gathered between the stages (NCCL), energy / virial all-reduced, forces all-gathered.
-    Returns (energy, forces [n,3], sigma6) on every rank."""
-    import torch
+    Returns (energy, forces [n,3], sigma6) on every rank.  The engine keeps the range forward for
+    ``distributed_d3_centroid_virials`` and ``distributed_d3_heat_flux``."""
     import torch.distributed as dist
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     engine.set_system(numbers, positions, cell, pbc)
-    n = engine.n
-    chunk = (n + world - 1) // world
-    lo, hi = min(rank * chunk, n), min((rank + 1) * chunk, n)
-
-    def gather(name, width):
-        buf = engine.buffer(name, shape=(n, width) if width > 1 else (n,))
-        padded = torch.zeros((world * chunk,) + tuple(buf.shape[1:]), dtype=buf.dtype, device=buf.device)
-        mine = torch.zeros((chunk,) + tuple(buf.shape[1:]), dtype=buf.dtype, device=buf.device)
-        mine[:hi - lo] = buf[lo:hi]
-        dist.all_gather_into_tensor(padded, mine, group=group)
-        buf.copy_(padded[:n])
-
+    chunk, lo, hi = _rank_range(engine.n, world, rank)
     engine.run_stage(1, lo, hi)
-    gather('cn', 1)
+    _gather_range(engine, 'cn', 1, lo, hi, chunk, group)
     engine.run_stage(2, lo, hi)
-    gather('dc6i', 1)
+    _gather_range(engine, 'dc6i', 1, lo, hi, chunk, group)
     engine.run_stage(3, lo, hi)
-    gather('force', 3)
+    _gather_range(engine, 'force', 3, lo, hi, chunk, group)
     for name in ('energy', 'sigma'):
         dist.all_reduce(engine.buffer(name), group=group)
     return engine.results()
+
+
+def distributed_d3_centroid_virials(engine: D3Engine, group=None):
+    """``D3Engine.centroid_virial`` after ``distributed_d3`` on the same group (C ABI ``s7b_d3_centroid_pass``,
+    DESIGN.md §8.8): each rank runs both passes on its slice of the bin-sorted atoms, with the packed neighbour
+    record (16 B per atom) all-gathered between them and the rows (72 B per atom) after them.  Returns [n, 3, 3]
+    float64 device tensor in eV, caller's atom order, the same on every rank and bit for bit that of the one-GPU
+    call.  Collective."""
+    import torch
+    import torch.distributed as dist
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    n = engine.n
+    chunk, lo, hi = _rank_range(n, world, rank)
+    with torch.cuda.device(engine.device):
+        check(engine.lib.s7b_d3_centroid_pass(engine._h, 1, lo, hi, engine._stream()))
+        _gather_range(engine, 'ct_nb', 4, lo, hi, chunk, group, dtype='f4')
+        check(engine.lib.s7b_d3_centroid_pass(engine._h, 2, lo, hi, engine._stream()))
+        _gather_range(engine, 'ct_out', 9, lo, hi, chunk, group)
+    out = torch.empty(n, 9, dtype=torch.float64, device=engine.device)
+    if n:
+        out[engine.buffer('order', dtype='i4').long()] = engine.buffer('ct_out', shape=(n, 9))
+    return out.reshape(n, 3, 3)
+
+
+def distributed_d3_heat_flux(engine: D3Engine, v, group=None):
+    """``D3Engine.heat_flux(v)`` after ``distributed_d3`` on the same group (C ABI ``s7b_d3_heat_flux_pass``,
+    DESIGN.md §8.8): each rank runs both passes on its slice of the bin-sorted atoms, with the packed neighbour
+    record (32 B per atom) all-gathered between them and the per-atom terms (48 B per atom) after them; every rank
+    then sums all n rows in the one-GPU order.  v [n, 3] every atom's velocity (Angstrom x any time unit, caller's
+    atom order), numpy or torch.  Returns (jpot, ju), [3] float64 device tensors in eV A x (the unit of v), the same
+    on every rank and bit for bit those of the one-GPU call.  Collective."""
+    import torch
+    import torch.distributed as dist
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    n = engine.n
+    v = torch.as_tensor(v).to(engine.device, torch.float64).contiguous()
+    if v.numel() != 3 * n or (v.dim() == 2 and v.shape[1] != 3) or v.dim() > 2:
+        raise ValueError(f'v has {tuple(v.shape)}, expected [{n}, 3] (atoms)')
+    chunk, lo, hi = _rank_range(n, world, rank)
+    jpot = torch.empty(1, 3, dtype=torch.float64, device=engine.device)
+    ju = torch.empty(1, 3, dtype=torch.float64, device=engine.device)
+    with torch.cuda.device(engine.device):
+        check(engine.lib.s7b_d3_heat_flux_pass(engine._h, 1, v.data_ptr(), lo, hi, engine._stream()))
+        _gather_range(engine, 'fx_nb', 8, lo, hi, chunk, group, dtype='f4')
+        check(engine.lib.s7b_d3_heat_flux_pass(engine._h, 2, None, lo, hi, engine._stream()))
+        _gather_range(engine, 'fx_out', 6, lo, hi, chunk, group)
+        check(engine.lib.s7b_d3_heat_flux_sums(engine._h, jpot.data_ptr(), ju.data_ptr(), engine._stream()))
+    return jpot[0], ju[0]
 
 
 def batch_inputs(torch, device, numbers, positions, cells, pbc, system_idx=None, atom_ptr=None, max_cutoff=None):

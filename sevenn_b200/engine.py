@@ -69,7 +69,8 @@ EXPORTS = [
     's7b_d3_set_element_tables', 's7b_d3_set_system_batch', 's7b_d3_system_results', 's7b_species_linear',
     's7b_engine_hvp', 's7b_engine_hvp_strain', 's7b_d3_hvp_strain', 's7b_engine_heat_flux',
     's7b_d3_heat_flux', 's7b_engine_centroid_virial', 's7b_engine_centroid_virial_host',
-    's7b_d3_centroid_virial', 's7b_engine_read_rows_f64_host',
+    's7b_d3_centroid_virial', 's7b_engine_read_rows_f64_host', 's7b_d3_centroid_pass', 's7b_d3_heat_flux_pass',
+    's7b_d3_heat_flux_sums',
 ]
 
 
@@ -126,6 +127,9 @@ def load_library() -> ctypes.CDLL:
     lib.s7b_engine_centroid_virial.argtypes = [vp, vp, vp]
     lib.s7b_engine_centroid_virial_host.argtypes = [vp, vp, vp]
     lib.s7b_d3_centroid_virial.argtypes = [vp, vp, vp]
+    lib.s7b_d3_centroid_pass.argtypes = [vp, i32, i32, i32, vp]
+    lib.s7b_d3_heat_flux_pass.argtypes = [vp, i32, vp, i32, i32, vp]
+    lib.s7b_d3_heat_flux_sums.argtypes = [vp, vp, vp, vp]
     lib.s7b_engine_buffer.argtypes = [vp, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(sz)]
     lib.s7b_engine_buffer.restype = vp
     lib.s7b_engine_compute_host.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]

@@ -32,7 +32,8 @@ between.  Here:
   (LAMMPS' ``newton on`` reverse communication, ``pair_e3gnn_parallel.cpp:461-480,681-687``);
 * after a step, ``centroid_virials()`` / ``heat_flux()`` run the engine's centroid-virial stages (DESIGN.md §8.7)
   eagerly: per layer one reverse exchange carries the ghost rows of all four adjoint channels, and the ghost rows of
-  the per-atom centroid virial travel once more at the end, added in fp64.
+  the per-atom centroid virial travel once more at the end, added in fp64.  With ``d3=`` they add the terms of a D3
+  forward that ``sevenn_b200.d3.distributed_d3`` shared over the same group (DESIGN.md §8.8).
 """
 from __future__ import annotations
 
@@ -545,15 +546,23 @@ class DistributedRunner:
                     virial=eng.buffer('virial', dtype='f8').clone(),
                     global_ids=self.part['global_ids'][:self.n_local])
 
-    # ---- Green-Kubo: per-atom centroid virial and heat flux (DESIGN.md §8.7) ------------------------------------
-    def centroid_virials(self):
+    # ---- Green-Kubo: per-atom centroid virial and heat flux (DESIGN.md §8.7, §8.8) ------------------------------
+    def _check_d3(self, d3):
+        if d3 is not None and d3.n != self.part['n_global']:
+            raise ValueError(f'd3 holds {d3.n} atoms, the runner\'s system {self.part["n_global"]}: pass the D3Engine '
+                             f'whose last forward was distributed_d3 of the whole system, in global-id order')
+
+    def centroid_virials(self, d3=None):
         """Per-atom centroid virial of this rank's atoms after ``compute()``: [n_local, 3, 3] float64 device tensor in eV,
         in ``results()`` order (``global_ids``).  Wc_i[a, b] = sum_j sum_i' (r_j - r_i')_a dU_j/dr_i',b over every
         atomic energy U_j of the whole system and every periodic image i' of atom i (``B200Engine.centroid_virial``
         of the whole system, DESIGN.md §8.5).  Runs the engine's CV stages eagerly (never in a CUDA graph): per layer one
         reverse exchange of the ghost rows of the four adjoint channels, then one of the ghost rows of Wc, added in
         fp64 in rank order.  Uploads the radial MLP of a table-mode engine on first use, as ``B200Engine.hvp``.
-        Collective: every rank calls it."""
+        ``d3``: a ``D3Engine`` whose last forward was ``sevenn_b200.d3.distributed_d3`` of the whole system, in
+        global-id order, on the same group; its rows (``distributed_d3_centroid_virials``) are added to the owned
+        atoms' in fp64.  Collective: every rank calls it."""
+        self._check_d3(d3)
         eng, T, n = self.engine, self.n_layers, self.n_nodes
         if hasattr(eng, '_upload_hvp_mlp'):
             with self.torch.cuda.device(self.device):
@@ -570,17 +579,27 @@ class DistributedRunner:
         eng.run_stage(STAGE_CV_END)
         wc = eng.buffer('centroid_virial', dtype='f8', shape=(n, 9))
         self.exchange.reverse_add_many([wc])
-        return wc[:self.n_local].reshape(self.n_local, 3, 3).clone()
+        out = wc[:self.n_local].reshape(self.n_local, 3, 3).clone()
+        if d3 is not None:
+            from . import d3 as d3mod
+            gids = self.torch.as_tensor(np.asarray(self.part['global_ids'][:self.n_local], dtype=np.int64))
+            rows = d3mod.distributed_d3_centroid_virials(d3, group=self.group)
+            out += rows[gids.to(rows.device)].to(out.device)
+        return out
 
-    def heat_flux(self, velocities, masses=None, convective: bool = True):
+    def heat_flux(self, velocities, masses=None, convective: bool = True, d3=None):
         """Heat flux of the whole system after ``compute()``, [3] float64 device tensor, the same on every rank
         (``sevenn_b200.heat_flux``'s definition): J_pot + J_conv, J_pot = sum_i Wc_i v_i over every rank's owned atoms
         (``centroid_virials``), J_conv = sum_i (U_i + m_i |v_i|^2 / 2) v_i.  velocities [n_global, 3] and masses
         [n_global] (needed when ``convective``) are indexed by global atom id, numpy or torch.  ``convective=False``
-        gives J_pot alone.  The per-rank sums are gathered and added in rank order.  Collective."""
+        gives J_pot alone.  The per-rank sums are gathered and added in rank order.  ``d3``: a ``D3Engine`` as in
+        ``centroid_virials``; D3's J_pot, plus its sum_j U_j v_j when ``convective``
+        (``distributed_d3_heat_flux``, already the whole system's on every rank), is added once to that total.
+        Collective."""
         torch = self.torch
         if convective and masses is None:
             raise ValueError('the convective flux needs the masses (or pass convective=False)')
+        self._check_d3(d3)
         gids = torch.as_tensor(np.asarray(self.part['global_ids'][:self.n_local], dtype=np.int64))
         host = lambda a: a.detach().cpu() if hasattr(a, 'detach') else torch.as_tensor(np.asarray(a))
         v = host(velocities).to(torch.float64).reshape(-1, 3)[gids].to(self.device)
@@ -597,7 +616,13 @@ class DistributedRunner:
         total = parts[0].clone()
         for p in parts[1:]:
             total += p
-        return total.to(self.device)
+        total = total.to(self.device)
+        if d3 is not None:
+            from . import d3 as d3mod
+            jpot, ju = d3mod.distributed_d3_heat_flux(d3, host(velocities).to(torch.float64).reshape(-1, 3),
+                                                      group=self.group)
+            total = total + (jpot + ju if convective else jpot).to(total.device)
+        return total
 
     # ---- end-to-end: host buffers in, host buffers out ---------------------------------------------
     def host_bytes(self):
